@@ -90,9 +90,14 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
   return ok != 0;
 }
 // Spin with a watchdog: a mis-programmed pipeline must trap (-> cudaErrorLaunchFailure on the
-// host, surfaced as RuntimeError) instead of hanging the GPU.  The spin loop lives out of line so that
-// the many call sites stay a single try_wait + branch (instruction-cache footprint of the hot loops).
-static __device__ __noinline__ void mbar_wait_slow(uint64_t* bar, uint32_t parity) {
+// host, surfaced as RuntimeError) instead of hanging the GPU.
+//
+// Rule: no function call may appear in a kernel that issues wgmma -- no __noinline__ helper, no printf, no assert.
+// ptxas cannot keep an asynchronous wgmma pipeline across a call, so it serializes EVERY wgmma of the kernel (warning
+// C7510: each MMA waits for the previous one to complete).  The watchdog is therefore fully inline and ends in __trap();
+// the diagnostic line is opt-in (-DYV6_WATCHDOG_PRINTF) for debugging builds only, as it brings the serialization back.  tests/test_sass_wgmma.py checks
+// the built library for calls and serialized MMAs.
+__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   uint64_t t0 = 0;
   uint32_t spins = 0;
   while (!mbar_try_wait(bar, parity)) {
@@ -101,14 +106,13 @@ static __device__ __noinline__ void mbar_wait_slow(uint64_t* bar, uint32_t parit
       asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(now));
       if (t0 == 0) t0 = now;
       else if (now - t0 > 4000000000ull) {  // 4 s
+#ifdef YV6_WATCHDOG_PRINTF
         if ((threadIdx.x & 31) == 0) printf("yv6: mbarrier wait timeout block %d warp %d\n", blockIdx.x, threadIdx.x >> 5);
+#endif
         __trap();
       }
     }
   }
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-  if (!mbar_try_wait(bar, parity)) mbar_wait_slow(bar, parity);
 }
 
 // ---- thread block clusters ----

@@ -275,6 +275,17 @@ __device__ __forceinline__ void epilogue_math(const ConvKParams& p, const float*
   }
 }
 
+// One K block of KSTEPS k16 MMAs, issued back to back as ONE commit group.  KSTEPS must be known at compile time: an MMA
+// under a runtime condition makes ptxas split the group and inject warpgroup.arrive around it (warning C7519).
+template <int BN, int KSTEPS>
+__device__ __forceinline__ void mma_kblock(float (&acc)[BN / 2], uint64_t ad, uint64_t bd, uint32_t scale_d) {
+  wgmma_fence();
+  Wgmma<BN, 0, 0>::mma(acc, ad, bd, scale_d);
+#pragma unroll
+  for (int k = 1; k < KSTEPS; ++k) Wgmma<BN, 0, 0>::mma(acc, ad + (uint64_t)(2 * k), bd + (uint64_t)(2 * k), 1u);
+  wgmma_commit();
+}
+
 // MODE: 0 = one TMA box per (tap, channel block); 1 / 3 = halo input tiles (stride 1 / stride-2 column-pair view), weights
 //       streamed through a ring; 2 / 4 = the same with the layer's weights resident in shared memory.  BN = the wgmma N and
 //       the width of the accumulator tile.  CP: CTA-pair variant (launched as clusters of two CTAs, see ConvKParams::cpair).
@@ -409,7 +420,8 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   } else if (warp >= 4) {
     // ================================ consumers ================================
     // Warpgroup wg (0 / 1) computes rows 64 wg .. 64 wg + 63 of every tile.  One wgmma group is kept in flight: after
-    // committing K block i the warpgroup waits for block i - 1 and only then releases that block's shared memory.
+    // committing K block i the warpgroup waits for block i - 1 and only then releases that block's shared memory.  Only the
+    // last group of a tile is waited for in full, before the epilogue.
     const int wg = (warp >> 2) - 1;
     const int ct = (int)threadIdx.x - 128;          // 0 .. 255
     const bool arrive_lane = ((warp & 3) == 0) && lane == 0;   // one arrival per warpgroup on the empty barriers
@@ -438,11 +450,14 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         const int pcs = p.npairs * p.cin_blocks, skip_cb = p.skip_cb, cin_blocks = p.cin_blocks, b_stages = p.b_stages;
         int slot = 0;
         uint32_t started = 0;
+        // Stages whose MMAs may still be in flight: the B stage of the last committed group and the A stage of the previous
+        // channel block.  Each is released once a later group has been committed and wgmma_wait<1> has returned, so the
+        // pipe never drains at a channel-block boundary; the one full wait per tile comes before the epilogue.
+        int prev_sb = -1, prev_sa = -1;
         for (int pc = 0; pc < pcs; ++pc) {
           mbar_wait(&a_full[sa], pha);
           const uint32_t a0 = a_base + (uint32_t)sa * halo_step + wg_off;
           const bool skip_s0 = (HG::SH == 2) && (pc % cin_blocks) < skip_cb;      // this channel block of the s = 0 taps is all zero
-          int prev_sb = -1;
 #pragma unroll
           for (int tap = 0; tap < HG::TAPS; ++tap) {
             if (HG::SH == 2 && (tap % HG::KW) == 0 && skip_s0) continue;
@@ -451,27 +466,29 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             if (!BRES || first) mbar_wait(&b_full[bs], BRES ? 0u : phb);
             const uint64_t ad = desc_a | (uint64_t)(a0 + (uint32_t)((tap / HG::KW) * HG::W + (tap % HG::KW)) * 8u);
             const uint64_t bd = desc_b | (uint64_t)(b_base + (uint32_t)bs * b_step);
-            wgmma_fence();
-            Wgmma<BN, 0, 0>::mma(acc, ad, bd, started);
-            Wgmma<BN, 0, 0>::mma(acc, ad + 2, bd + 2, 1u);
-            Wgmma<BN, 0, 0>::mma(acc, ad + 4, bd + 4, 1u);
-            Wgmma<BN, 0, 0>::mma(acc, ad + 6, bd + 6, 1u);
-            wgmma_commit();
+            mma_kblock<BN, 4>(acc, ad, bd, started);
             started = 1u;
-            if (!BRES) {
+            if (!BRES || prev_sa >= 0) {
               wgmma_wait<1>();
-              if (prev_sb >= 0 && arrive_lane) release_b(&b_empty[prev_sb]);
+              if (arrive_lane) {
+                if (!BRES && prev_sb >= 0) release_b(&b_empty[prev_sb]);
+                if (prev_sa >= 0) mbar_arrive(&a_empty[prev_sa]);
+              }
+              prev_sa = -1;
+            }
+            if (!BRES) {
               prev_sb = sb;
               if (++sb == b_stages) { sb = 0; phb ^= 1; }
             }
             ++slot;
           }
-          wgmma_wait<0>();
-          if (arrive_lane) {
-            if (!BRES && prev_sb >= 0) release_b(&b_empty[prev_sb]);
-            mbar_arrive(&a_empty[sa]);
-          }
+          prev_sa = sa;
           if (++sa == p.a_stages) { sa = 0; pha ^= 1; }
+        }
+        wgmma_wait<0>();
+        if (arrive_lane) {
+          if (!BRES && prev_sb >= 0) release_b(&b_empty[prev_sb]);
+          if (prev_sa >= 0) mbar_arrive(&a_empty[prev_sa]);
         }
       } else {
         const uint64_t desc = wgmma_desc(16u, (uint32_t)p.sbo_bytes, (uint32_t)p.layout_type);
@@ -482,14 +499,12 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           mbar_wait(&full[stage], phase);
           const uint64_t ad = desc | (uint64_t)(a_base + (uint32_t)stage * a_step + wg_off);
           const uint64_t bd = desc | (uint64_t)(b_base + (uint32_t)stage * b_step);
-          wgmma_fence();
-          Wgmma<BN, 0, 0>::mma(acc, ad, bd, (uint32_t)(kb != 0));
-          if (ksteps > 1) Wgmma<BN, 0, 0>::mma(acc, ad + 2, bd + 2, 1u);
-          if (ksteps > 2) {
-            Wgmma<BN, 0, 0>::mma(acc, ad + 4, bd + 4, 1u);
-            Wgmma<BN, 0, 0>::mma(acc, ad + 6, bd + 6, 1u);
+          const uint32_t scale_d = (uint32_t)(kb != 0);
+          switch (ksteps) {          // 16-, 32- or 64-channel K blocks
+            case 1: mma_kblock<BN, 1>(acc, ad, bd, scale_d); break;
+            case 2: mma_kblock<BN, 2>(acc, ad, bd, scale_d); break;
+            default: mma_kblock<BN, 4>(acc, ad, bd, scale_d); break;
           }
-          wgmma_commit();
           wgmma_wait<1>();
           if (prev >= 0 && arrive_lane) release_b(&empty[prev]);
           prev = stage;
