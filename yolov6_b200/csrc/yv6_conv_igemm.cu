@@ -16,8 +16,9 @@
 //     shared memory as `rows` consecutive K-major rows in the 128/64/32-byte swizzle that
 //     wgmma consumes directly -- no im2col buffer, no index math on the SMs.
 //   * B tile = [BN x KB] slice of the weights, one TMA load from a 3-D map (K, Cout, plane).
-//   * warpgroup 0 = TMA producer (one warp), warpgroups 1 and 2 = consumers: each issues
-//     wgmma m64nBNk16 for its 64 rows of the 128-row tile and keeps its accumulators in registers.
+//   * warpgroup 0 = TMA producer (one warp), warpgroups 1 and 2 = consumers in a ping-pong schedule: each owns
+//     every other tile of the CTA, issues wgmma m64nBNk16 for all 128 rows of it and keeps its accumulators in
+//     registers.  The two take turns on the tensor cores, so one's epilogue runs under the other's MMAs.
 //     The epilogue stages the fp32 tile in shared memory and writes it with coalesced 16-channel
 //     chunks (bias / activation / residual / dtype / bf16x3 planes / channel slices fused there).
 //   * persistent CTAs (grid = #SMs) over a static tile schedule; smem ring of `stages` K-blocks
@@ -82,7 +83,8 @@ struct HaloGeom {
 };
 constexpr int kMaxAStages = 6, kMaxBStages = 40;
 
-// fp32 staging tile of the epilogue: 128 rows x BN columns, rows padded by 4 floats (16-byte aligned, fewer bank conflicts)
+// fp32 staging tile of the epilogue: 128 rows x BN columns, rows padded by 4 floats (16-byte aligned, fewer bank conflicts);
+// each consumer warpgroup owns 64 of the rows and writes its tile out through them in two passes
 __host__ __device__ constexpr int stage_pitch(int bn) { return bn + 4; }
 __host__ __device__ constexpr int staging_bytes(int bn) { return kTileRows * stage_pitch(bn) * 4; }
 
@@ -104,9 +106,13 @@ __device__ __forceinline__ void tma_load_3d_mc(void* dst, const CUtensorMap* m, 
       "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "h"(mask)
       : "memory");
 }
-__device__ __forceinline__ void consumer_bar_sync() {  // the 256 threads of the two consumer warpgroups
-  asm volatile("bar.sync 1, 256;" ::: "memory");
+__device__ __forceinline__ void warpgroup_bar_sync(int wg) {  // the 128 threads of consumer warpgroup wg (named barrier 1 + wg)
+  asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
 }
+// warp-specialised register split: the producer warpgroup gives registers back, the two consumer warpgroups take them
+// (128 x 40 + 256 x 232 <= 64 K), so that a consumer can hold the fp32 accumulators of a whole 128 x BN tile
+__device__ __forceinline__ void producer_regs() { asm volatile("setmaxnreg.dec.sync.aligned.u32 40;"); }
+__device__ __forceinline__ void consumer_regs() { asm volatile("setmaxnreg.inc.sync.aligned.u32 232;"); }
 
 struct TileCoord {
   int w0, h0, i0, n0;
@@ -275,14 +281,18 @@ __device__ __forceinline__ void epilogue_math(const ConvKParams& p, const float*
   }
 }
 
-// One K block of KSTEPS k16 MMAs, issued back to back as ONE commit group.  KSTEPS must be known at compile time: an MMA
-// under a runtime condition makes ptxas split the group and inject warpgroup.arrive around it (warning C7519).
+// One K block of a 128-row tile: 2 x KSTEPS k16 MMAs (rows 0-63 from descriptor ad, rows 64-127 from ad + a_hi, the same
+// B operand), issued back to back as ONE commit group.  KSTEPS must be known at compile time: an MMA under a runtime
+// condition makes ptxas split the group and inject warpgroup.arrive around it (warning C7519).
 template <int BN, int KSTEPS>
-__device__ __forceinline__ void mma_kblock(float (&acc)[BN / 2], uint64_t ad, uint64_t bd, uint32_t scale_d) {
+__device__ __forceinline__ void mma_kblock(float (&acc)[2][BN / 2], uint64_t ad, uint32_t a_hi, uint64_t bd, uint32_t scale_d) {
   wgmma_fence();
-  Wgmma<BN, 0, 0>::mma(acc, ad, bd, scale_d);
 #pragma unroll
-  for (int k = 1; k < KSTEPS; ++k) Wgmma<BN, 0, 0>::mma(acc, ad + (uint64_t)(2 * k), bd + (uint64_t)(2 * k), 1u);
+  for (int k = 0; k < KSTEPS; ++k) {
+    const uint32_t sd = k == 0 ? scale_d : 1u;
+    Wgmma<BN, 0, 0>::mma(acc[0], ad + (uint64_t)(2 * k), bd + (uint64_t)(2 * k), sd);
+    Wgmma<BN, 0, 0>::mma(acc[1], ad + (uint64_t)(a_hi + 2 * k), bd + (uint64_t)(2 * k), sd);
+  }
   wgmma_commit();
 }
 
@@ -306,6 +316,7 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   uint64_t* a_empty = a_full + kMaxAStages;
   uint64_t* b_full = a_empty + kMaxAStages;
   uint64_t* b_empty = b_full + kMaxBStages;
+  uint64_t* mma_turn = b_empty + kMaxBStages;       // [wg]: warpgroup wg may start the MMAs of its next tile
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -328,14 +339,15 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       tma_prefetch_desc(&tmA);
       tma_prefetch_desc(&tmB);
     }
-    // full barriers: the producer's expect_tx arrival; empty barriers: one arrival per consumer warpgroup (of both CTAs when
-    // the weight stages are multicast; the input-only a_empty ring of the halo modes stays per CTA)
-    constexpr int kBarSlots = 2 * kMaxStages + 2 * kMaxAStages + 2 * kMaxBStages;
-    for (int i = lane; i < kBarSlots; i += 32) {
-      const bool is_b_empty = (i >= kMaxStages && i < 2 * kMaxStages) || (i >= 2 * kMaxStages + 2 * kMaxAStages + kMaxBStages);
-      const bool is_a_empty = (i >= 2 * kMaxStages + kMaxAStages && i < 2 * kMaxStages + 2 * kMaxAStages);
-      mbar_init(&bars[i], is_b_empty ? (CP ? 4u : 2u) : is_a_empty ? 2u : 1u);
+    // full barriers: the producer's expect_tx arrival; empty barriers: one arrival from the warpgroup that owns the stage's
+    // tile (in both CTAs when the weight stages are multicast; the input-only a_empty ring of the halo modes stays per CTA);
+    // mma_turn: all 128 threads of the other consumer warpgroup
+    constexpr int kRingSlots = 2 * kMaxStages + 2 * kMaxAStages + 2 * kMaxBStages;
+    for (int i = lane; i < kRingSlots + 2; i += 32) {
+      const bool is_b_empty = (i >= kMaxStages && i < 2 * kMaxStages) || (i >= 2 * kMaxStages + 2 * kMaxAStages + kMaxBStages && i < kRingSlots);
+      mbar_init(&bars[i], i >= kRingSlots ? 128u : (is_b_empty && CP) ? 2u : 1u);
     }
+    static_assert((kRingSlots + 2) * sizeof(uint64_t) <= 1024, "barriers overflow their 1 KB of shared memory");
     fence_mbar_init();
   }
   if (CP) cluster_sync_all();   // the peer's barriers are initialised before anything multicasts into it or arrives on them
@@ -343,111 +355,139 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 
   const int kblocks = p.npairs * p.taps * p.cin_blocks;
 
-  if (warp == 0) {
-    // ================================ TMA producer ================================
-    // The whole warp walks the schedule (keeps control flow convergent so addresses / coordinates
-    // live in uniform registers); one elected lane arms the barrier and issues the TMA loads.
-    if constexpr (HALO) {
-      int sa = 0, sb = 0;
-      uint32_t pha = 0, phb = 0;
-      bool first = true;
-      const uint32_t a_tx = (uint32_t)HG::kBytes, b_tx = (uint32_t)(BN * 128);
-      for (int tile = unit0; tile < p.num_tiles; tile += ustep) {
-        const TileCoord t = coord(tile);
-        int slot = 0;
-        for (int pi = 0; pi < p.npairs; ++pi) {
-          const int pa = kPairA[6 - p.npairs + pi], pb = kPairB[6 - p.npairs + pi];
-          for (int cb = 0; cb < p.cin_blocks; ++cb) {
-            mbar_wait(&a_empty[sa], pha ^ 1);
-            if (elect_one()) {
-              mbar_expect_tx(&a_full[sa], a_tx);
-              tma_load_5d(sA + (size_t)sa * HG::kStageBytes, &tmA, &a_full[sa], cb * 64, t.w0 - 1, t.h0 * HG::SH - 1, t.i0, pa);
-            }
-            __syncwarp();
-            if (++sa == p.a_stages) { sa = 0; pha ^= 1; }
-            for (int tap = 0; tap < HG::TAPS; ++tap) {
-              if (HG::SH == 2 && (tap % HG::KW) == 0 && cb < p.skip_cb) continue;     // all-zero weight block
-              if constexpr (BRES) {
-                if (first && elect_one()) {
-                  mbar_expect_tx(&b_full[slot], b_tx);
-                  load_b(sB + (size_t)slot * p.b_stage_bytes, &b_full[slot], tap * p.Cin + cb * 64, t.n0, pb);
-                }
-                __syncwarp();
-              } else {
-                mbar_wait(&b_empty[sb], phb ^ 1);
-                if (elect_one()) {
-                  mbar_expect_tx(&b_full[sb], b_tx);
-                  load_b(sB + (size_t)sb * p.b_stage_bytes, &b_full[sb], tap * p.Cin + cb * 64, t.n0, pb);
-                }
-                __syncwarp();
-                if (++sb == p.b_stages) { sb = 0; phb ^= 1; }
-              }
-              ++slot;
-            }
-          }
-        }
-        first = false;
-      }
-    } else {
-      int stage = 0;
-      uint32_t phase = 0;
-      const uint32_t tx = (uint32_t)(p.rows * p.kb_bytes + BN * p.kb_bytes);
-      for (int tile = unit0; tile < p.num_tiles; tile += ustep) {
-        const TileCoord t = coord(tile);
-        for (int pi = 0; pi < p.npairs; ++pi) {
-          const int pa = kPairA[6 - p.npairs + pi], pb = kPairB[6 - p.npairs + pi];
-          for (int tap = 0; tap < p.taps; ++tap) {
-            const int r = tap / p.kw, s = tap - r * p.kw;
-            const int cx = t.w0 * p.stride_w + s - p.pad_w;
-            const int cy = t.h0 * p.stride + r - p.pad;
+  if (warp < 4) {
+    producer_regs();
+    if (warp == 0) {
+      // ================================ TMA producer ================================
+      // The whole warp walks the schedule (keeps control flow convergent so addresses / coordinates
+      // live in uniform registers); one elected lane arms the barrier and issues the TMA loads.
+      // It fills the rings in tile order; which consumer warpgroup owns a tile does not concern it.
+      if constexpr (HALO) {
+        int sa = 0, sb = 0;
+        uint32_t pha = 0, phb = 0;
+        bool first = true;
+        const uint32_t a_tx = (uint32_t)HG::kBytes, b_tx = (uint32_t)(BN * 128);
+        for (int tile = unit0; tile < p.num_tiles; tile += ustep) {
+          const TileCoord t = coord(tile);
+          int slot = 0;
+          for (int pi = 0; pi < p.npairs; ++pi) {
+            const int pa = kPairA[6 - p.npairs + pi], pb = kPairB[6 - p.npairs + pi];
             for (int cb = 0; cb < p.cin_blocks; ++cb) {
-              mbar_wait(&empty[stage], phase ^ 1);
+              mbar_wait(&a_empty[sa], pha ^ 1);
               if (elect_one()) {
-                mbar_expect_tx(&full[stage], tx);
-                tma_load_5d(sA + (size_t)stage * p.a_stage_bytes, &tmA, &full[stage], cb * p.kb_elems, cx, cy, t.i0, pa);
-                load_b(sB + (size_t)stage * p.b_stage_bytes, &full[stage], tap * p.Cin + cb * p.kb_elems, t.n0, pb);
+                mbar_expect_tx(&a_full[sa], a_tx);
+                tma_load_5d(sA + (size_t)sa * HG::kStageBytes, &tmA, &a_full[sa], cb * 64, t.w0 - 1, t.h0 * HG::SH - 1, t.i0, pa);
               }
               __syncwarp();
-              if (++stage == p.stages) {
-                stage = 0;
-                phase ^= 1;
+              if (++sa == p.a_stages) { sa = 0; pha ^= 1; }
+              for (int tap = 0; tap < HG::TAPS; ++tap) {
+                if (HG::SH == 2 && (tap % HG::KW) == 0 && cb < p.skip_cb) continue;     // all-zero weight block
+                if constexpr (BRES) {
+                  if (first && elect_one()) {
+                    mbar_expect_tx(&b_full[slot], b_tx);
+                    load_b(sB + (size_t)slot * p.b_stage_bytes, &b_full[slot], tap * p.Cin + cb * 64, t.n0, pb);
+                  }
+                  __syncwarp();
+                } else {
+                  mbar_wait(&b_empty[sb], phb ^ 1);
+                  if (elect_one()) {
+                    mbar_expect_tx(&b_full[sb], b_tx);
+                    load_b(sB + (size_t)sb * p.b_stage_bytes, &b_full[sb], tap * p.Cin + cb * 64, t.n0, pb);
+                  }
+                  __syncwarp();
+                  if (++sb == p.b_stages) { sb = 0; phb ^= 1; }
+                }
+                ++slot;
+              }
+            }
+          }
+          first = false;
+        }
+      } else {
+        int stage = 0;
+        uint32_t phase = 0;
+        const uint32_t tx = (uint32_t)(p.rows * p.kb_bytes + BN * p.kb_bytes);
+        for (int tile = unit0; tile < p.num_tiles; tile += ustep) {
+          const TileCoord t = coord(tile);
+          for (int pi = 0; pi < p.npairs; ++pi) {
+            const int pa = kPairA[6 - p.npairs + pi], pb = kPairB[6 - p.npairs + pi];
+            for (int tap = 0; tap < p.taps; ++tap) {
+              const int r = tap / p.kw, s = tap - r * p.kw;
+              const int cx = t.w0 * p.stride_w + s - p.pad_w;
+              const int cy = t.h0 * p.stride + r - p.pad;
+              for (int cb = 0; cb < p.cin_blocks; ++cb) {
+                mbar_wait(&empty[stage], phase ^ 1);
+                if (elect_one()) {
+                  mbar_expect_tx(&full[stage], tx);
+                  tma_load_5d(sA + (size_t)stage * p.a_stage_bytes, &tmA, &full[stage], cb * p.kb_elems, cx, cy, t.i0, pa);
+                  load_b(sB + (size_t)stage * p.b_stage_bytes, &full[stage], tap * p.Cin + cb * p.kb_elems, t.n0, pb);
+                }
+                __syncwarp();
+                if (++stage == p.stages) {
+                  stage = 0;
+                  phase ^= 1;
+                }
               }
             }
           }
         }
       }
     }
-  } else if (warp >= 4) {
+  } else {
+    consumer_regs();
     // ================================ consumers ================================
-    // Warpgroup wg (0 / 1) computes rows 64 wg .. 64 wg + 63 of every tile.  One wgmma group is kept in flight: after
-    // committing K block i the warpgroup waits for block i - 1 and only then releases that block's shared memory.  Only the
-    // last group of a tile is waited for in full, before the epilogue.
+    // Ping-pong: the CTA's local tile j (its j-th schedule unit) belongs to warpgroup j & 1, which computes all 128 rows of
+    // it.  The two take turns on the tensor cores: a warpgroup issues the first MMA of a tile only once the other has
+    // committed the last MMA of the preceding tile (mma_turn), so each tile's epilogue runs under the next tile's MMAs.
+    // Within a tile one wgmma group is kept in flight: after committing K block i the warpgroup waits for block i - 1 and
+    // only then releases that block's shared memory.  Only the last group of a tile is waited for in full, before the
+    // epilogue.  A warpgroup steps over the ring stages of the other's tiles (a tile takes the same number of stages
+    // throughout a launch) and never waits on their barriers.
     const int wg = (warp >> 2) - 1;
-    const int ct = (int)threadIdx.x - 128;          // 0 .. 255
-    const bool arrive_lane = ((warp & 3) == 0) && lane == 0;   // one arrival per warpgroup on the empty barriers
+    const int ct = (int)threadIdx.x - 128 * (wg + 1);   // 0 .. 127
+    const bool arrive_lane = ct == 0;                    // one arrival per tile owner on the empty barriers
     // a weight-carrying stage is released in both CTAs of a pair (the peer's producer multicasts into this CTA's copy)
     auto release_b = [&](uint64_t* bar) {
       mbar_arrive(bar);
       if (CP) mbar_arrive_cluster(bar, (uint32_t)(rank ^ 1));
     };
-    float acc[BN / 2];
+    auto skip_stages = [](int& s, uint32_t& ph, int n, int ring) {
+      s += n;
+      ph ^= (uint32_t)(s / ring) & 1u;
+      s %= ring;
+    };
+    float acc[2][BN / 2];                                // rows 0-63 and 64-127 of the tile
     const uint32_t a_base = smem_u32(sA) >> 4, b_base = smem_u32(sB) >> 4;
     const int num_tiles = p.num_tiles, ksteps = p.ksteps, nstages = p.stages;
+    // ring stages of one tile: mode 0: kblocks; halo modes: pcs input stages and b_tile weight stages (streamed weights)
+    const int pcs = p.npairs * p.cin_blocks;
+    const int b_tile = p.npairs * (p.cin_blocks * HG::TAPS - (HG::SH == 2 ? (HG::TAPS / HG::KW) * p.skip_cb : 0));
     int stage = 0;
     uint32_t phase = 0;
     int sa = 0, sb = 0;
-    uint32_t pha = 0, phb = 0;
+    uint32_t pha = 0, phb = 0, turn_ph = 0;
     bool first = true;
-    for (int tile = unit0; tile < num_tiles; tile += ustep) {
+    float* sCw = sC + wg * 64 * stage_pitch(BN);         // this warpgroup's half of the staging tile
+    for (int tile = unit0 + wg * ustep; tile < num_tiles; tile += 2 * ustep) {
+      if (tile != unit0) {                               // the other warpgroup owns the preceding tile
+        if constexpr (HALO) {
+          skip_stages(sa, pha, pcs, p.a_stages);
+          if (!BRES) skip_stages(sb, phb, b_tile, p.b_stages);
+        } else {
+          skip_stages(stage, phase, kblocks, nstages);
+        }
+        mbar_wait(&mma_turn[wg], turn_ph);
+        turn_ph ^= 1;
+      }
       if constexpr (HALO) {
         // A descriptors walk the halo tile: 8-row groups are the 8 pixels of one output row, SH halo rows apart;
-        // tap (r,s) shifts the start address by (W r + s) pixels, the second warpgroup by 8 output rows.
+        // tap (r,s) shifts the start address by (W r + s) pixels, rows 64-127 start 8 output rows further.
         const uint32_t row_bytes = (uint32_t)(HG::W * 128 * HG::SH);
         const uint64_t desc_a = wgmma_desc(16u, row_bytes, 1u);
         const uint64_t desc_b = wgmma_desc(16u, 1024u, 1u);
         const uint32_t halo_step = (uint32_t)HG::kStageBytes >> 4, b_step = (uint32_t)p.b_stage_bytes >> 4;
-        const uint32_t wg_off = (uint32_t)wg * 8u * (row_bytes >> 4);
-        const int pcs = p.npairs * p.cin_blocks, skip_cb = p.skip_cb, cin_blocks = p.cin_blocks, b_stages = p.b_stages;
+        const uint32_t a_hi = 8u * (row_bytes >> 4);
+        const int skip_cb = p.skip_cb, cin_blocks = p.cin_blocks, b_stages = p.b_stages;
         int slot = 0;
         uint32_t started = 0;
         // Stages whose MMAs may still be in flight: the B stage of the last committed group and the A stage of the previous
@@ -456,17 +496,17 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         int prev_sb = -1, prev_sa = -1;
         for (int pc = 0; pc < pcs; ++pc) {
           mbar_wait(&a_full[sa], pha);
-          const uint32_t a0 = a_base + (uint32_t)sa * halo_step + wg_off;
+          const uint32_t a0 = a_base + (uint32_t)sa * halo_step;
           const bool skip_s0 = (HG::SH == 2) && (pc % cin_blocks) < skip_cb;      // this channel block of the s = 0 taps is all zero
 #pragma unroll
           for (int tap = 0; tap < HG::TAPS; ++tap) {
             if (HG::SH == 2 && (tap % HG::KW) == 0 && skip_s0) continue;
             const int bs = BRES ? slot : sb;
-            // resident weights were loaded (and waited for) during this CTA's first tile
+            // resident weights were loaded during the CTA's first tile; each warpgroup waits for them before its first tile
             if (!BRES || first) mbar_wait(&b_full[bs], BRES ? 0u : phb);
             const uint64_t ad = desc_a | (uint64_t)(a0 + (uint32_t)((tap / HG::KW) * HG::W + (tap % HG::KW)) * 8u);
             const uint64_t bd = desc_b | (uint64_t)(b_base + (uint32_t)bs * b_step);
-            mma_kblock<BN, 4>(acc, ad, bd, started);
+            mma_kblock<BN, 4>(acc, ad, a_hi, bd, started);
             started = 1u;
             if (!BRES || prev_sa >= 0) {
               wgmma_wait<1>();
@@ -485,6 +525,7 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           prev_sa = sa;
           if (++sa == p.a_stages) { sa = 0; pha ^= 1; }
         }
+        mbar_arrive(&mma_turn[wg ^ 1]);                  // the other warpgroup may start its tile's MMAs
         wgmma_wait<0>();
         if (arrive_lane) {
           if (!BRES && prev_sb >= 0) release_b(&b_empty[prev_sb]);
@@ -493,17 +534,17 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       } else {
         const uint64_t desc = wgmma_desc(16u, (uint32_t)p.sbo_bytes, (uint32_t)p.layout_type);
         const uint32_t a_step = (uint32_t)p.a_stage_bytes >> 4, b_step = (uint32_t)p.b_stage_bytes >> 4;
-        const uint32_t wg_off = (uint32_t)(wg * 64 * p.kb_bytes) >> 4;
+        const uint32_t a_hi = (uint32_t)(64 * p.kb_bytes) >> 4;
         int prev = -1;
         for (int kb = 0; kb < kblocks; ++kb) {
           mbar_wait(&full[stage], phase);
-          const uint64_t ad = desc | (uint64_t)(a_base + (uint32_t)stage * a_step + wg_off);
+          const uint64_t ad = desc | (uint64_t)(a_base + (uint32_t)stage * a_step);
           const uint64_t bd = desc | (uint64_t)(b_base + (uint32_t)stage * b_step);
           const uint32_t scale_d = (uint32_t)(kb != 0);
           switch (ksteps) {          // 16-, 32- or 64-channel K blocks
-            case 1: mma_kblock<BN, 1>(acc, ad, bd, scale_d); break;
-            case 2: mma_kblock<BN, 2>(acc, ad, bd, scale_d); break;
-            default: mma_kblock<BN, 4>(acc, ad, bd, scale_d); break;
+            case 1: mma_kblock<BN, 1>(acc, ad, a_hi, bd, scale_d); break;
+            case 2: mma_kblock<BN, 2>(acc, ad, a_hi, bd, scale_d); break;
+            default: mma_kblock<BN, 4>(acc, ad, a_hi, bd, scale_d); break;
           }
           wgmma_wait<1>();
           if (prev >= 0 && arrive_lane) release_b(&empty[prev]);
@@ -513,53 +554,60 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             phase ^= 1;
           }
         }
+        mbar_arrive(&mma_turn[wg ^ 1]);                  // the other warpgroup may start its tile's MMAs
         wgmma_wait<0>();
         if (prev >= 0 && arrive_lane) release_b(&empty[prev]);
       }
-      wgmma_fence_operand(acc);
+      wgmma_fence_operand(acc[0]);
+      wgmma_fence_operand(acc[1]);
       first = false;
 
-      // ---- epilogue: fragment -> fp32 staging tile -> coalesced 16-channel chunks with the fused tail ----
-      consumer_bar_sync();                       // the previous tile's chunks have all been read from the staging tile
-      {
-        const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
-        const int c0 = 2 * (lane & 3);
+      // ---- epilogue, in two 64-row passes: fragment -> this warpgroup's staging half -> coalesced 16-channel chunks
+      //      with the fused tail ----
+      const TileCoord t = coord(tile);
+      constexpr int kChunks = BN / 16;
+      const int r0 = (warp & 3) * 16 + (lane >> 2);
+      const int c0 = 2 * (lane & 3);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int rows = min(64, p.rows - 64 * h);
+        if (rows <= 0) break;
+        warpgroup_bar_sync(wg);                  // the previous pass's chunks have all been read from the staging half
 #pragma unroll
         for (int j = 0; j < BN / 8; ++j) {
 #pragma unroll
           for (int i = 0; i < 2; ++i) {
-            *reinterpret_cast<float2*>(sC + (r0 + 8 * i) * stage_pitch(BN) + 8 * j + c0) =
-                make_float2(acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]);
+            *reinterpret_cast<float2*>(sCw + (r0 + 8 * i) * stage_pitch(BN) + 8 * j + c0) =
+                make_float2(acc[h][4 * j + 2 * i], acc[h][4 * j + 2 * i + 1]);
           }
         }
-      }
-      consumer_bar_sync();
-      const TileCoord t = coord(tile);
-      constexpr int kChunks = BN / 16;
-      for (int item = ct; item < p.rows * kChunks; item += 256) {
-        const int row = item / kChunks, ch = item - row * kChunks;
-        const int n = t.n0 + 16 * ch;
-        const int ncol = min(16, p.Cout - n);
-        if (ncol <= 0) continue;
-        const int bw = row % p.BW, tq = row / p.BW;
-        const int bh = tq % p.BH, bi = tq / p.BH;
-        const int img = t.i0 + bi, ho = t.h0 + bh, wo = t.w0 + bw;
-        if (img >= p.N || ho >= p.Ho || wo >= p.Wo) continue;
-        const int64_t off = (int64_t)img * p.y_img_stride + (int64_t)ho * p.y_h_stride + (int64_t)wo * p.y_w_stride;
-        const int64_t roff = (int64_t)img * p.res_img_stride + (int64_t)ho * p.res_h_stride + (int64_t)wo * p.res_w_stride;
-        const float4* src = reinterpret_cast<const float4*>(sC + row * stage_pitch(BN) + 16 * ch);
-        uint32_t r[16];
+        warpgroup_bar_sync(wg);
+        for (int item = ct; item < rows * kChunks; item += 128) {
+          const int lr = item / kChunks, ch = item - lr * kChunks;
+          const int row = 64 * h + lr;
+          const int n = t.n0 + 16 * ch;
+          const int ncol = min(16, p.Cout - n);
+          if (ncol <= 0) continue;
+          const int bw = row % p.BW, tq = row / p.BW;
+          const int bh = tq % p.BH, bi = tq / p.BH;
+          const int img = t.i0 + bi, ho = t.h0 + bh, wo = t.w0 + bw;
+          if (img >= p.N || ho >= p.Ho || wo >= p.Wo) continue;
+          const int64_t off = (int64_t)img * p.y_img_stride + (int64_t)ho * p.y_h_stride + (int64_t)wo * p.y_w_stride;
+          const int64_t roff = (int64_t)img * p.res_img_stride + (int64_t)ho * p.res_h_stride + (int64_t)wo * p.res_w_stride;
+          const float4* src = reinterpret_cast<const float4*>(sCw + lr * stage_pitch(BN) + 16 * ch);
+          uint32_t r[16];
 #pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          const float4 f = src[q];
-          r[4 * q + 0] = __float_as_uint(f.x);
-          r[4 * q + 1] = __float_as_uint(f.y);
-          r[4 * q + 2] = __float_as_uint(f.z);
-          r[4 * q + 3] = __float_as_uint(f.w);
+          for (int q = 0; q < 4; ++q) {
+            const float4 f = src[q];
+            r[4 * q + 0] = __float_as_uint(f.x);
+            r[4 * q + 1] = __float_as_uint(f.y);
+            r[4 * q + 2] = __float_as_uint(f.z);
+            r[4 * q + 3] = __float_as_uint(f.w);
+          }
+          float v[16];
+          epilogue_math(p, nullptr, r, n, ncol, true, roff, v);
+          store_chunk(p, off, n, ncol, v);
         }
-        float v[16];
-        epilogue_math(p, nullptr, r, n, ncol, true, roff, v);
-        store_chunk(p, off, n, ncol, v);
       }
     }
   }
@@ -577,7 +625,7 @@ struct ConvPlan {
   CUtensorMapSwizzle swz;
 };
 
-// wgmma N of the kernel variants (accumulator registers per consumer thread = BN / 2)
+// wgmma N of the kernel variants (accumulator registers per consumer thread = BN: two m64 halves of BN / 2)
 constexpr int kBNs[4] = {32, 64, 96, 128};
 
 static inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
