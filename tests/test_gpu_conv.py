@@ -167,7 +167,7 @@ def test_stem_kernels_match_torch(N, H, W, Cout, act, u8, fp32_math):
     """yv6_stem_fwd (3x3 stride-2 conv over the 3-channel image, common.py:197-255 deploy form of the first
     RepVGGBlock / ConvBNSiLU): tensor-core path on bf16-rounded image / weights, and the fp32 CUDA-core path."""
     import ctypes as C
-    from yolov6_b200 import _lib
+    from yolov6_b200 import _lib, ops
     dev = torch.device("cuda:0")
     g = torch.Generator().manual_seed(H * 131 + W)
     x = (torch.rand(N, 3, H, W, generator=g) * 255).to(torch.uint8) if u8 else torch.rand(N, 3, H, W, generator=g)
@@ -184,11 +184,7 @@ def test_stem_kernels_match_torch(N, H, W, Cout, act, u8, fp32_math):
     wd = w.permute(2, 3, 1, 0).contiguous().to(dev)        # [3][3][3][Cout]
     bd = b.to(dev)
     y = torch.full((N, Ho, Wo, Cout), float("nan"), dtype=torch.bfloat16, device=dev)
-    d = _lib.StemDesc()
-    d.x, d.x_dtype, d.in_scale = xd.data_ptr(), (_lib.DT_U8 if u8 else _lib.DT_F32), 1.0 / 255.0
-    d.N, d.H, d.W = N, H, W
-    d.w, d.bias, d.Cout, d.act = wd.data_ptr(), bd.data_ptr(), Cout, _lib.ACT_CODES[act]
-    d.y, d.y_plane_stride, d.nsplit, d.fp32_math = y.data_ptr(), 0, 1, fp32_math
+    d = ops.stem_desc(xd.data_ptr(), N, H, W, u8, wd.data_ptr(), bd.data_ptr(), Cout, act, y.data_ptr(), fp32_math=fp32_math)
     _lib.check(_lib.lib().yv6_stem_fwd(_lib.handle(0), C.byref(d), _lib.stream_ptr()))
     got = y.float().permute(0, 3, 1, 2).double().cpu()
     assert torch.isfinite(got).all()

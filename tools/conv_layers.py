@@ -25,12 +25,11 @@ MODEL, BATCH, SIZE = "yolov6s", 32, 640
 
 
 def plan_str(p):
-    """yv6_conv_plan output -> 'BWxBHxBI BN<n> kb<k> st<stages> [halo<h> a<A stages>[ res]] [pair]'."""
-    bw, bh, bi, bn, kb, stages, _grid, _tiles, halo, flags = p
-    s = f"{bw}x{bh}x{bi} BN{bn} kb{kb} st{stages}"
-    if halo:
-        s += f" halo{halo} a{flags // 100}" + (" res" if flags % 10 else "")
-    if (flags // 10) % 10:
+    """Plan dict (ops.PLAN_KEYS) -> 'BWxBHxBI BN<n> kb<k> st<stages> [halo<h> a<A stages>[ res]] [pair]'."""
+    s = f"{p['BW']}x{p['BH']}x{p['BI']} BN{p['BN']} kb{p['KB']} st{p['stages']}"
+    if p["halo"]:
+        s += f" halo{p['halo']} a{p['a_res'] // 100}" + (" res" if p["a_res"] % 10 else "")
+    if (p["a_res"] // 10) % 10:
         s += " pair"
     return s
 

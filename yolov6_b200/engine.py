@@ -10,23 +10,122 @@ Precision modes: "bf16" (bf16 operands, fp32 accumulate) and "fp32" (bf16x3 spli
 equivalent products, used for the 1e-4 parity bar of BASELINE.json).
 """
 import ctypes as C
+import itertools
 import os
 
-import numpy as np
 import torch
 
 from . import _lib, ops
-from ._lib import ACT_CODES, DT_BF16, DT_F32, DT_U8, ConvDesc, StemDesc
+from ._lib import ConvDesc
 from .fold import fold_op
 
 
-def _split3(t):
-    t = t.float()
-    p0 = t.to(torch.bfloat16)
-    r1 = t - p0.float()
-    p1 = r1.to(torch.bfloat16)
-    p2 = (r1 - p1.float()).to(torch.bfloat16)
-    return torch.stack([p0, p1, p2])
+def siblings(g):
+    """Pairs of convs that read the same tensor with the same geometry and can run as ONE launch over the
+    concatenated output channels: the cls / reg branches of the decoupled head (effidehead.py:79-84).  {first: second}"""
+    pairs = {}
+    for i, a in enumerate(g.ops):
+        if a.kind != "conv" or not a.name.startswith("detect.cls_convs."):
+            continue
+        for j in range(i + 1, min(i + 3, len(g.ops))):
+            b = g.ops[j]
+            if (b.kind == "conv" and b.name == a.name.replace("cls_convs", "reg_convs") and b.src == a.src and
+                    (b.k, b.s, b.act, b.cout, b.cin) == (a.k, a.s, a.act, a.cout, a.cin) and a.res is None and b.res is None and
+                    a.dst.c_off == 0 and b.dst.c_off == 0 and a.cout % 64 == 0):
+                pairs[i] = j
+    return pairs
+
+
+def sibling_slices(g, sibling):
+    """Sibling convs write one [.., 2 x Cout] buffer and their consumers read its two channel halves:
+    graph buffer index -> (first conv of the pair, channel offset, channel pitch) in that buffer."""
+    out = {}
+    for i, j in sibling.items():
+        c = g.ops[i].cout
+        out[g.ops[i].dst.buf] = (i, 0, 2 * c)
+        out[g.ops[j].dst.buf] = (i, c, 2 * c)
+    return out
+
+
+def pair_view_candidate(op):
+    """3x3 stride-2 convs over <= 32 channels, or over 64 | 128 (the view's zero blocks are skipped there): the convs that get
+    column-pair-view weights and may run on the view (pair_view)."""
+    return op.kind == "conv" and op.k == 3 and op.s == 2 and (op.cin <= 32 or op.cin in (64, 128))
+
+
+def pair_view(d, w_pair, plan_fn):
+    """Descriptor d of a 3x3 stride-2 conv, moved onto the column-pair view of the same memory where that pays; d otherwise.
+
+    On the view, [N, H, W/2, 2*Cin] with the weights w_pair (ops.pair_view_weights), it is a 3x2 conv with stride (2, 1) over
+    contiguous 2*Cin-channel rows.  <= 32 channels: 64-byte pixels fetched with an element stride of 2 keep the TMA unit, not the
+    tensor pipe, busy (ERBlock_2.0 of YOLOv6-S: 170 -> 135 us).  More channels: kept only where the library's halo-reuse
+    mainloop takes the view (plan_fn(view)["halo"] == 2; one 9 x 33 input box per 8 x 16 output tile instead of one box per tap,
+    include/yv6.h `pair_view`), so the input operand crosses L2 -> shared memory 2.6x less often, which is what bounds these
+    small-K layers; on the generic mainloop the plain stride-2 conv moves fewer bytes.  Needs an unsliced input of even width."""
+    if d.x_c_total != d.Cin or d.W % 2:
+        return d
+    v = ConvDesc.from_buffer_copy(d)
+    v.W, v.Cin, v.x_c_total = d.W // 2, 2 * d.Cin, 2 * d.Cin
+    v.w, v.w_plane_stride = w_pair, d.w_plane_stride // 9 * 12          # planes of [Cout][3][2][2*Cin] instead of [Cout][3][3][Cin]
+    v.kw, v.stride_w, v.pad_w, v.out_w, v.pair_view = 2, 1, 1, d.W // 2, 1
+    return v if d.Cin <= 32 or plan_fn(v)["halo"] == 2 else d
+
+
+def conv_launches(g, N, H, W, nsplit, sibling, addr, plan_fn):
+    """Descriptors of the conv launches of one inference forward of graph g over an [N, 3, H, W] input, in launch order:
+    {op index: [ConvDesc, ...]} -- four 1x1 quadrant launches for a transposed conv, one otherwise; the first conv of a sibling pair
+    computes both.  Descriptors only: no allocation and no CUDA call, so the planner can be checked on these launches without a GPU.
+
+    nsplit: 1 (bf16) or 3 (bf16x3 planes); sibling: siblings(g) or {}.  addr(kind, key, q=0) resolves device addresses:
+    ("buf", buffer index) activation buffers, ("fused", first conv of the pair) the [.., 2 x Cout] sibling outputs,
+    ("head", "cls" | "reg") the [N, A, ch] fp32 head tensors, ("w", op index, quadrant q of a transposed conv) packed weights,
+    ("w_pair" | "w_fused" | "bias" | "bias_fused", op index) the other packed weights and padded biases; ("alpha", op index) is
+    the residual scale.
+    plan_fn(desc) -> plan dict (ops.PLAN_KEYS) decides where the column-pair view is kept."""
+    offs = list(itertools.accumulate(((H // s) * (W // s) for s in g.strides), initial=0))    # first anchor of each level
+    A = offs[-1]
+    slices = sibling_slices(g, sibling)
+    second = set(sibling.values())
+
+    def view(t):
+        """(address, channel offset, (N, h, w, channel pitch)) of graph tensor slice t."""
+        b = g.bufs[t.buf]
+        nhw = (N, H >> b.level, W >> b.level)
+        if t.buf in slices:
+            i, c0, pitch = slices[t.buf]
+            return addr("fused", i), c0 + t.c_off, nhw + (pitch,)
+        return addr("buf", t.buf), t.c_off, nhw + (b.c_total,)
+
+    out = {}
+    for i, op in enumerate(g.ops):
+        if op.kind not in ("conv", "pred", "convT") or i in second:
+            continue                      # the second conv of a sibling pair is computed by the first one's launch
+        if op.kind == "pred" and op.head[0] not in ("cls", "reg"):
+            continue                      # eval forward: anchor-free (cls, reg) branches only (effidehead_fuseab.py:141-199, _distill_ns.py:105-150)
+        fused = i in sibling
+        x, x_off, xs = view(op.src)
+        k, s = (1, 1) if op.kind == "convT" else (op.k, op.s)
+        ws = (2 * op.cout if fused else op.cout, k, k, op.cin)
+        kw = dict(x_c_off=x_off, bias=addr("bias_fused" if fused else "bias", i), stride=s, act=op.act, nsplit=nsplit)
+        if op.res is not None:
+            r, r_off, (_, rh, rw, rct) = view(op.res)
+            kw.update(res=r, res_c_off=r_off, res_strides=(rh * rw * rct, rw * rct, rct), alpha=addr("alpha", i))
+        if op.kind == "pred":
+            which, lvl = op.head
+            ch, lw = op.cout, W // g.strides[lvl]
+            out[i] = [ops.conv_desc(x, xs, addr("w", i), ws, addr("head", which), (A * ch, lw * ch, ch), y_elem_off=offs[lvl] * ch,
+                                    y_f32=True, **kw)]
+            continue
+        y, y_off, (_, dh, dw, dct) = view(op.dst)
+        if op.kind == "convT":           # scatter quadrant (dy, dx) of the 2x upsample
+            out[i] = [ops.conv_desc(x, xs, addr("w", i, q), ws, y, (dh * dw * dct, 2 * dw * dct, 2 * dct), y_c_off=y_off,
+                                    y_elem_off=(q // 2 * dw + q % 2) * dct, **kw) for q in range(4)]
+            continue
+        d = ops.conv_desc(x, xs, addr("w_fused" if fused else "w", i), ws, y, (dh * dw * dct, dw * dct, dct), y_c_off=y_off, **kw)
+        if pair_view_candidate(op):
+            d = pair_view(d, addr("w_pair", i), plan_fn)
+        out[i] = [d]
+    return out
 
 
 class InferEngine:
@@ -51,27 +150,15 @@ class InferEngine:
         self._pack(state_dict)
 
     # ------------------------------------------------------------------ weight packing
-    def _siblings(self):
-        """Pairs of convs that read the same tensor with the same geometry and can run as ONE launch over the
-        concatenated output channels: the cls / reg branches of the decoupled head (effidehead.py:79-84)."""
-        pairs = {}
-        ops = self.g.ops
-        for i, a in enumerate(ops):
-            if a.kind != "conv" or not a.name.startswith("detect.cls_convs."):
-                continue
-            for j in range(i + 1, min(i + 3, len(ops))):
-                b = ops[j]
-                if (b.kind == "conv" and b.name == a.name.replace("cls_convs", "reg_convs") and b.src == a.src and
-                        (b.k, b.s, b.act, b.cout, b.cin) == (a.k, a.s, a.act, a.cout, a.cin) and a.res is None and b.res is None and
-                        a.dst.c_off == 0 and b.dst.c_off == 0 and a.cout % 64 == 0):
-                    pairs[i] = j
-        return pairs
-
     def _pack(self, sd):
         sd = {k: v.detach().cpu() for k, v in sd.items()}
         dev = self.device
-        self.sibling = self._siblings() if self.fuse_siblings else {}
-        self.sibling_second = {j: i for i, j in self.sibling.items()}
+
+        def planes(w):       # KRSC weights in the precision's operand layout
+            w = w.float().to(dev)
+            return ops.split3(w).contiguous() if self.nsplit == 3 else w.to(torch.bfloat16).contiguous()
+
+        self.sibling = siblings(self.g) if self.fuse_siblings else {}
         for i, op in enumerate(self.g.ops):
             if op.kind == "pool" or (op.kind == "pred" and op.head[0] not in ("cls", "reg")):   # fuse_ab / distillation preds: training only
                 continue
@@ -82,28 +169,16 @@ class InferEngine:
                 ent["b_dev"] = b.float().contiguous().to(dev)
             else:
                 ws = w if isinstance(w, list) else [w]
-                packed = []
-                for wi in ws:
-                    wi = wi.float().to(dev)
-                    packed.append(_split3(wi).contiguous() if self.nsplit == 3 else wi.to(torch.bfloat16).contiguous())
-                ent["w"] = packed
-                if op.kind == "conv" and op.k == 3 and op.s == 2 and (op.cin <= 32 or op.cin in (64, 128)):     # (64 | 128: the view's zero blocks are skipped)
-                    # column-pair view (see _plan): [Cout][3][2][2*Cin]; tap 0 = input columns (2j-2 | 2j-1), tap 1 = (2j | 2j+1)
-                    wf = ops.pair_view_weights(ws[0].float()).to(dev)
-                    ent["w_pair"] = _split3(wf).contiguous() if self.nsplit == 3 else wf.to(torch.bfloat16).contiguous()
-                bias = torch.zeros((op.cout + 255) // 256 * 256, dtype=torch.float32, device=dev)
-                bias[:op.cout] = b.float().to(dev)
-                ent["bias"] = bias
+                ent["w"] = [planes(wi) for wi in ws]
+                if pair_view_candidate(op):      # [Cout][3][2][2*Cin] weights of the column-pair view (see pair_view)
+                    ent["w_pair"] = planes(ops.pair_view_weights(ws[0].float()))
+                ent["bias"] = ops.pad_bias(b.to(dev), op.cout)
             ent["alpha"] = float(sd[op.alpha]) if (op.alpha and op.res is not None) else 1.0
             self.weights[i] = ent
         for i, j in self.sibling.items():      # one conv with 2 x Cout output channels: [cls branch | reg branch]
             (wa, ba), (wb, bb) = fold_op(sd, self.g.ops[i]), fold_op(sd, self.g.ops[j])
-            wf = torch.cat([wa, wb], 0).float().to(dev)
-            c2 = wf.shape[0]
-            bias = torch.zeros((c2 + 255) // 256 * 256, dtype=torch.float32, device=dev)
-            bias[:c2] = torch.cat([ba, bb]).float().to(dev)
-            self.weights[i]["w_fused"] = _split3(wf).contiguous() if self.nsplit == 3 else wf.to(torch.bfloat16).contiguous()
-            self.weights[i]["bias_fused"] = bias
+            self.weights[i]["w_fused"] = planes(torch.cat([wa, wb], 0))
+            self.weights[i]["bias_fused"] = ops.pad_bias(torch.cat([ba, bb]).to(dev), 2 * self.g.ops[i].cout)
 
     # ------------------------------------------------------------------ per-shape plan
     def _plan(self, N, H, W, in_dtype):
@@ -127,8 +202,7 @@ class InferEngine:
             shape = (P, N, h, w, b.c_total) if P == 3 else (N, h, w, b.c_total)
             plan["bufs"].append(torch.zeros(shape, dtype=torch.bfloat16, device=dev))
         sizes = [(H // s, W // s) for s in g.strides]
-        offs = np.concatenate([[0], np.cumsum([h * w for h, w in sizes])]).astype(int)
-        A = int(offs[-1])
+        A = sum(h * w for h, w in sizes)
         nc, R = g.num_classes, 4 * (g.reg_max + 1)
         plan["cls"] = torch.empty(N, A, nc, dtype=torch.float32, device=dev)
         plan["reg"] = torch.empty(N, A, R, dtype=torch.float32, device=dev)
@@ -139,140 +213,73 @@ class InferEngine:
         plan["lvl_s"] = (C.c_float * len(sizes))(*[float(s) for s in g.strides])
         plan["image"] = None
 
-        # sibling convs write one [.., 2C] buffer; their consumers read its two channel halves
-        redirect = {}       # graph buffer index -> (fused tensor, channel offset, channel pitch)
-        plan["fused_bufs"] = []
-        for i, j in self.sibling.items():
-            a, b2 = g.ops[i], g.ops[j]
-            lvl = g.bufs[a.dst.buf].level
-            h, w = H >> lvl, W >> lvl
-            shape = (P, N, h, w, 2 * a.cout) if P == 3 else (N, h, w, 2 * a.cout)
-            fb = torch.zeros(shape, dtype=torch.bfloat16, device=dev)
-            plan["fused_bufs"].append(fb)
-            redirect[a.dst.buf] = (fb, 0, 2 * a.cout)
-            redirect[b2.dst.buf] = (fb, a.cout, 2 * a.cout)
+        slices = sibling_slices(g, self.sibling)
+        fused = {}          # first conv of a sibling pair -> the pair's [.., 2 x Cout] output
+        for i in self.sibling:
+            lvl = g.bufs[g.ops[i].dst.buf].level
+            shape = (N, H >> lvl, W >> lvl, 2 * g.ops[i].cout)
+            fused[i] = torch.zeros((P,) + shape if P == 3 else shape, dtype=torch.bfloat16, device=dev)
+        plan["fused_bufs"] = list(fused.values())
 
         def view(t):
-            b = g.bufs[t.buf]
-            h, w = H >> b.level, W >> b.level
-            if t.buf in redirect:
-                fb, coff, pitch = redirect[t.buf]
-                return fb, h, w, pitch
-            return plan["bufs"][t.buf], h, w, b.c_total
-
-        def coff(t):
-            return t.c_off + (redirect[t.buf][1] if t.buf in redirect else 0)
+            """(tensor, first channel) of a graph tensor slice."""
+            if t.buf in slices:
+                i, c0, _ = slices[t.buf]
+                return fused[i], c0 + t.c_off
+            return plan["bufs"][t.buf], t.c_off
 
         def span(t):
             """(tensor identity, first channel, end channel) of a graph tensor slice: the unit of the dependency analysis."""
-            return (id(view(t)[0]), coff(t), coff(t) + t.c)
+            buf, c0 = view(t)
+            return (id(buf), c0, c0 + t.c)
 
+        def addr(kind, key, q=0):
+            """Device addresses of this plan's tensors and the packed weights (see conv_launches)."""
+            if kind == "buf":
+                return plan["bufs"][key].data_ptr()
+            if kind == "fused":
+                return fused[key].data_ptr()
+            if kind == "head":
+                return plan[key].data_ptr()
+            if kind == "alpha":
+                return self.weights[key]["alpha"]
+            t = self.weights[key][kind]
+            return (t[q] if kind == "w" else t).data_ptr()
+
+        launches = conv_launches(g, N, H, W, P, self.sibling, addr, lambda d: ops.plan_of(d, dev.index or 0))
         for i, op in enumerate(g.ops):
-            ent = self.weights.get(i)
             if op.kind == "stem":
-                buf, h, w, ct = view(op.dst)
-                d = StemDesc()
-                d.x_dtype = DT_U8 if in_dtype == torch.uint8 else DT_F32
-                d.in_scale = 1.0 / 255.0
-                d.N, d.H, d.W = N, H, W
-                d.w = ent["w_dev"].data_ptr()
-                d.bias = ent["b_dev"].data_ptr()
-                d.Cout, d.act = op.cout, ACT_CODES[op.act]
-                d.y = buf.data_ptr()
-                d.y_plane_stride = buf.stride(0) if P == 3 else 0
-                d.nsplit = P
+                buf, _ = view(op.dst)
+                ent = self.weights[i]
+                d = ops.stem_desc(0, N, H, W, in_dtype == torch.uint8, ent["w_dev"].data_ptr(), ent["b_dev"].data_ptr(), op.cout, op.act,
+                                  buf.data_ptr(), P, buf.stride(0) if P == 3 else 0)
                 plan["stem"] = d
                 plan["calls"].append(("stem", d))
                 plan["deps"].append(dict(reads=[], writes=[span(op.dst)]))
-            elif op.kind in ("conv", "pred", "convT"):
-                if op.kind == "pred" and op.head[0] not in ("cls", "reg"):
-                    continue                      # eval forward: anchor-free (cls, reg) branches only (effidehead_fuseab.py:141-199, _distill_ns.py:105-150)
-                if i in self.sibling_second:
-                    continue                      # computed by its sibling's launch
-                sbuf, sh, sw, sct = view(op.src)
-                quads = ent["w"] if op.kind == "convT" else [ent["w"][0]]
-                fused = i in self.sibling
-                for q, wq in enumerate(quads):
-                    d = ConvDesc()
-                    d.x = sbuf.data_ptr() + coff(op.src) * 2
-                    d.N, d.H, d.W, d.Cin, d.x_c_total = N, sh, sw, op.cin, sct
-                    d.x_plane_stride = sbuf.stride(0) if P == 3 else 0
-                    if fused:
-                        wq = ent["w_fused"]
-                    d.w = wq.data_ptr()
-                    d.w_plane_stride = wq.stride(0) if P == 3 else 0
-                    d.bias = (ent["bias_fused"] if fused else ent["bias"]).data_ptr()
-                    d.Cout = op.cout * (2 if fused else 1)
-                    d.kh = d.kw = 1 if op.kind == "convT" else op.k
-                    d.stride = 1 if op.kind == "convT" else op.s
-                    d.pad = d.kh // 2
-                    d.pad_w = _lib.PAD_SAME
-                    d.act = ACT_CODES[op.act]
-                    d.nsplit = P
-                    oh, ow = (sh + 2 * d.pad - d.kh) // d.stride + 1, (sw + 2 * d.pad - d.kw) // d.stride + 1
-                    plan["conv_info"].append(dict(name=op.name if op.kind != "convT" else f"{op.name}[{q}]", cin=op.cin, cout=int(d.Cout),
-                                                  k=d.kh, s=d.stride, ho=oh, wo=ow, h=sh, w=sw,
-                                                  flops=2.0 * N * oh * ow * d.Cout * op.cin * d.kh * d.kw,
-                                                  y_f32=op.kind == "pred"))
-                    if op.kind == "pred":
-                        which, lvl = op.head
-                        out = plan[which]
-                        ch = out.shape[2]
-                        lh, lw = sizes[lvl]
-                        d.y = out.data_ptr() + int(offs[lvl]) * ch * 4
-                        plan["pred_descs"].append((d, which, int(offs[lvl]) * ch * 4))
-                        d.y_dtype = DT_F32
-                        d.y_img_stride, d.y_h_stride, d.y_w_stride = A * ch, lw * ch, ch
-                    else:
-                        dbuf, dh, dw, dct = view(op.dst)
-                        d.y_dtype = DT_BF16
-                        d.y_plane_stride = dbuf.stride(0) if P == 3 else 0
-                        if op.kind == "convT":   # scatter quadrant (dy, dx) of the 2x upsample
-                            dy, dx = q // 2, q % 2
-                            d.y = dbuf.data_ptr() + ((dy * dw + dx) * dct + op.dst.c_off) * 2
-                            d.y_img_stride, d.y_h_stride, d.y_w_stride = dh * dw * dct, 2 * dw * dct, 2 * dct
-                        else:
-                            d.y = dbuf.data_ptr() + (coff(op.dst) if not fused else 0) * 2
-                            d.y_img_stride, d.y_h_stride, d.y_w_stride = dh * dw * dct, dw * dct, dct
-                    if op.res is not None:
-                        rbuf, rh, rw, rct = view(op.res)
-                        d.res = rbuf.data_ptr() + coff(op.res) * 2
-                        d.res_img_stride, d.res_h_stride, d.res_w_stride = rh * rw * rct, rw * rct, rct
-                        d.res_plane_stride = rbuf.stride(0) if P == 3 else 0
-                        d.alpha = ent["alpha"]
-                    if "w_pair" in ent and op.src.c_off == 0 and sct == op.cin and sw % 2 == 0:
-                        # 3x3 stride-2 conv over <= 128 channels.  On the column-pair view of the same memory, [N, H, W/2, 2*Cin],
-                        # it is a 3x2 conv with stride (2, 1) over contiguous 2*Cin-channel rows.  <= 32 channels: 64-byte pixels
-                        # fetched with an element stride of 2 keep the TMA unit, not the tensor pipe, busy (ERBlock_2.0 of
-                        # YOLOv6-S: 170 -> 135 us).  And where the library's halo-reuse mainloop takes the view (one 9 x 33 input
-                        # box per 8 x 16 output tile instead of one box per tap, include/yv6.h `pair_view`) the input operand
-                        # crosses L2 -> shared memory 2.6x less often, which is what bounds these small-K layers.
-                        keep = (d.W, d.Cin, d.x_c_total, d.w, d.w_plane_stride, d.kw, d.stride_w, d.pad_w, d.out_w)
-                        d.W, d.Cin, d.x_c_total = sw // 2, 2 * op.cin, 2 * op.cin
-                        d.w = ent["w_pair"].data_ptr()
-                        d.w_plane_stride = ent["w_pair"].stride(0) if P == 3 else 0
-                        d.kw, d.stride_w, d.pad_w, d.out_w = 2, 1, 1, sw // 2
-                        d.pair_view = 1
-                        out10 = (C.c_int32 * 10)()
-                        _lib.check(self.lib.yv6_conv_plan(self.handle, C.byref(d), out10))
-                        if op.cin > 32 and out10[8] != 2:       # generic mainloop: the plain stride-2 conv moves fewer bytes
-                            d.W, d.Cin, d.x_c_total, d.w, d.w_plane_stride, d.kw, d.stride_w, d.pad_w, d.out_w = keep
-                            d.pair_view = 0
-                    if "neck_start" not in plan and op.name.startswith("neck."):
-                        plan["neck_start"] = len(plan["calls"])     # first launch after the backbone (pipeline.DetectStream forks here)
-                    plan["calls"].append(("conv", d))
-                    reads = [span(op.src)] + ([span(op.res)] if op.res is not None else [])
-                    if op.kind == "pred":
-                        writes = [(("head",) + tuple(op.head), 0, 1)]
-                    elif fused:
-                        writes = [(id(dbuf), 0, 2 * op.cout)]
-                    else:
-                        writes = [span(op.dst)]
-                    plan["deps"].append(dict(reads=reads, writes=writes))
             elif op.kind == "pool":
-                buf, h, w, ct = view(op.dst)
+                buf, _ = view(op.dst)
+                h, w, ct = buf.shape[-3:]
                 plan["calls"].append(("pool", (buf.data_ptr(), N, h, w, op.cin, ct, P, buf.stride(0) if P == 3 else 0)))
                 plan["deps"].append(dict(reads=[(id(buf), 0, op.cin)], writes=[(id(buf), op.cin, 4 * op.cin)]))
+            for q, d in enumerate(launches.get(i, ())):
+                lvl = g.bufs[op.src.buf].level
+                sh, sw, k, s = H >> lvl, W >> lvl, d.kh, d.stride      # (of the 3x3 stride-2 conv, also on the column-pair view)
+                oh, ow = (sh + 2 * (k // 2) - k) // s + 1, (sw + 2 * (k // 2) - k) // s + 1
+                plan["conv_info"].append(dict(name=op.name if op.kind != "convT" else f"{op.name}[{q}]", cin=op.cin, cout=d.Cout,
+                                              k=k, s=s, ho=oh, wo=ow, h=sh, w=sw, flops=2.0 * N * oh * ow * d.Cout * op.cin * k * k,
+                                              y_f32=op.kind == "pred"))
+                reads = [span(op.src)] + ([span(op.res)] if op.res is not None else [])
+                if op.kind == "pred":
+                    plan["pred_descs"].append((d, op.head[0], d.y - plan[op.head[0]].data_ptr()))
+                    writes = [(("head",) + tuple(op.head), 0, 1)]
+                elif i in fused:
+                    writes = [(id(fused[i]), 0, 2 * op.cout)]
+                else:
+                    writes = [span(op.dst)]
+                if "neck_start" not in plan and op.name.startswith("neck."):
+                    plan["neck_start"] = len(plan["calls"])     # first launch after the backbone (pipeline.DetectStream forks here)
+                plan["calls"].append(("conv", d))
+                plan["deps"].append(dict(reads=reads, writes=writes))
         self._schedule(plan)
         self._plans[key] = plan
         return plan
@@ -477,8 +484,6 @@ class InferEngine:
             ho, wo = ci["ho"], ci["wo"]
             fl = ci["flops"]
             by = 2.0 * d.N * (ci["h"] * ci["w"] * ci["cin"] + ho * wo * ci["cout"])
-            out = (C.c_int32 * 10)()
-            _lib.check(self.lib.yv6_conv_plan(self.handle, C.byref(d), out))
             rows.append(dict(name=name, cin=ci["cin"], cout=ci["cout"], k=ci["k"], s=ci["s"], hw=f"{ho}x{wo}", ms=ms,
-                             tflops=fl / ms / 1e9, gbs=by / ms / 1e6, plan=list(out)))
+                             tflops=fl / ms / 1e9, gbs=by / ms / 1e6, plan=ops.plan_of(d, self.device.index or 0)))
         return rows

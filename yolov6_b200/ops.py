@@ -1,24 +1,30 @@
-"""Thin Python wrappers over the C ABI: one function per kernel entry point.
-
-Tensors are torch CUDA tensors used purely as device memory; all layout decisions (NHWC, channel
-slices, bf16x3 planes) are made by the caller (`yolov6_b200.engine`).
+"""Thin Python wrappers over the C ABI: the conv / stem descriptor builders, which take device addresses and shapes (no
+GPU needed), and launch functions over torch CUDA tensors used purely as device memory.  All layout decisions (NHWC,
+channel slices, bf16x3 planes) are made by the caller (`yolov6_b200.engine`).
 """
 import ctypes as C
 
 import torch
 
 from . import _lib
-from ._lib import ACT_CODES, DT_BF16, DT_F32, ConvDesc
+from ._lib import ACT_CODES, DT_BF16, DT_F32, DT_U8, ConvDesc, StemDesc
+
+# Names of the yv6_conv_plan (10) / yv6_conv_plan_host (12) output words.  a_res = A stages * 100 + CTA pair * 10 + B resident.
+PLAN_KEYS = ("BW", "BH", "BI", "BN", "KB", "stages", "grid", "tiles", "halo", "a_res", "smem", "threads")
 
 
 def _ptr(t):
     return C.c_void_p(t.data_ptr()) if t is not None else C.c_void_p(0)
 
 
+def bias_buffer(cout, device):
+    """Zeroed fp32 bias buffer of Cout rounded up to a multiple of 256 (the kernel reads 16 floats at a time)."""
+    return torch.zeros((cout + 255) // 256 * 256, dtype=torch.float32, device=device)
+
+
 def pad_bias(bias, cout):
-    """fp32 bias padded with zeros to a multiple of 256 (the kernel reads 16 floats at a time)."""
-    n = (cout + 255) // 256 * 256
-    out = torch.zeros(n, dtype=torch.float32, device=bias.device)
+    """fp32 bias padded with zeros to a multiple of 256 (see bias_buffer)."""
+    out = bias_buffer(cout, bias.device)
     out[:cout] = bias.float()
     return out
 
@@ -46,6 +52,69 @@ def pair_view_weights(w33):
     return wf
 
 
+def conv_desc(x, x_shape, w, w_shape, y, y_strides, *, x_c_off=0, bias=0, stride=1, act=None, y_c_off=0, y_elem_off=0,
+              y_f32=False, res=None, res_c_off=0, res_strides=None, alpha=1.0, accumulate=False, nsplit=1, pad=None, out_hw=None,
+              stride_w=0, pair_view=0, force=None):
+    """yv6_conv_desc of y[..., y_c_off:+Cout] = act(conv(x[..., x_c_off:+Cin], w) + bias) (+ alpha * res), built from device
+    addresses (ints) and shapes only, so that launches can be described and planned without a GPU.
+
+    x: bf16 NHWC buffer of shape x_shape = (N, H, W, channel pitch); w: bf16 KRSC weights of shape w_shape = (Cout, kh, kw, Cin);
+    bias: padded fp32 (pad_bias) or 0; y: bf16 (fp32 if y_f32) output whose element (n, ho, wo, c) is at
+    y + y_elem_off + c + n * y_strides[0] + ho * y_strides[1] + wo * y_strides[2]; res: bf16 residual laid out the same way with
+    res_strides, or accumulate = True: y += conv(...) (the residual epilogue reads the old value of the same element).
+    nsplit = 3: x, w, res and a bf16 y are each three contiguous bf16 planes.  pad = (rows, columns), default kh // 2 for both.
+    force: {"bw": 8, ...} -> the descriptor's force_* tuning overrides."""
+    N, H, W, Ct = x_shape
+    Cout, kh, kw, Cin = w_shape
+    planes = nsplit == 3
+    d = ConvDesc()
+    d.x = x + x_c_off * 2
+    d.N, d.H, d.W, d.Cin, d.x_c_total = N, H, W, Cin, Ct
+    d.x_plane_stride = N * H * W * Ct if planes else 0
+    d.w = w
+    d.w_plane_stride = Cout * kh * kw * Cin if planes else 0
+    d.bias = bias
+    d.Cout, d.kh, d.kw, d.stride = Cout, kh, kw, stride
+    d.pad, d.pad_w = (kh // 2, _lib.PAD_SAME) if pad is None else pad
+    if out_hw is not None:
+        d.out_h, d.out_w = out_hw
+    d.stride_w, d.pair_view = stride_w, pair_view
+    d.act = ACT_CODES[act]
+    d.y = y + (y_c_off + y_elem_off) * (4 if y_f32 else 2)
+    d.y_dtype = DT_F32 if y_f32 else DT_BF16
+    d.y_img_stride, d.y_h_stride, d.y_w_stride = y_strides
+    d.y_plane_stride = N * y_strides[0] if planes and not y_f32 else 0
+    if accumulate:
+        res, res_c_off, res_strides, alpha = d.y, 0, y_strides, 1.0
+    if res is not None:
+        d.res = res + res_c_off * 2
+        d.res_img_stride, d.res_h_stride, d.res_w_stride = res_strides
+        d.res_plane_stride = N * res_strides[0] if planes else 0
+        d.alpha = alpha
+    d.nsplit = nsplit
+    for k, v in (force or {}).items():
+        setattr(d, "force_" + k, int(v))
+    return d
+
+
+def plan_of(d, device=0):
+    """Tile plan yv6_conv_fwd would use for descriptor d on a device: {PLAN_KEYS[i]: value}."""
+    out = (C.c_int32 * 10)()
+    _lib.check(_lib.lib().yv6_conv_plan(_lib.handle(device), C.byref(d), out))
+    return dict(zip(PLAN_KEYS, out))
+
+
+def stem_desc(x, N, H, W, u8, w, bias, cout, act, y, nsplit=1, y_plane_stride=0, fp32_math=0):
+    """yv6_stem_desc from device addresses: x [N,3,H,W] fp32 (uint8 if u8, scaled by 1/255), w fp32 [3][3][3][Cout], bias fp32
+    [Cout] or 0, y NHWC bf16 (nsplit planes y_plane_stride apart)."""
+    d = StemDesc()
+    d.x, d.x_dtype, d.in_scale = x, DT_U8 if u8 else DT_F32, 1.0 / 255.0
+    d.N, d.H, d.W = N, H, W
+    d.w, d.bias, d.Cout, d.act = w, bias, cout, ACT_CODES[act]
+    d.y, d.y_plane_stride, d.nsplit, d.fp32_math = y, y_plane_stride, nsplit, fp32_math
+    return d
+
+
 def conv_fwd(x, w, bias, y, *, cin=None, x_c_offset=0, stride=1, act=None, y_c_offset=0,
              y_img_stride=None, y_h_stride=None, y_w_stride=None, y_elem_offset=0,
              res=None, res_c_offset=0, alpha=1.0, nsplit=1, force=None, stream=None, pad=None, out_hw=None, stride_w=0, pair_view=0):
@@ -55,69 +124,24 @@ def conv_fwd(x, w, bias, y, *, cin=None, x_c_offset=0, stride=1, act=None, y_c_o
     bias: padded fp32 (see pad_bias) or None; y: NHWC buffer, bf16 ([3,...] when nsplit=3) or fp32.
     """
     planes = nsplit == 3
-    xs = x.shape[1:] if planes else x.shape
     ws = w.shape[1:] if planes else w.shape
-    N, H, W, Ct = xs
-    Cout, kh, kw, Cin = ws
-    if cin is None:
-        cin = Cin
-    assert cin == Cin, (cin, Cin)
-    d = ConvDesc()
-    esz = x.element_size()
-    d.x = x.data_ptr() + x_c_offset * esz
-    d.N, d.H, d.W, d.Cin, d.x_c_total = N, H, W, Cin, Ct
-    d.x_plane_stride = x.stride(0) if planes else 0
-    d.w = w.data_ptr()
-    d.w_plane_stride = w.stride(0) if planes else 0
-    d.bias = bias.data_ptr() if bias is not None else 0
-    d.Cout, d.kh, d.kw, d.stride, d.pad = Cout, kh, kw, stride, (kh // 2 if pad is None else pad[0])
-    d.pad_w = _lib.PAD_SAME if pad is None else pad[1]
-    if out_hw is not None:
-        d.out_h, d.out_w = out_hw
-    d.stride_w, d.pair_view = int(stride_w), int(pair_view)
-    d.act = ACT_CODES[act]
-    y_planes = planes and y.dtype == torch.bfloat16
-    ysh = y.shape[1:] if y_planes else y.shape
-    yst = y.stride()[1:] if y_planes else y.stride()
-    d.y = y.data_ptr() + (y_c_offset + y_elem_offset) * y.element_size()
-    d.y_dtype = DT_BF16 if y.dtype == torch.bfloat16 else DT_F32
-    d.y_img_stride = yst[0] if y_img_stride is None else y_img_stride
-    d.y_h_stride = yst[1] if y_h_stride is None else y_h_stride
-    d.y_w_stride = yst[2] if y_w_stride is None else y_w_stride
-    d.y_plane_stride = y.stride(0) if y_planes else 0
-    if res is not None:
-        rst = res.stride()[1:] if planes else res.stride()
-        d.res = res.data_ptr() + res_c_offset * res.element_size()
-        d.res_img_stride, d.res_h_stride, d.res_w_stride = rst[0], rst[1], rst[2]
-        d.res_plane_stride = res.stride(0) if planes else 0
-    d.alpha = float(alpha)
-    d.nsplit = nsplit
-    if force:
-        for k, v in force.items():
-            setattr(d, "force_" + k, int(v))
+    assert cin is None or cin == ws[3], (cin, ws[3])
+    y_f32 = y.dtype != torch.bfloat16
+    yst = y.stride()[1:] if planes and not y_f32 else y.stride()
+    y_strides = [s if o is None else o for s, o in zip(yst, (y_img_stride, y_h_stride, y_w_stride))]
+    rst = None if res is None else (res.stride()[1:] if planes else res.stride())[:3]
+    d = conv_desc(x.data_ptr(), x.shape[1:] if planes else x.shape, w.data_ptr(), ws, y.data_ptr(), y_strides, x_c_off=x_c_offset,
+                  bias=bias.data_ptr() if bias is not None else 0, stride=stride, act=act, y_c_off=y_c_offset, y_elem_off=y_elem_offset,
+                  y_f32=y_f32, res=None if res is None else res.data_ptr(), res_c_off=res_c_offset, res_strides=rst, alpha=alpha,
+                  nsplit=nsplit, pad=pad, out_hw=out_hw, stride_w=stride_w, pair_view=pair_view, force=force)
     dev = x.device.index or 0
     _lib.check(_lib.lib().yv6_conv_fwd(_lib.handle(dev), C.byref(d), _lib.stream_ptr(stream)))
     return y
 
 
 def conv_plan(x_shape, w_shape, stride=1, nsplit=1, force=None, device=0, stride_w=0, pad=None, out_hw=None, pair_view=0):
-    """Tile plan (BW,BH,BI,BN,KB,stages,grid,tiles) the kernel would use for a shape."""
-    N, H, W, Ct = x_shape
-    Cout, kh, kw, Cin = w_shape
-    d = ConvDesc()
-    d.x = d.w = d.y = 16  # plan only: non-null, aligned
-    d.N, d.H, d.W, d.Cin, d.x_c_total = N, H, W, Cin, Ct
-    d.Cout, d.kh, d.kw, d.stride, d.pad = Cout, kh, kw, stride, kh // 2
-    d.pad_w = _lib.PAD_SAME
-    if pad is not None:
-        d.pad, d.pad_w = pad
-    if out_hw is not None:
-        d.out_h, d.out_w = out_hw
-    d.stride_w, d.pair_view = int(stride_w), int(pair_view)
-    d.nsplit = nsplit
-    if force:
-        for k, v in force.items():
-            setattr(d, "force_" + k, int(v))
-    out = (C.c_int32 * 10)()
-    _lib.check(_lib.lib().yv6_conv_plan(_lib.handle(device), C.byref(d), out))
-    return dict(zip(("BW", "BH", "BI", "BN", "KB", "stages", "grid", "tiles", "halo", "a_res"), list(out)))
+    """Tile plan (PLAN_KEYS) the kernel would use for a shape."""
+    # plan only: non-null, aligned addresses
+    d = conv_desc(16, x_shape, 16, w_shape, 16, (0, 0, 0), stride=stride, nsplit=nsplit, pad=pad, out_hw=out_hw, stride_w=stride_w,
+                  pair_view=pair_view, force=force)
+    return plan_of(d, device)

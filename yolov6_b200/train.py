@@ -33,9 +33,8 @@ import os
 import numpy as np
 import torch
 
-from . import _lib
-from ._lib import (ACT_CODES, DT_BF16, DT_F32, DT_U8, XF_BF16, XF_F32, XF_F64, XFORM_CHUNK, BnDesc, BnStatsDesc, ConvDesc,
-                   StemDesc, WgradDesc, XformSeg)
+from . import _lib, ops
+from ._lib import ACT_CODES, DT_F32, DT_U8, XF_BF16, XF_F32, XF_F64, XFORM_CHUNK, BnDesc, BnStatsDesc, WgradDesc, XformSeg
 from .flat import FlatState
 
 BN_EPS, BN_MOMENTUM = 1e-3, 0.03
@@ -198,7 +197,7 @@ class TrainEngine:
             if op.kind == "pred":
                 ch, cin, chp = op.cout, op.cin, (op.cout + 15) // 16 * 16
                 W["w"] = bf16(ch, 1, 1, cin)
-                W["bias"] = torch.zeros((ch + 255) // 256 * 256, dtype=torch.float32, device=dev)
+                W["bias"] = ops.bias_buffer(ch, dev)
                 W["wt"] = bf16(cin, 1, 1, chp)                                   # dgrad: [Cin][ch_pad], zero padded
                 wsrc, bsrc = fl.ptr(op.name + ".weight"), fl.ptr(op.name + ".bias")
                 pack.append(_seg(W["w"].data_ptr(), wsrc, [ch * cin], [1], [1], XF_BF16, XF_F32))
@@ -210,7 +209,7 @@ class TrainEngine:
                 co, ci = op.cout, op.cin
                 W["w"] = bf16(4, co, 1, 1, ci)                                   # quadrant q = dy*2+dx: [Cout][Cin]
                 W["wt"] = bf16(4, ci, 1, 1, co)                                  # dgrad of quadrant q: [Cin][Cout]
-                W["bias"] = torch.zeros((co + 255) // 256 * 256, dtype=torch.float32, device=dev)
+                W["bias"] = ops.bias_buffer(co, dev)
                 wsrc = fl.ptr(op.name + ".upsample_transpose.weight")            # [Cin][Cout][2][2]
                 pack.append(_seg(W["w"].data_ptr(), wsrc, [4, co, ci], [co * ci, ci, 1], [1, 4, co * 4], XF_BF16, XF_F32))
                 pack.append(_seg(W["wt"].data_ptr(), wsrc, [4, ci, co], [ci * co, co, 1], [1, co * 4, 4], XF_BF16, XF_F32))
@@ -326,34 +325,11 @@ class TrainEngine:
         return segs
 
     # ================================================================== per-shape plan
-    def _conv_desc(self, x, x_off, cin, w, y, y_off, cout, k, stride, *, pad=None, out_hw=None, bias=None, act=None,
-                   y_strides=None, y_elem_off=0, accumulate=False, y_f32=False):
-        """y[..., y_off:+cout] (+)= conv(x[..., x_off:+cin], w).  x: [N,H,W,Ct] bf16, w: [cout,kh,kw,cin] bf16 KRSC,
+    def _conv_desc(self, x, x_off, w, y, y_off=0, *, bias=None, y_strides=None, **kw):
+        """y[..., y_off:+Cout] (+)= conv(x[..., x_off:+Cin], w) (ops.conv_desc).  x: [N,H,W,Ct] bf16, w: [Cout,kh,kw,Cin] bf16 KRSC,
         y: [N,Ho,Wo,Cyt] bf16 (or fp32 head tensor with explicit strides)."""
-        d = ConvDesc()
-        N, H, W, Ct = x.shape
-        d.x = x.data_ptr() + x_off * 2
-        d.N, d.H, d.W, d.Cin, d.x_c_total = N, H, W, cin, Ct
-        d.w = w.data_ptr()
-        d.bias = _p(bias)
-        d.Cout, d.kh, d.kw, d.stride = cout, w.shape[1], w.shape[2], stride
-        d.pad, d.pad_w = (k // 2, _lib.PAD_SAME) if pad is None else pad
-        if out_hw is not None:
-            d.out_h, d.out_w = out_hw
-        d.act = ACT_CODES[act]
-        d.nsplit = 1
-        es = 4 if y_f32 else 2
-        d.y = y.data_ptr() + (y_off + y_elem_off) * es
-        d.y_dtype = DT_F32 if y_f32 else DT_BF16
-        if y_strides is None:
-            _, Ho, Wo, Cyt = y.shape
-            y_strides = (Ho * Wo * Cyt, Wo * Cyt, Cyt)
-        d.y_img_stride, d.y_h_stride, d.y_w_stride = y_strides
-        if accumulate:   # y += conv(...): the residual epilogue reads the old value of the same element
-            d.res = d.y
-            d.alpha = 1.0
-            d.res_img_stride, d.res_h_stride, d.res_w_stride = y_strides
-        return d
+        return ops.conv_desc(x.data_ptr(), x.shape, w.data_ptr(), w.shape, y.data_ptr(), y_strides or y.stride()[:3], x_c_off=x_off,
+                             y_c_off=y_off, bias=_p(bias), y_f32=y.dtype == torch.float32, **kw)
 
     def _wgrad_desc(self, x, x_off, cin, dy, dy_off, cout, k, stride, dw_ptr):
         d = WgradDesc()
@@ -384,11 +360,10 @@ class TrainEngine:
                 d.stats[b] = st.data_ptr()
         return d
 
-    def _dgrad_descs(self, dc, ent, k, stride, gsrc, g_off, cin):
-        """g(src)[..., g_off:+cin] += conv_transpose(dc, w) as one (stride 1) or up to four (stride 2) accumulating convs."""
-        cout = dc.shape[3]
+    def _dgrad_descs(self, dc, ent, k, stride, gsrc, g_off):
+        """g(src)[..., g_off:+Cin] += conv_transpose(dc, w) as one (stride 1) or up to four (stride 2) accumulating convs."""
         if stride == 1:
-            return [self._conv_desc(dc, 0, cout, ent["wt"][0], gsrc, g_off, cin, k, 1, accumulate=True)]
+            return [self._conv_desc(dc, 0, ent["wt"][0], gsrc, g_off, accumulate=True)]
         n, hs, ws, gct = gsrc.shape
         ho, wo = dc.shape[1], dc.shape[2]
         out = []
@@ -402,7 +377,7 @@ class TrainEngine:
                 else:
                     wt = ent["wt"][j]
                     j += 1
-                out.append(self._conv_desc(dc, 0, cout, wt, gsrc, g_off, cin, k, 1, pad=(0, 0), out_hw=(ho, wo), accumulate=True,
+                out.append(self._conv_desc(dc, 0, wt, gsrc, g_off, pad=(0, 0), out_hw=(ho, wo), accumulate=True,
                                            y_strides=(hs * ws * gct, 2 * ws * gct, 2 * gct), y_elem_off=(ph * ws + pw) * gct))
         return out
 
@@ -474,8 +449,8 @@ class TrainEngine:
                 raw = torch.empty(N, lh * lw, ch, dtype=torch.float32, device=dev)
                 dl = bf(N, lh, lw, chp)
                 st["raw_" + which[:3]], st["dl_" + which[:3]] = raw, dl
-                fwd.append(("conv", self._conv_desc(src, op.src.c_off, op.cin, Wt["w"], raw, 0, op.cout, 1, 1, bias=Wt["bias"], act=op.act,
-                                                    y_f32=True, y_strides=(lh * lw * ch, lw * ch, ch), y_elem_off=0)))
+                fwd.append(("conv", self._conv_desc(src, op.src.c_off, Wt["w"], raw, bias=Wt["bias"], act=op.act,
+                                                    y_strides=(lh * lw * ch, lw * ch, ch))))
                 if which == "reg_ab":          # second of the level's pair in forward order, first in backward order
                     anc = [v / float(g.strides[lvl]) for v in g.anchors_init[lvl]]          # effidehead_fuseab.py:35
                     st["anchors"] = (C.c_float * 6)(*anc)
@@ -483,7 +458,7 @@ class TrainEngine:
                     calls.append(("abg", lvl))
                 calls.append(("wgrad", self._wgrad_desc(src, op.src.c_off, op.cin, dl, 0, ch, 1, 1, z(i, "dw"))))
                 calls.append(("stats", self._stats_desc([(dl, 0)], chp, N * lh * lw, z(i, "bsum"), z(i, "bcnt"))))
-                calls.append(("conv", self._conv_desc(dl, 0, chp, Wt["wt"], gsrc, op.src.c_off, op.cin, 1, 1, accumulate=True),
+                calls.append(("conv", self._conv_desc(dl, 0, Wt["wt"], gsrc, op.src.c_off, accumulate=True),
                               dict(buf=op.src.buf, off=op.src.c_off, n=op.cin, full=True)))
                 bwd_rev.append(calls)
                 continue
@@ -495,14 +470,14 @@ class TrainEngine:
                 ch = out.shape[2]
                 chp = (ch + 15) // 16 * 16
                 lh, lw = self.sizes[lvl]
-                fwd.append(("conv", self._conv_desc(src, op.src.c_off, op.cin, Wt["w"], out, 0, op.cout, 1, 1, bias=Wt["bias"], act=op.act,
-                                                    y_f32=True, y_strides=(A * ch, lw * ch, ch), y_elem_off=self.offs[lvl] * ch)))
+                fwd.append(("conv", self._conv_desc(src, op.src.c_off, Wt["w"], out, bias=Wt["bias"], act=op.act,
+                                                    y_strides=(A * ch, lw * ch, ch), y_elem_off=self.offs[lvl] * ch)))
                 dl = bf(N, lh, lw, chp)
                 calls.append(("hgp", (grad.data_ptr(), self.cls.data_ptr() if which == "cls" else 0, N, A, ch, self.offs[lvl], lh * lw, chp,
                                       dl.data_ptr()), dl))
                 calls.append(("wgrad", self._wgrad_desc(src, op.src.c_off, op.cin, dl, 0, ch, 1, 1, z(i, "dw"))))
                 calls.append(("stats", self._stats_desc([(dl, 0)], chp, N * lh * lw, z(i, "bsum"), z(i, "bcnt"))))
-                calls.append(("conv", self._conv_desc(dl, 0, chp, Wt["wt"], gsrc, op.src.c_off, op.cin, 1, 1, accumulate=True),
+                calls.append(("conv", self._conv_desc(dl, 0, Wt["wt"], gsrc, op.src.c_off, accumulate=True),
                               dict(buf=op.src.buf, off=op.src.c_off, n=op.cin, full=True)))
                 bwd_rev.append(calls)
                 continue
@@ -513,7 +488,7 @@ class TrainEngine:
                 _, sh, sw, _ = src.shape
                 for q in range(4):
                     dy, dx = q // 2, q % 2
-                    fwd.append(("conv", self._conv_desc(src, op.src.c_off, op.cin, Wt["w"][q], dst, op.dst.c_off, op.cout, 1, 1, bias=Wt["bias"],
+                    fwd.append(("conv", self._conv_desc(src, op.src.c_off, Wt["w"][q], dst, op.dst.c_off, bias=Wt["bias"],
                                                         y_strides=(dh * dw * dct, 2 * dw * dct, 2 * dct), y_elem_off=(dy * dw + dx) * dct)))
                 gd = gdst[..., op.dst.c_off:op.dst.c_off + op.cout]
                 calls.append(("dbg", (i, gd)))
@@ -527,7 +502,7 @@ class TrainEngine:
                     dq = dq_pool[q][:need].view(N, sh, sw, op.cout)
                     calls.append(("copy", (dq, gd[:, dy::2, dx::2, :])))               # gradient of quadrant q, dense
                     calls.append(("wgrad", self._wgrad_desc(src, op.src.c_off, op.cin, dq, 0, op.cout, 1, 1, z(i, "dw") + 4 * q * op.cout * op.cin)))
-                    calls.append(("conv", self._conv_desc(dq, 0, op.cout, Wt["wt"][q], gsrc, op.src.c_off, op.cin, 1, 1, accumulate=True),
+                    calls.append(("conv", self._conv_desc(dq, 0, Wt["wt"][q], gsrc, op.src.c_off, accumulate=True),
                                   dict(buf=op.src.buf, off=op.src.c_off, n=op.cin, full=True)))
                 bwd_rev.append(calls)
                 continue
@@ -549,15 +524,11 @@ class TrainEngine:
                 raw = bf(n, ho, wo, op.cout)
                 self.ctx[i]["branches"][b]["x"] = raw
                 if op.kind == "stem":
-                    d = StemDesc()
-                    d.x, d.x_dtype, d.in_scale = self.x_static.data_ptr(), x_dt, 1.0 / 255.0
-                    d.N, d.H, d.W = N, H, W
-                    d.w, d.bias, d.Cout, d.act = ent["w"].data_ptr(), 0, op.cout, 0
-                    d.y, d.y_plane_stride, d.nsplit, d.fp32_math = raw.data_ptr(), 0, 1, 1
-                    fwd.append(("stem", d))
+                    fwd.append(("stem", ops.stem_desc(self.x_static.data_ptr(), N, H, W, in_dtype == torch.uint8, ent["w"].data_ptr(), 0,
+                                                      op.cout, None, raw.data_ptr(), fp32_math=1)))
                 else:
                     src, _ = view(op.src)
-                    fwd.append(("conv", self._conv_desc(src, op.src.c_off, op.cin, ent["w"], raw, 0, op.cout, k, op.s)))
+                    fwd.append(("conv", self._conv_desc(src, op.src.c_off, ent["w"], raw, stride=op.s)))
                 xs.append((raw, 0))
             fin = [(ent["prefix"] + (".bn" if ent["k"] else ""), st[b]) for b, ent in enumerate(br)]
             fwd.append(("stats", self._stats_desc(xs, op.cout, count, z(i, "fsum"), z(i, "fcnt"), fin)))
@@ -611,7 +582,7 @@ class TrainEngine:
                     if ent["k"] == 0:
                         continue
                     calls.append(("wgrad", self._wgrad_desc(src, op.src.c_off, op.cin, dcs[b], 0, op.cout, ent["k"], op.s, z(i, "dw", b)), par))
-                    dds = self._dgrad_descs(dcs[b], ent, ent["k"], op.s, gsrc, op.src.c_off, op.cin)
+                    dds = self._dgrad_descs(dcs[b], ent, ent["k"], op.s, gsrc, op.src.c_off)
                     # a stride-2 3x3 dgrad = four parity convolutions that together cover every pixel; 1x1 stride 2 covers one parity
                     full = op.s == 1 or ent["k"] == 3
                     for gi, dd in enumerate(dds):
