@@ -196,6 +196,27 @@ int yv6_eval_boxes(yv6_handle* h, const float* det, const int32_t* count, const 
                    float* out, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Serving from decoded frames: the two steps of the reference's Inferer around the model, for a whole batch per launch.
+ * Per-image geometry table geo [B][YV6_LB_GEO] int32 (device) = (src_off, h0, w0, nh, nw, top, left, 0):
+ *   src_off   byte offset of the image in `src` (images packed back to back, each uint8 HWC BGR [h0][w0][3]);
+ *   nh, nw    new_unpad of letterbox (data_augment.py:43), top / left its integer border (:54-55), computed by the caller
+ *             with the reference's Python expressions; the kernels recompute none of them.
+ *
+ * yv6_letterbox: letterbox(im, (H, W), auto=False) (data_augment.py:29-58) + HWC->CHW + BGR->RGB of Inferer.process_image
+ *   (core/inferer.py:161-171) -> dst uint8 NCHW [B,3,H,W] (the stem's YV6_DT_U8 input; the 1/255 stays in the stem).
+ *   Canvas outside [top, top+nh) x [left, left+nw) = 114; inside, cv2.resize INTER_LINEAR of the uint8 source, bit-exact,
+ *   or a plain copy when (nh, nw) == (h0, w0).  A slot with nh = 0 is all border.  W % 16 == 0, dst 16-byte aligned.
+ * yv6_rescale_boxes: Inferer.rescale((H, W), det[:, :4], (h0, w0)) followed by .round() (inferer.py:103, 173-188) on the
+ *   NMS output det [B,max_det,6] / count [B] -> out [B,max_det,6] (x1, y1, x2, y2 in source pixels, conf, cls), rows
+ *   beyond count[b] zeroed.  Reads h0, w0 of geo.  Ratio and padding are the reference's doubles, box math its fp32.
+ * ---------------------------------------------------------------------------------------------- */
+#define YV6_LB_GEO 8
+int yv6_letterbox(yv6_handle* h, const uint8_t* src, const int32_t* geo, int32_t B, int32_t H, int32_t W, uint8_t* dst,
+                  void* stream);
+int yv6_rescale_boxes(yv6_handle* h, const float* det, const int32_t* count, const int32_t* geo, int32_t B, int32_t max_det,
+                      int32_t H, int32_t W, float* out, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Training-side irregular work: target preprocessing, label assignment, fused loss.
  * Compact assignment format shared by the assigners and the loss:
  *   gt      [B,G,5] float64  (class, x1, y1, x2, y2 in pixels; pad rows = -1,0,0,0,0)

@@ -1,0 +1,153 @@
+// yv6_letterbox.cu -- the image side of the reference's Inferer around the model, for a whole batch per launch:
+//   yv6_letterbox:      letterbox (yolov6/data/data_augment.py:29-58, auto=False) + HWC->CHW + BGR->RGB of
+//                       Inferer.process_image (core/inferer.py:161-171); the 1/255 stays in the stem kernel.
+//   yv6_rescale_boxes:  Inferer.rescale (core/inferer.py:173-188) followed by the `.round()` of inferer.py:103.
+//
+// Resampling is OpenCV's uint8 INTER_LINEAR path of cv2.resize, reproduced bit for bit:
+//   - source coordinate fx = (float)((dx + 0.5) * scale - 0.5) in DOUBLE, scale = 1 / (dst / src) (cv::resize keeps the
+//     inverse scale and inverts it), sx = floor(fx), fx -= sx in float;
+//   - horizontal: a border tap (sx < 0 or sx >= w0 - 1) is clamped AND gets fx = 0; coefficients
+//     saturate_cast<short>((1 - fx) * 2048), saturate_cast<short>(fx * 2048) (round half to even); S = s0*a0 + s1*a1;
+//   - vertical: the row indices sy, sy + 1 are clamped to [0, h0) but fy is NOT reset at the borders, so an upscaled
+//     image's first / last rows blend one row with itself at uneven weights -- which the truncating vertical pass below
+//     does not always map back to that row's value;
+//   - vertical pass of the SIMD kernel (VResizeLinearVec_32s8u): ((b0*(S0>>4))>>16) + ((b1*(S1>>4))>>16) + 2) >> 2.
+// The double-precision coordinate and the unreset vertical fraction are what a float32 restatement with clamped fy gets
+// wrong on upscaling shapes.  Every float / double operation is an explicit round-to-nearest intrinsic, so ptxas cannot
+// contract it into an FMA.
+#include "yv6_common.cuh"
+#include "yv6_handle.h"
+
+namespace yv6 {
+
+constexpr int kLbPix = 16;     // output pixels per thread: one 16-byte store into each channel plane
+
+struct LinTap {
+  int s0, s1, c0, c1;
+};
+
+// One axis of cv::resize's INTER_LINEAR coefficient table for destination index d.
+__device__ __forceinline__ LinTap lin_tap(int d, double scale, int src, bool reset_border) {
+  const float f = __double2float_rn(__dsub_rn(__dmul_rn(__dadd_rn((double)d, 0.5), scale), 0.5));
+  int s = (int)floorf(f);
+  float fr = __fsub_rn(f, (float)s);
+  if (reset_border) {
+    if (s < 0) fr = 0.f, s = 0;
+    if (s >= src - 1) fr = 0.f, s = src - 1;
+  }
+  LinTap t;
+  t.c0 = __float2int_rn(__fmul_rn(__fsub_rn(1.f, fr), 2048.f));
+  t.c1 = __float2int_rn(__fmul_rn(fr, 2048.f));
+  t.s0 = min(max(s, 0), src - 1);
+  t.s1 = min(max(s + 1, 0), src - 1);
+  return t;
+}
+
+// geo [B][YV6_LB_GEO] = (src_off, h0, w0, nh, nw, top, left, 0); thread = 16 consecutive pixels of one canvas row.
+__global__ void __launch_bounds__(256) letterbox_kernel(const uint8_t* __restrict__ src, const int32_t* __restrict__ geo, int H, int W,
+                                                        uint8_t* __restrict__ dst) {
+  const int b = blockIdx.y;
+  const int per_row = W / kLbPix;
+  const int q = blockIdx.x * blockDim.x + threadIdx.x;
+  if (q >= H * per_row) return;
+  const int y = q / per_row, x0 = (q - y * per_row) * kLbPix;
+  const int32_t* g = geo + b * YV6_LB_GEO;
+  const int off = __ldg(g + 0), h0 = __ldg(g + 1), w0 = __ldg(g + 2), nh = __ldg(g + 3), nw = __ldg(g + 4), top = __ldg(g + 5),
+            left = __ldg(g + 6);
+  const uint8_t* im = src + off;
+  alignas(16) uint8_t o[3][kLbPix];
+  const int ys = y - top;
+  if (ys < 0 || ys >= nh) {
+#pragma unroll
+    for (int i = 0; i < kLbPix; ++i) o[0][i] = o[1][i] = o[2][i] = 114;
+  } else if (nh == h0 && nw == w0) {           // data_augment.py:52: no resize, a plain copy
+    const uint8_t* row = im + (int64_t)ys * w0 * 3;
+#pragma unroll
+    for (int i = 0; i < kLbPix; ++i) {
+      const int xs = x0 + i - left;
+      const bool in = xs >= 0 && xs < nw;
+#pragma unroll
+      for (int c = 0; c < 3; ++c) o[c][i] = in ? __ldg(row + xs * 3 + 2 - c) : (uint8_t)114;
+    }
+  } else {
+    const double sy_scale = __ddiv_rn(1.0, __ddiv_rn((double)nh, (double)h0));
+    const double sx_scale = __ddiv_rn(1.0, __ddiv_rn((double)nw, (double)w0));
+    const LinTap v = lin_tap(ys, sy_scale, h0, false);
+    const uint8_t* r0 = im + (int64_t)v.s0 * w0 * 3;
+    const uint8_t* r1 = im + (int64_t)v.s1 * w0 * 3;
+#pragma unroll
+    for (int i = 0; i < kLbPix; ++i) {
+      const int xs = x0 + i - left;
+      if (xs < 0 || xs >= nw) {
+        o[0][i] = o[1][i] = o[2][i] = 114;
+        continue;
+      }
+      const LinTap hz = lin_tap(xs, sx_scale, w0, true);
+#pragma unroll
+      for (int c = 0; c < 3; ++c) {
+        const int ch = 2 - c;                  // BGR -> RGB
+        const int S0 = __ldg(r0 + hz.s0 * 3 + ch) * hz.c0 + __ldg(r0 + hz.s1 * 3 + ch) * hz.c1;
+        const int S1 = __ldg(r1 + hz.s0 * 3 + ch) * hz.c0 + __ldg(r1 + hz.s1 * 3 + ch) * hz.c1;
+        const int t = (((v.c0 * (S0 >> 4)) >> 16) + ((v.c1 * (S1 >> 4)) >> 16) + 2) >> 2;
+        o[c][i] = (uint8_t)min(max(t, 0), 255);
+      }
+    }
+  }
+  const int64_t plane = (int64_t)H * W;
+  uint8_t* d = dst + (int64_t)b * 3 * plane + (int64_t)y * W + x0;
+#pragma unroll
+  for (int c = 0; c < 3; ++c) *reinterpret_cast<uint4*>(d + c * plane) = *reinterpret_cast<const uint4*>(o[c]);
+}
+
+// Inferer.rescale(img.shape[2:], det[:, :4], img_src.shape).round(): ratio and padding are the reference's Python doubles,
+// the box arithmetic is torch's fp32 (x - (float)pad) / (float)ratio, clamp to the source image, round half to even.
+// Rows beyond count[b] are zeroed.
+__global__ void rescale_boxes_kernel(const float* __restrict__ det, const int32_t* __restrict__ count, const int32_t* __restrict__ geo,
+                                     int B, int max_det, int H, int W, float* __restrict__ out) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= B * max_det) return;
+  const int b = i / max_det, j = i - b * max_det;
+  float* o = out + (int64_t)i * 6;
+  if (j >= count[b]) {
+    o[0] = o[1] = o[2] = o[3] = o[4] = o[5] = 0.f;
+    return;
+  }
+  const double h0 = geo[b * YV6_LB_GEO + 1], w0 = geo[b * YV6_LB_GEO + 2];
+  const double ratio = fmin(__ddiv_rn((double)H, h0), __ddiv_rn((double)W, w0));                 // inferer.py:176
+  const float pad_x = __double2float_rn(__ddiv_rn(__dsub_rn((double)W, __dmul_rn(w0, ratio)), 2.0));   // :177
+  const float pad_y = __double2float_rn(__ddiv_rn(__dsub_rn((double)H, __dmul_rn(h0, ratio)), 2.0));
+  const float rf = __double2float_rn(ratio), wf = (float)w0, hf = (float)h0;
+  const float* r = det + (int64_t)i * 6;
+  o[0] = rintf(fminf(fmaxf(__fdiv_rn(__fsub_rn(r[0], pad_x), rf), 0.f), wf));
+  o[1] = rintf(fminf(fmaxf(__fdiv_rn(__fsub_rn(r[1], pad_y), rf), 0.f), hf));
+  o[2] = rintf(fminf(fmaxf(__fdiv_rn(__fsub_rn(r[2], pad_x), rf), 0.f), wf));
+  o[3] = rintf(fminf(fmaxf(__fdiv_rn(__fsub_rn(r[3], pad_y), rf), 0.f), hf));
+  o[4] = r[4];
+  o[5] = r[5];
+}
+
+}  // namespace yv6
+
+using namespace yv6;
+
+extern "C" int yv6_letterbox(yv6_handle* h, const uint8_t* src, const int32_t* geo, int32_t B, int32_t H, int32_t W, uint8_t* dst,
+                             void* stream) {
+  yv6_device_guard _dev(h);
+  YV6_REQUIRE(h && src && geo && dst && B > 0 && H > 0 && W > 0, "letterbox: bad argument");
+  YV6_REQUIRE(W % kLbPix == 0 && ((uintptr_t)dst & 15) == 0, "letterbox: W (%d) must be a multiple of 16 and dst 16-byte aligned", W);
+  YV6_REQUIRE(B <= 65535, "letterbox: batch %d too large", B);
+  const int chunks = H * (W / kLbPix);
+  letterbox_kernel<<<dim3((chunks + 255) / 256, B), 256, 0, (cudaStream_t)stream>>>(src, geo, H, W, dst);
+  YV6_CHECK_CUDA(cudaGetLastError());
+  return YV6_OK;
+}
+
+extern "C" int yv6_rescale_boxes(yv6_handle* h, const float* det, const int32_t* count, const int32_t* geo, int32_t B, int32_t max_det,
+                                 int32_t H, int32_t W, float* out, void* stream) {
+  yv6_device_guard _dev(h);
+  YV6_REQUIRE(h && det && count && geo && out && B > 0 && max_det > 0 && H > 0 && W > 0, "rescale_boxes: bad argument");
+  const int total = B * max_det;
+  rescale_boxes_kernel<<<(total + 255) / 256, 256, 0, (cudaStream_t)stream>>>(det, count, geo, B, max_det, H, W, out);
+  YV6_CHECK_CUDA(cudaGetLastError());
+  return YV6_OK;
+}

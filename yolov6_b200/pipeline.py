@@ -11,23 +11,54 @@ launches and all Python/ctypes work disappear from the steady state (SURVEY.md 8
 stream instead: with two pipelines used alternately (see `DetectRing`) the copy of batch i+1 runs on the
 copy engine while the kernels of batch i run on the SMs, so a serving loop is bound by max(copy, compute)
 instead of their sum.
+
+`raw_input=True` serves decoded frames (OpenCV `imread` layout: uint8 HWC BGR, any size, sizes mixed freely within a batch) instead
+of letterboxed batches: the frames' bytes and a per-image geometry table go through a fixed-capacity pinned staging buffer
+(`max_src_bytes`) and are copied to the device on the copy stream, and the graph runs letterbox -> network -> NMS -> rescale
+-> D2H (`yolov6_b200.preprocess`).  Results are per-image [k, 6] rows in source pixels, what `Inferer.infer` holds in `det` after
+core/inferer.py:103.  The geometry is data, so one captured graph serves any mix of image sizes.
 """
 import torch
 
 from .nms import nms_batched_head, workspace_bytes
+from .preprocess import GEO, letterbox_launch, pack_frames, rescale_launch
+
+RAW_DEFAULT_BYTES = 1920 * 1080 * 3        # staging bytes per batch slot when max_src_bytes is not given: one 1080p frame each
+
+
+def raw_buffers(batch, height, width, max_det, max_src_bytes, dev):
+    """Pinned staging + device buffers of one raw-frame slot."""
+    cap = int(max_src_bytes) if max_src_bytes else batch * RAW_DEFAULT_BYTES
+    geo = torch.tensor([[0, height, width, 0, 0, 0, 0, 0]] * batch, dtype=torch.int32)     # all border until frames arrive
+    return dict(src_host=torch.empty(cap, dtype=torch.uint8).pin_memory(), geo_host=geo.pin_memory(),
+                src_dev=torch.zeros(cap, dtype=torch.uint8, device=dev), geo_dev=geo.to(dev), res_geo=geo.to(dev),
+                res=torch.zeros(batch, max_det, 6, device=dev), nbytes=0)
+
+
+def raw_h2d(slot):
+    """Copy the used staging bytes and the geometry of one raw-frame slot to the device (current stream)."""
+    n = slot["nbytes"]
+    if n:
+        slot["src_dev"][:n].copy_(slot["src_host"][:n], non_blocking=True)
+    slot["geo_dev"].copy_(slot["geo_host"], non_blocking=True)
 
 
 class DetectPipeline:
     def __init__(self, model, batch, height, width, conf_thres=0.25, iou_thres=0.45, classes=None, agnostic=False,
-                 multi_label=False, max_det=300, host_input=True, overlap_h2d=False, copy_stream=None):
+                 multi_label=False, max_det=300, host_input=True, overlap_h2d=False, copy_stream=None, raw_input=False,
+                 max_src_bytes=None):
         self.model = model.eval()
         self.dev = next(model.parameters()).device
         if self.dev.type != "cuda":
             raise RuntimeError("DetectPipeline needs a CUDA model")
+        if raw_input and not host_input:
+            raise RuntimeError("DetectPipeline: raw_input takes host frames (host_input=True)")
         self.kw = dict(conf_thres=conf_thres, iou_thres=iou_thres, classes=classes, agnostic=agnostic,
                        multi_label=multi_label, max_det=max_det)
         self.host_input = host_input
-        self.overlap_h2d = bool(overlap_h2d and host_input)
+        self.raw = raw_input and raw_buffers(batch, height, width, max_det, max_src_bytes, self.dev)
+        self.n_frames = batch
+        self.overlap_h2d = bool((overlap_h2d or raw_input) and host_input)
         if self.overlap_h2d:
             self.copy_stream = copy_stream or torch.cuda.Stream(device=self.dev)
             self.ev_copied = torch.cuda.Event()
@@ -35,7 +66,7 @@ class DetectPipeline:
             self._used = False
         dt = torch.uint8 if host_input else torch.float32
         self.x_dev = torch.zeros(batch, 3, height, width, dtype=dt, device=self.dev)
-        self.x_host = torch.zeros(batch, 3, height, width, dtype=torch.uint8).pin_memory() if host_input else None
+        self.x_host = torch.zeros(batch, 3, height, width, dtype=torch.uint8).pin_memory() if host_input and not self.raw else None
         self.out_host = torch.zeros(batch, max_det, 6).pin_memory()
         self.count_host = torch.zeros(batch + 1, dtype=torch.int32).pin_memory()
         self.eng = model.engine()
@@ -48,12 +79,16 @@ class DetectPipeline:
         self._warm()
 
     def _body(self):
-        if self.host_input and not self.overlap_h2d:
+        if self.raw:
+            letterbox_launch(self.raw["src_dev"], self.raw["geo_dev"], self.x_dev)
+        elif self.host_input and not self.overlap_h2d:
             self.x_dev.copy_(self.x_host, non_blocking=True)
         # the [B, A, 5+nc] prediction tensor of Detect.forward (effidehead.py:131-139) is never materialised here: the NMS
         # kernels scan the class scores where the cls_pred convs wrote them and decode boxes for the candidates only
         cls, reg, sizes = self.eng.forward(self.x_dev, decode=False)
         out, count, src, overflow = nms_batched_head(cls, reg, sizes, self.model.graph.strides, workspace=self.nms_ws, **self.kw)
+        if self.raw:
+            out = rescale_launch(out, count, self.raw["geo_dev"], self.x_dev.shape[2], self.x_dev.shape[3], res=self.raw["res"])
         self.out_dev, self.count_dev = out, count
         if self.host_input:
             self.out_host.copy_(out, non_blocking=True)
@@ -79,7 +114,10 @@ class DetectPipeline:
             if self._used:
                 self.copy_stream.wait_event(self.ev_done)      # the previous batch of THIS pipeline is done with x_dev
             with torch.cuda.stream(self.copy_stream):
-                self.x_dev.copy_(self.x_host, non_blocking=True)
+                if self.raw:
+                    raw_h2d(self.raw)
+                else:
+                    self.x_dev.copy_(self.x_host, non_blocking=True)
                 self.ev_copied.record(self.copy_stream)
             cur.wait_event(self.ev_copied)
             self.graph.replay()
@@ -89,17 +127,23 @@ class DetectPipeline:
         self.graph.replay()
 
     def __call__(self, images=None):
-        """images: uint8 [B,3,H,W] host tensor (host_input) or fp32 device tensor.  Returns the list of
-        per-image [k,6] detections (host tensors when host_input) like `non_max_suppression`."""
+        """images: uint8 [B,3,H,W] host tensor (host_input) or fp32 device tensor; with raw_input, a list of 1..B uint8 HWC BGR
+        frames (numpy arrays or CPU tensors).  Returns the list of per-image [k,6] detections (host tensors when host_input)
+        like `non_max_suppression`; with raw_input in source pixels, rounded (Inferer.rescale(...).round())."""
         if images is not None:
-            (self.x_host if self.host_input else self.x_dev).copy_(images)
+            if self.raw:
+                self.raw["nbytes"], _ = pack_frames(images, self.x_dev.shape[0], self.x_dev.shape[2], self.x_dev.shape[3], True,
+                                                    self.raw["src_host"], self.raw["geo_host"])
+                self.n_frames = len(images)
+            else:
+                (self.x_host if self.host_input else self.x_dev).copy_(images)
         self.launch()
         torch.cuda.current_stream(self.dev).synchronize()
         if self.host_input:
             counts = self.count_host.tolist()
             if counts[-1]:
                 raise RuntimeError("non_max_suppression: more than 65536 near-identical candidate scores in one image; raise conf_thres")
-            return [self.out_host[i, :counts[i]].clone() for i in range(self.out_host.shape[0])]
+            return [self.out_host[i, :counts[i]].clone() for i in range(self.n_frames)]
         counts = self.count_dev.tolist()
         return [self.out_dev[i, :counts[i]] for i in range(self.out_dev.shape[0])]
 
@@ -153,21 +197,29 @@ class DetectStream:
 
     host_input=True: uint8 images come from pinned host memory (H2D of batch i + 1 on a copy stream under the kernels of
     batch i, as in DetectRing) and detections go back to pinned host memory inside the NMS branch.
+
+    raw_input=True: `submit(frames)` takes 1..B decoded uint8 HWC BGR frames of any sizes (see the module docstring); the step
+    graph letterboxes them before the network and the NMS branch rescales the previous batch's rows to its source pixels.
     """
 
     def __init__(self, model, batch, height, width, conf_thres=0.25, iou_thres=0.45, classes=None, agnostic=False,
-                 multi_label=False, max_det=300, host_input=True, engine=None):
+                 multi_label=False, max_det=300, host_input=True, engine=None, raw_input=False, max_src_bytes=None):
         self.model = model.eval()
         self.dev = next(model.parameters()).device
         if self.dev.type != "cuda":
             raise RuntimeError("DetectStream needs a CUDA model")
+        if raw_input and not host_input:
+            raise RuntimeError("DetectStream: raw_input takes host frames (host_input=True)")
         self.kw = dict(conf_thres=conf_thres, iou_thres=iou_thres, classes=classes, agnostic=agnostic,
                        multi_label=multi_label, max_det=max_det)
         self.host_input = bool(host_input)
         self.B = batch
         dt = torch.uint8 if host_input else torch.float32
         self.x_dev = [torch.zeros(batch, 3, height, width, dtype=dt, device=self.dev) for _ in range(2)]
-        self.x_host = [torch.zeros(batch, 3, height, width, dtype=torch.uint8).pin_memory() for _ in range(2)] if host_input else None
+        self.raw = [raw_buffers(batch, height, width, max_det, max_src_bytes, self.dev) for _ in range(2)] if raw_input else None
+        self.n_frames = {}        # batch number -> frames in it (raw_input)
+        self.x_host = ([torch.zeros(batch, 3, height, width, dtype=torch.uint8).pin_memory() for _ in range(2)]
+                       if host_input and not raw_input else None)
         self.out_host = [torch.zeros(batch, max_det, 6).pin_memory() for _ in range(2)]
         self.count_host = [torch.zeros(batch + 1, dtype=torch.int32).pin_memory() for _ in range(2)]
         self.dev_step, self.dev_drain = {}, {}      # head set -> (out, count, overflow) device tensors of the step / drain graphs
@@ -195,6 +247,10 @@ class DetectStream:
         cls = plan["cls_alt"] if k == 1 else plan["cls"]
         reg = plan["reg_alt"] if k == 1 else plan["reg"]
         out, count, src, overflow = nms_batched_head(cls, reg, plan["sizes"], self.model.graph.strides, workspace=self.nms_ws, **self.kw)
+        if self.raw:
+            # res_geo[k] is the geometry of the batch whose network wrote head set k: the copy stream may already be refilling
+            # geo_dev[k] with the batch after next
+            out = rescale_launch(out, count, self.raw[k]["res_geo"], self.x_dev[k].shape[2], self.x_dev[k].shape[3], res=self.raw[k]["res"])
         store[k] = (out, count, overflow)
         if self.host_input:
             self.out_host[k].copy_(out, non_blocking=True)
@@ -216,14 +272,21 @@ class DetectStream:
         # (forking at the start of the step gains 2 %, measured).
         plan = self.eng._plan(self.B, self.x_dev[0].shape[2], self.x_dev[0].shape[3], self.x_dev[0].dtype)
         at = plan.get("neck_start", 0) if self.fork_at_neck else 0
+        self._letterbox(k)
         self.eng.forward(self.x_dev[k], decode=False, head_set=k, hook=(at, fork))
         cur.wait_event(self.ev_join)
+
+    def _letterbox(self, k):
+        if self.raw:
+            letterbox_launch(self.raw[k]["src_dev"], self.raw[k]["geo_dev"], self.x_dev[k])
+            self.raw[k]["res_geo"].copy_(self.raw[k]["geo_dev"])
 
     def _build(self):
         s = torch.cuda.Stream(device=self.dev)
         s.wait_stream(torch.cuda.current_stream(self.dev))
         with torch.cuda.stream(s), torch.no_grad():
             for k in (0, 1, 0, 1):     # both head sets exist and hold valid scores before anything is captured
+                self._letterbox(k)
                 self.eng.forward(self.x_dev[k], decode=False, head_set=k)
                 self._nms(k, {})
         torch.cuda.current_stream(self.dev).wait_stream(s)
@@ -244,7 +307,10 @@ class DetectStream:
             if self.steps >= 2:
                 self.copy_stream.wait_event(self.ev_done[k])   # the step that last read x_dev[k] has finished
             with torch.cuda.stream(self.copy_stream):
-                self.x_dev[k].copy_(self.x_host[k], non_blocking=True)
+                if self.raw:
+                    raw_h2d(self.raw[k])
+                else:
+                    self.x_dev[k].copy_(self.x_host[k], non_blocking=True)
                 self.ev_copied[k].record(self.copy_stream)
             cur.wait_event(self.ev_copied[k])
         self.graphs[k].replay()
@@ -260,18 +326,23 @@ class DetectStream:
         if self.host_input:
             if self.steps >= 2:
                 self.ev_done[k].synchronize()                  # x_host[k] was copied by the step two submissions ago
-            self.x_host[k].copy_(images)
+            if self.raw:
+                self.raw[k]["nbytes"], _ = pack_frames(images, self.B, self.x_dev[k].shape[2], self.x_dev[k].shape[3], True,
+                                                       self.raw[k]["src_host"], self.raw[k]["geo_host"])
+                self.n_frames[self.steps] = len(images)
+            else:
+                self.x_host[k].copy_(images)
         else:
             self.x_dev[k].copy_(images)
         self._drained = False
         self.launch()
 
-    def _results(self, k, store):
+    def _results(self, k, store, n):
         if self.host_input:
             counts = self.count_host[k].tolist()
             if counts[-1]:
                 raise RuntimeError("non_max_suppression: more than 65536 near-identical candidate scores in one image; raise conf_thres")
-            return [self.out_host[k][j, :counts[j]].clone() for j in range(self.B)]
+            return [self.out_host[k][j, :counts[j]].clone() for j in range(n)]
         out, count, overflow = store[k]
         if int(overflow.item()):
             raise RuntimeError("non_max_suppression: more than 65536 near-identical candidate scores in one image; raise conf_thres")
@@ -293,7 +364,7 @@ class DetectStream:
         else:
             return None
         self.collected += 1
-        return self._results(t & 1, store)
+        return self._results(t & 1, store, self.n_frames.pop(t, self.B))
 
     def drain(self):
         """NMS of the last submitted batch (nothing follows it in the pipeline)."""
