@@ -367,9 +367,17 @@ __global__ void __launch_bounds__(kTrThreads, 2) bn_bwd_reduce_kernel(const BwdP
 #pragma unroll
   for (int b = 0; b < NB; ++b) block_colsum(m, p.C, t[b], red, p.work + (size_t)b * p.C);
   if (p.dalpha != nullptr) {
+    // the block is cgs * rows threads, not always whole warps (C = 384: 240 threads, the last warp has 16 lanes): shuffle
+    // among the lanes that exist only.  Lane 0 adds the same pairs in the same order as a full-warp xor butterfly would.
+    const int lane = threadIdx.x & 31;
+    const int lanes = min(32, (int)blockDim.x - (int)(threadIdx.x & ~31u));
+    const unsigned mask = (lanes == 32) ? 0xffffffffu : ((1u << lanes) - 1u);
 #pragma unroll
-    for (int o = 16; o > 0; o >>= 1) da += __shfl_xor_sync(0xffffffffu, da, o);
-    if ((threadIdx.x & 31) == 0) atomicAdd(p.dalpha, (double)da);
+    for (int o = 16; o > 0; o >>= 1) {
+      const float other = __shfl_down_sync(mask, da, o);
+      if (lane + o < lanes) da += other;
+    }
+    if (lane == 0) atomicAdd(p.dalpha, (double)da);
   }
   if (!last_block_done(p.counter)) return;
   for (int i = threadIdx.x; i < NB * p.C; i += blockDim.x) {
