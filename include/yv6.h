@@ -217,6 +217,40 @@ int yv6_rescale_boxes(yv6_handle* h, const float* det, const int32_t* count, con
                       int32_t H, int32_t W, float* out, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Training augmentation from decoded frames: TrainValDataset.__getitem__ (yolov6/data/datasets.py:166-255) with
+ * augment=True for a whole batch, bit-exact against the cv2 calls it makes.  All images live in one device byte arena
+ * `base` (uint8 HWC BGR, packed); every offset below is a byte offset into it.  yolov6_b200/augment.py builds the tables.
+ *
+ * yv6_aug_resize: jobs [J][YV6_AUG_JOB] int64 = (src_off, h0, w0, dst_off, nh, nw, 0, 0): cv2.resize(INTER_LINEAR) of
+ *   each source to nh x nw (a plain copy when the sizes are equal).  One launch serves load_image's resize of every source
+ *   of a batch; a second launch over its results serves the letterbox branch's resize.  max_pix >= every nh * nw.
+ * yv6_augment: samples [B] (yv6_aug_sample, device) -> dst uint8 NCHW RGB [B,3,H,W].  Per output pixel: the flips as an
+ *   index remap, then for each canvas cv2.warpAffine's INTER_LINEAR / BORDER_CONSTANT 114 sample of a virtual canvas --
+ *   a 114 background of ch x cw with ntile placed rectangles, later tiles over earlier ones -- the fp64 mixup blend, and
+ *   augment_hsv's BGR -> HSV -> LUT -> BGR.  W % 32 == 0 (OpenCV's vector HSV path then covers whole rows), dst
+ *   16-byte aligned.
+ * ---------------------------------------------------------------------------------------------- */
+#define YV6_AUG_JOB 8
+typedef struct {
+  int64_t org;                 /* arena offset of canvas pixel (0, 0) in this tile's image (may lie outside the image) */
+  int32_t pitch;               /* image width in pixels */
+  int32_t y0, y1, x0, x1;      /* the tile's canvas rectangle [y0, y1) x [x0, x1) */
+  int32_t pad;
+} yv6_aug_tile;
+typedef struct {
+  double minv[2][6];           /* per canvas: M[:2] inverted as cv::warpAffine inverts it (dst -> canvas) */
+  double mix_r;                /* mixup: trunc(c0 * r + c1 * (1 - r)) in fp64 */
+  yv6_aug_tile tile[2][4];
+  int32_t ch[2], cw[2];        /* canvas sizes */
+  int32_t ntile[2];
+  int32_t mixup, hsv, flipud, fliplr;
+  uint8_t lut[3][256];         /* augment_hsv's hue, saturation and value tables */
+} yv6_aug_sample;
+int yv6_aug_resize(yv6_handle* h, uint8_t* base, const int64_t* jobs, int32_t J, int64_t max_pix, void* stream);
+int yv6_augment(yv6_handle* h, const uint8_t* base, const yv6_aug_sample* samples, int32_t B, int32_t H, int32_t W, uint8_t* dst,
+                void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Training-side irregular work: target preprocessing, label assignment, fused loss.
  * Compact assignment format shared by the assigners and the loss:
  *   gt      [B,G,5] float64  (class, x1, y1, x2, y2 in pixels; pad rows = -1,0,0,0,0)

@@ -1,0 +1,485 @@
+"""Training augmentation on the device: decoded frames in, the `TrainStep` batch out.
+
+The reference builds every training sample on the host in `TrainValDataset.__getitem__` (yolov6/data/datasets.py:166-255):
+`load_image`'s INTER_LINEAR resize, a 2H x 2W mosaic canvas (or a letterbox), `random_affine`'s cv2.warpAffine, mixup,
+`augment_hsv`'s BGR -> HSV -> LUT -> BGR round trip and the flips.  Here that work is split three ways:
+
+  - `Sampler` draws every random number the reference draws, in the reference's order, from the same generators (Python's
+    global `random` and numpy's global `np.random`), and returns one plain-data `Sample` per image.  A training script that
+    seeds those generators as the reference does gets the reference's augmentation sequence.
+  - `sample_labels` moves the labels with the reference's own float64 / float32 numpy expressions: about seven boxes per
+    image are not worth a kernel, and the same arithmetic gives the same rows.
+  - Two kernels per batch (`yv6_aug_resize`, `yv6_augment`, csrc/yv6_augment.cu) produce the pixels, bit-exact against
+    the cv2 calls above.  The canvas is never materialised: a per-sample table describes it as a 114 background with up
+    to four placed rectangles of resized sources, and the augment kernel samples it where warpAffine would.
+
+`AugmentFeed` ties them to a `TrainStep`: it stages the sources of batch i+1 in pinned memory, copies and resizes them on
+side streams while batch i's graphs run, and writes the augmented images straight into the step's static uint8 input,
+ordered by events rather than host synchronisation.  Decoding (JPEG / PNG -> pixels) stays with the caller.
+
+Not provided: `rect` batches, `specific_shape` / `shrink_size` datasets and the dataloader's worker processes.
+"""
+import ctypes as C
+import math
+import random
+from dataclasses import dataclass, field
+
+import numpy as np
+import torch
+
+from . import _lib
+from .preprocess import as_frame
+
+# yolov6/configs/*.py data_aug of the two flagship configurations
+HYP_YOLOV6S = dict(hsv_h=0.015, hsv_s=0.7, hsv_v=0.4, degrees=0.0, translate=0.1, scale=0.5, shear=0.0, flipud=0.0,
+                   fliplr=0.5, mosaic=1.0, mixup=0.0)
+HYP_YOLOV6L6 = dict(HYP_YOLOV6S, scale=0.9, mixup=0.2)
+
+@dataclass
+class Canvas:
+    """One canvas of a sample: the source indices placed on it (4 for a mosaic, 1 for a letterbox), the mosaic centre
+    (yc, xc; None for a letterbox), and get_transform_matrix's M (float64 3x3) and scale s."""
+    indices: list
+    yc: int
+    xc: int
+    M: np.ndarray
+    s: float
+
+
+@dataclass
+class Sample:
+    """Everything `__getitem__` draws for one image: the mosaic decision, one canvas (two with mixup), the mixup ratio,
+    the HSV gains (None when every gain is 0) and the two flips."""
+    index: int
+    mosaic: bool
+    canvases: list = field(default_factory=list)
+    mix_r: float = None
+    gains: np.ndarray = None
+    flipud: bool = False
+    fliplr: bool = False
+
+    def sources(self):
+        return [i for cv in self.canvases for i in cv.indices]
+
+
+def transform_matrix(img_shape, new_shape, degrees, scale, shear, translate):
+    """get_transform_matrix (data_augment.py:116-143): six random.uniform draws, always made.  cv2.getRotationMatrix2D
+    about (0, 0) is [[cos(a') s, sin(a') s], [-sin(a') s, cos(a') s]] with a' = a * (pi / 180) in double."""
+    new_height, new_width = new_shape
+    Cm = np.eye(3)
+    Cm[0, 2] = -img_shape[1] / 2
+    Cm[1, 2] = -img_shape[0] / 2
+    R = np.eye(3)
+    a = random.uniform(-degrees, degrees)
+    s = random.uniform(1 - scale, 1 + scale)
+    ang = a * (math.pi / 180)
+    alpha, beta = math.cos(ang) * s, math.sin(ang) * s
+    R[:2] = [[alpha, beta, 0.0], [-beta, alpha, 0.0]]
+    S = np.eye(3)
+    S[0, 1] = math.tan(random.uniform(-shear, shear) * math.pi / 180)
+    S[1, 0] = math.tan(random.uniform(-shear, shear) * math.pi / 180)
+    T = np.eye(3)
+    T[0, 2] = random.uniform(0.5 - translate, 0.5 + translate) * new_width
+    T[1, 2] = random.uniform(0.5 - translate, 0.5 + translate) * new_height
+    M = T @ S @ R @ Cm
+    return M, s
+
+
+class Sampler:
+    """The random draws of TrainValDataset.__getitem__ with augment=True, for a dataset of `n_images` images, training
+    images of H x W and `load_image` size `img_size` (default max(H, W))."""
+
+    def __init__(self, n_images, H, W, hyp, img_size=None):
+        self.n, self.H, self.W, self.hyp = int(n_images), int(H), int(W), dict(hyp)
+        self.img_size = int(img_size or max(H, W))
+
+    def _mosaic(self, index):
+        """get_mosaic (datasets.py:452-467) + the draws of mosaic_augmentation (data_augment.py:156, 201)."""
+        indices = [index] + random.choices(range(0, self.n), k=3)
+        random.shuffle(indices)
+        yc, xc = (int(random.uniform(x // 2, 3 * x // 2)) for x in (self.H, self.W))
+        h = self.hyp
+        M, s = transform_matrix((2 * self.H, 2 * self.W), (self.H, self.W), h["degrees"], h["scale"], h["shear"], h["translate"])
+        return Canvas(indices, yc, xc, M, s)
+
+    def draw_one(self, index):
+        h = self.hyp
+        rec = Sample(int(index), random.random() < h["mosaic"])
+        if rec.mosaic:
+            rec.canvases.append(self._mosaic(index))
+            if random.random() < h["mixup"]:
+                rec.canvases.append(self._mosaic(random.randint(0, self.n - 1)))
+                rec.mix_r = float(np.random.beta(32.0, 32.0))
+        else:
+            M, s = transform_matrix((self.H, self.W), (self.H, self.W), h["degrees"], h["scale"], h["shear"], h["translate"])
+            rec.canvases.append(Canvas([int(index)], None, None, M, s))
+        if h["hsv_h"] or h["hsv_s"] or h["hsv_v"]:
+            rec.gains = np.random.uniform(-1, 1, 3) * [h["hsv_h"], h["hsv_s"], h["hsv_v"]] + 1
+        rec.flipud = random.random() < h["flipud"]
+        rec.fliplr = random.random() < h["fliplr"]
+        return rec
+
+    def draw(self, indices):
+        """One Sample per dataset index, in order.  `Plan.sources` lists the distinct source images the batch needs."""
+        return Plan([self.draw_one(i) for i in indices])
+
+
+class Plan:
+    """The records of one batch and the distinct source indices they read, in first-use order."""
+
+    def __init__(self, samples):
+        self.samples = samples
+        self.sources = list(dict.fromkeys(i for s in samples for i in s.sources()))
+
+
+def resized_shape(h0, w0, img_size):
+    """load_image's size (datasets.py:287-295): (int(h0 * r), int(w0 * r)) with r = img_size / max(h0, w0), or (h0, w0)."""
+    ratio = img_size / max(h0, w0)
+    if ratio == 1:
+        return h0, w0
+    return int(h0 * ratio), int(w0 * ratio)
+
+
+def letterbox_fit(h, w, H, W):
+    """letterbox(..., auto=False, scaleup=True) of an h x w image on H x W: (r, (nw, nh), (left, top))."""
+    r = min(H / h, W / w)
+    nw, nh = int(round(w * r)), int(round(h * r))
+    dw, dh = (W - nw) / 2, (H - nh) / 2
+    return r, (nw, nh), (int(round(dw - 0.1)), int(round(dh - 0.1)))
+
+
+def box_candidates(box1, box2, wh_thr=2, ar_thr=20, area_thr=0.1, eps=1e-16):
+    """data_augment.py:69-74."""
+    w1, h1 = box1[2] - box1[0], box1[3] - box1[1]
+    w2, h2 = box2[2] - box2[0], box2[3] - box2[1]
+    ar = np.maximum(w2 / (h2 + eps), h2 / (w2 + eps))
+    return (w2 > wh_thr) & (h2 > wh_thr) & (w2 * h2 / (w1 * h1 + eps) > area_thr) & (ar < ar_thr)
+
+
+def _affine_labels(labels, M, s, height, width):
+    """The label half of random_affine (data_augment.py:90-111)."""
+    n = len(labels)
+    if n:
+        xy = np.ones((n * 4, 3))
+        xy[:, :2] = labels[:, [1, 2, 3, 4, 1, 4, 3, 2]].reshape(n * 4, 2)
+        xy = xy @ M.T
+        xy = xy[:, :2].reshape(n, 8)
+        x = xy[:, [0, 2, 4, 6]]
+        y = xy[:, [1, 3, 5, 7]]
+        new = np.concatenate((x.min(1), y.min(1), x.max(1), y.max(1))).reshape(4, n).T
+        new[:, [0, 2]] = new[:, [0, 2]].clip(0, width)
+        new[:, [1, 3]] = new[:, [1, 3]].clip(0, height)
+        i = box_candidates(box1=labels[:, 1:5].T * s, box2=new.T, area_thr=0.1)
+        labels = labels[i]
+        labels[:, 1:5] = new[i]
+    return labels
+
+
+def _canvas_labels(rec, cv, hw, labels, H, W):
+    """Pixel-space labels of one canvas after its affine: mosaic_augmentation (data_augment.py:158-206) or the letterbox
+    branch of __getitem__ (datasets.py:196-229)."""
+    if rec.mosaic:
+        tiles = _tiles(hw, cv.yc, cv.xc, H, W)
+        labels4 = []
+        for (h, w), (y1a, _, x1a, _, y1b, x1b), lab in zip(hw, tiles, labels):
+            padw, padh = x1a - x1b, y1a - y1b
+            lab = lab.copy()
+            if lab.size:
+                boxes = np.copy(lab[:, 1:])
+                boxes[:, 0] = w * (lab[:, 1] - lab[:, 3] / 2) + padw
+                boxes[:, 1] = h * (lab[:, 2] - lab[:, 4] / 2) + padh
+                boxes[:, 2] = w * (lab[:, 1] + lab[:, 3] / 2) + padw
+                boxes[:, 3] = h * (lab[:, 2] + lab[:, 4] / 2) + padh
+                lab[:, 1:] = boxes
+            labels4.append(lab)
+        labels4 = np.concatenate(labels4, 0)
+        labels4[:, 1::2] = np.clip(labels4[:, 1::2], 0, 2 * W)
+        labels4[:, 2::2] = np.clip(labels4[:, 2::2], 0, 2 * H)
+        return _affine_labels(labels4, cv.M, cv.s, H, W)
+    (h, w), lab = hw[0], labels[0].copy()
+    ratio, _, pad = letterbox_fit(h, w, H, W)
+    if H != W:
+        # a non-square shape reaches __getitem__ only as a numpy row of batch_shapes, which makes the ratio a numpy
+        # float64 and so the box arithmetic below float64 instead of float32
+        ratio = np.float64(ratio)
+    if lab.size:
+        w *= ratio
+        h *= ratio
+        boxes = np.copy(lab[:, 1:])
+        boxes[:, 0] = w * (lab[:, 1] - lab[:, 3] / 2) + pad[0]
+        boxes[:, 1] = h * (lab[:, 2] - lab[:, 4] / 2) + pad[1]
+        boxes[:, 2] = w * (lab[:, 1] + lab[:, 3] / 2) + pad[0]
+        boxes[:, 3] = h * (lab[:, 2] + lab[:, 4] / 2) + pad[1]
+        lab[:, 1:] = boxes
+    return _affine_labels(lab, cv.M, cv.s, H, W)
+
+
+def sample_labels(rec, shapes, labels, H, W, img_size):
+    """labels_out of __getitem__ (float32 [n, 6], column 0 zero) for a Sample, from the decoded sources' (h0, w0) and
+    their YOLO-format labels (float32 [k, 5]: cls, cx, cy, w, h normalised), both keyed by source index."""
+    out = []
+    for cv in rec.canvases:
+        hw = [resized_shape(*shapes[i], img_size) for i in cv.indices]
+        out.append(_canvas_labels(rec, cv, hw, [labels[i] for i in cv.indices], H, W))
+    lab = np.concatenate(out, 0) if len(out) > 1 else out[0]
+    if len(lab):
+        h, w = H, W
+        lab[:, [1, 3]] = lab[:, [1, 3]].clip(0, w - 1e-3)
+        lab[:, [2, 4]] = lab[:, [2, 4]].clip(0, h - 1e-3)
+        boxes = np.copy(lab[:, 1:])
+        boxes[:, 0] = ((lab[:, 1] + lab[:, 3]) / 2) / w
+        boxes[:, 1] = ((lab[:, 2] + lab[:, 4]) / 2) / h
+        boxes[:, 2] = (lab[:, 3] - lab[:, 1]) / w
+        boxes[:, 3] = (lab[:, 4] - lab[:, 2]) / h
+        lab[:, 1:] = boxes
+    if rec.flipud and len(lab):
+        lab[:, 2] = 1 - lab[:, 2]
+    if rec.fliplr and len(lab):
+        lab[:, 1] = 1 - lab[:, 1]
+    labels_out = torch.zeros((len(lab), 6))
+    if len(lab):
+        labels_out[:, 1:] = torch.from_numpy(lab)
+    return labels_out
+
+
+def _tiles(hw, yc, xc, H, W):
+    """mosaic placement (data_augment.py:162-175) of four h x w tiles: (y1a, y2a, x1a, x2a, y1b, x1b) each."""
+    out = []
+    for i, (h, w) in enumerate(hw):
+        if i == 0:
+            x1a, y1a, x2a, y2a = max(xc - w, 0), max(yc - h, 0), xc, yc
+            x1b, y1b = w - (x2a - x1a), h - (y2a - y1a)
+        elif i == 1:
+            x1a, y1a, x2a, y2a = xc, max(yc - h, 0), min(xc + w, W * 2), yc
+            x1b, y1b = 0, h - (y2a - y1a)
+        elif i == 2:
+            x1a, y1a, x2a, y2a = max(xc - w, 0), yc, xc, min(H * 2, yc + h)
+            x1b, y1b = w - (x2a - x1a), 0
+        else:
+            x1a, y1a, x2a, y2a = xc, yc, min(xc + w, W * 2), min(H * 2, yc + h)
+            x1b, y1b = 0, 0
+        out.append((y1a, y2a, x1a, x2a, y1b, x1b))
+    return out
+
+
+def check_labels(lab, where):
+    """YOLO-format label rows of one image -> float32 [k, 5]; RuntimeError when malformed (check_label_files' rules)."""
+    a = np.asarray(lab.numpy() if isinstance(lab, torch.Tensor) else lab, dtype=np.float32)
+    if a.size == 0:
+        return np.zeros((0, 5), np.float32)
+    if a.ndim != 2 or a.shape[1] != 5:
+        raise RuntimeError(f"augment: labels of {where} must be [k, 5] (cls, cx, cy, w, h), got shape {a.shape}")
+    if not np.isfinite(a).all() or (a < 0).any() or (a[:, 1:] > 1).any():
+        raise RuntimeError(f"augment: labels of {where} must be finite, non-negative and normalised to [0, 1]")
+    return a
+
+
+# ---------------------------------------------------------------------------------------------------- the device side
+class AugTile(C.Structure):
+    """Mirror of `yv6_aug_tile` (include/yv6.h)."""
+    _fields_ = [("org", C.c_int64), ("pitch", C.c_int32), ("y0", C.c_int32), ("y1", C.c_int32), ("x0", C.c_int32),
+                ("x1", C.c_int32), ("pad", C.c_int32)]
+
+
+class AugSample(C.Structure):
+    """Mirror of `yv6_aug_sample` (include/yv6.h)."""
+    _fields_ = [("minv", (C.c_double * 6) * 2), ("mix_r", C.c_double), ("tile", (AugTile * 4) * 2),
+                ("ch", C.c_int32 * 2), ("cw", C.c_int32 * 2), ("ntile", C.c_int32 * 2),
+                ("mixup", C.c_int32), ("hsv", C.c_int32), ("flipud", C.c_int32), ("fliplr", C.c_int32),
+                ("lut", (C.c_uint8 * 256) * 3)]
+
+
+JOB = 8               # int64 per resize job (YV6_AUG_JOB)
+
+
+def invert_affine(M):
+    """cv::warpAffine's inversion of M[:2] (double), the matrix its kernel maps destination pixels with."""
+    m = [float(v) for v in np.asarray(M, np.float64)[:2].reshape(-1)]
+    D = m[0] * m[4] - m[1] * m[3]
+    D = 1.0 / D if D != 0 else 0.0
+    A11, A22 = m[4] * D, m[0] * D
+    m[0] = A11
+    m[1] *= -D
+    m[3] *= -D
+    m[4] = A22
+    b1 = -m[0] * m[2] - m[1] * m[5]
+    b2 = -m[3] * m[2] - m[4] * m[5]
+    m[2], m[5] = b1, b2
+    return m
+
+
+def hsv_luts(gains):
+    """augment_hsv's lookup tables (data_augment.py:20-23) for the drawn gains."""
+    x = np.arange(0, 256, dtype=np.float64)
+    return (((x * gains[0]) % 180).astype(np.uint8), np.clip(x * gains[1], 0, 255).astype(np.uint8),
+            np.clip(x * gains[2], 0, 255).astype(np.uint8))
+
+
+class AugmentFeed:
+    """Double-buffered device augmentation for batches of `batch` H x W training images.
+
+        feed = AugmentFeed(batch, H, W, hyp, n_images, max_src_bytes, step=train_step)
+        plan = feed.draw(indices)                    # Sampler draws; plan.sources = images to decode
+        feed.submit(plan, frames, labels)            # frames / labels keyed by source index
+        feed.wait()                                  # the current stream waits; step.images / step.targets hold the batch
+        out = train_step.run(epoch)
+
+    `submit` validates every frame (uint8 HWC, 3 channels) and label array ([k, 5] normalised) and raises RuntimeError
+    before anything is enqueued.  It then stages the sources in pinned memory, copies them on a copy stream, resizes them
+    on an augmentation stream, and writes the batch into `images` / `targets` once everything enqueued on the caller's
+    stream before the call (the previous step) is done.  The host waits only before reusing a staging slot, for the batch
+    submitted two calls earlier.  Without `step`, the feed owns `images` and `targets`."""
+
+    def __init__(self, batch, H, W, hyp, n_images, max_src_bytes, img_size=None, step=None, max_targets=None, device=None):
+        if W % 32:
+            raise RuntimeError(f"augment: W ({W}) must be a multiple of 32")
+        self.B, self.H, self.W = int(batch), int(H), int(W)
+        self.sampler = Sampler(n_images, H, W, hyp, img_size)
+        self.img_size = self.sampler.img_size
+        self.max_src = int(max_src_bytes)
+        if step is not None:
+            if (step.B, step.H, step.W) != (self.B, self.H, self.W) or step.images.dtype != torch.uint8:
+                raise RuntimeError("augment: the TrainStep must take uint8 [batch, 3, H, W] images")
+            self.dev, self.images, self.targets = step.dev, step.images, step.targets
+        else:
+            self.dev = device or torch.device("cuda", torch.cuda.current_device())
+            self.images = torch.empty(self.B, 3, H, W, dtype=torch.uint8, device=self.dev)
+            self.targets = torch.full((int(max_targets or self.B * 64), 6), -1.0, device=self.dev)
+        self.max_targets = self.targets.shape[0]
+        self.copy_stream = torch.cuda.Stream(device=self.dev)
+        self.aug_stream = torch.cuda.Stream(device=self.dev)
+        self.slots = [dict(staged=torch.empty(self.max_src, dtype=torch.uint8).pin_memory(), arena=None,
+                           samples=torch.empty(self.B * C.sizeof(AugSample), dtype=torch.uint8).pin_memory(),
+                           samples_dev=torch.empty(self.B * C.sizeof(AugSample), dtype=torch.uint8, device=self.dev),
+                           jobs=torch.empty(2, 2 * 8 * self.B * JOB, dtype=torch.int64).pin_memory(),
+                           jobs_dev=torch.empty(2, 2 * 8 * self.B * JOB, dtype=torch.int64, device=self.dev),
+                           tgt=torch.empty(self.max_targets, 6).pin_memory(), done=None) for _ in range(2)]
+        self.turn = 0
+        self.ready = None
+
+    def draw(self, indices):
+        if len(indices) != self.B:
+            raise RuntimeError(f"augment: {len(indices)} indices for a batch of {self.B}")
+        return self.sampler.draw(indices)
+
+    def _layout(self, plan, frames):
+        """Arena offsets, resize jobs and sample tables of one batch (host only)."""
+        off, loc, shapes = 0, {}, {}
+        for i in plan.sources:
+            loc[i] = off
+            shapes[i] = tuple(frames[i].shape[:2])
+            off += frames[i].numel()
+        used = off
+        jobs1, jobs2, res, lb = [], [], {}, {}
+        for i in plan.sources:
+            h0, w0 = shapes[i]
+            h, w = resized_shape(h0, w0, self.img_size)
+            if h < 1 or w < 1:
+                raise RuntimeError(f"augment: source {i} of {h0}x{w0} resizes to {h}x{w}")
+            if (h, w) == (h0, w0):
+                res[i] = (loc[i], h, w)
+            else:
+                jobs1.append([loc[i], h0, w0, off, h, w, 0, 0])
+                res[i] = (off, h, w)
+                off += h * w * 3
+        smp = (AugSample * self.B)()
+        for k, rec in enumerate(plan.samples):
+            s = smp[k]
+            for j, cv in enumerate(rec.canvases):
+                s.minv[j][:] = invert_affine(cv.M)
+                if rec.mosaic:
+                    hw = [res[i][1:] for i in cv.indices]
+                    s.ch[j], s.cw[j], s.ntile[j] = 2 * self.H, 2 * self.W, 4
+                    for t, (i, (y1a, y2a, x1a, x2a, y1b, x1b)) in enumerate(zip(cv.indices, _tiles(hw, cv.yc, cv.xc, self.H, self.W))):
+                        o, _, w = res[i]
+                        s.tile[j][t] = AugTile(o + ((y1b - y1a) * w + (x1b - x1a)) * 3, w, y1a, y2a, x1a, x2a, 0)
+                else:
+                    i = cv.indices[0]
+                    o, h, w = res[i]
+                    _, (nw, nh), (left, top) = letterbox_fit(h, w, self.H, self.W)
+                    if (nh, nw) != (h, w):
+                        if i not in lb:
+                            jobs2.append([o, h, w, off, nh, nw, 0, 0])
+                            lb[i] = off
+                            off += nh * nw * 3
+                        o = lb[i]
+                    s.ch[j], s.cw[j], s.ntile[j] = self.H, self.W, 1
+                    s.tile[j][0] = AugTile(o - (top * nw + left) * 3, nw, top, top + nh, left, left + nw, 0)
+            s.mixup = int(rec.mix_r is not None)
+            s.mix_r = rec.mix_r or 0.0
+            s.hsv = int(rec.gains is not None)
+            if rec.gains is not None:
+                for c, lut in enumerate(hsv_luts(rec.gains)):
+                    s.lut[c][:] = lut.tolist()
+            s.flipud, s.fliplr = int(rec.flipud), int(rec.fliplr)
+        return used, off, shapes, loc, jobs1, jobs2, smp
+
+    def submit(self, plan, frames, labels):
+        """Enqueue one batch.  frames: {source index: uint8 HWC BGR image (numpy or CPU tensor)} covering plan.sources;
+        labels: {source index: float32 [k, 5] YOLO rows}.  Returns the host targets [n, 6] (collate_fn's rows)."""
+        try:
+            fr = {i: as_frame(frames[i]) for i in plan.sources}
+            lab = {i: check_labels(labels[i], f"source {i}") for i in plan.sources}
+        except KeyError as e:
+            raise RuntimeError(f"augment: no frame or labels for source {e.args[0]}") from None
+        used = sum(f.numel() for f in fr.values())
+        if used > self.max_src:
+            raise RuntimeError(f"augment: the sources hold {used} bytes, the staging buffer {self.max_src} (raise max_src_bytes)")
+        used, total, shapes, loc, jobs1, jobs2, smp = self._layout(plan, fr)
+        tg = [sample_labels(rec, shapes, lab, self.H, self.W, self.img_size) for rec in plan.samples]
+        for k, t in enumerate(tg):
+            t[:, 0] = k
+        targets = torch.cat(tg, 0)
+        if targets.shape[0] > self.max_targets:
+            raise RuntimeError(f"augment: {targets.shape[0]} target rows exceed max_targets={self.max_targets}")
+
+        slot = self.slots[self.turn]
+        self.turn ^= 1
+        if slot["done"] is not None:
+            slot["done"].synchronize()              # the batch submitted two calls ago has left this slot
+        if slot["arena"] is None or slot["arena"].numel() < total:
+            slot["arena"] = torch.empty(max(total, 1), dtype=torch.uint8, device=self.dev)
+        for i in plan.sources:
+            slot["staged"][loc[i]:loc[i] + fr[i].numel()].copy_(fr[i].view(-1))
+        C.memmove(slot["samples"].data_ptr(), C.addressof(smp), C.sizeof(smp))
+        nj = (len(jobs1), len(jobs2))
+        for r, jobs in enumerate((jobs1, jobs2)):
+            if jobs:
+                slot["jobs"][r, :len(jobs) * JOB].copy_(torch.tensor(jobs, dtype=torch.int64).view(-1))
+        n = targets.shape[0]
+        slot["tgt"][:n].copy_(targets)
+
+        released = torch.cuda.Event()
+        released.record(torch.cuda.current_stream(self.dev))       # the consumer's previous step has read images / targets
+        arena = slot["arena"]
+        with torch.cuda.stream(self.copy_stream):
+            self.copy_stream.wait_stream(self.aug_stream)          # the previous batch is done with this slot's arena
+            arena[:used].copy_(slot["staged"][:used], non_blocking=True)
+            slot["samples_dev"].copy_(slot["samples"], non_blocking=True)
+            slot["jobs_dev"].copy_(slot["jobs"], non_blocking=True)
+        h = _lib.handle(self.dev.index or 0)
+        L = _lib.lib()
+        with torch.cuda.stream(self.aug_stream):
+            self.aug_stream.wait_stream(self.copy_stream)
+            sp = _lib.stream_ptr(self.aug_stream)
+            for r, jobs in enumerate((jobs1, jobs2)):
+                if jobs:
+                    max_pix = max(j[4] * j[5] for j in jobs)
+                    _lib.check(L.yv6_aug_resize(h, C.c_void_p(arena.data_ptr()), C.c_void_p(slot["jobs_dev"][r].data_ptr()), nj[r],
+                                                max_pix, sp))
+            self.aug_stream.wait_event(released)
+            _lib.check(L.yv6_augment(h, C.c_void_p(arena.data_ptr()), C.c_void_p(slot["samples_dev"].data_ptr()), self.B, self.H, self.W,
+                                     C.c_void_p(self.images.data_ptr()), sp))
+            self.targets[:n].copy_(slot["tgt"][:n], non_blocking=True)
+            if n < self.max_targets:
+                self.targets[n:].fill_(-1.0)
+            done = torch.cuda.Event()
+            done.record(self.aug_stream)
+        slot["done"] = self.ready = done
+        return targets
+
+    def wait(self):
+        """Make the current stream wait for the last submitted batch (no host synchronisation)."""
+        if self.ready is None:
+            raise RuntimeError("augment: no batch was submitted")
+        torch.cuda.current_stream(self.dev).wait_event(self.ready)

@@ -17,31 +17,11 @@
 // contract it into an FMA.
 #include "yv6_common.cuh"
 #include "yv6_handle.h"
+#include "yv6_resize.cuh"
 
 namespace yv6 {
 
 constexpr int kLbPix = 16;     // output pixels per thread: one 16-byte store into each channel plane
-
-struct LinTap {
-  int s0, s1, c0, c1;
-};
-
-// One axis of cv::resize's INTER_LINEAR coefficient table for destination index d.
-__device__ __forceinline__ LinTap lin_tap(int d, double scale, int src, bool reset_border) {
-  const float f = __double2float_rn(__dsub_rn(__dmul_rn(__dadd_rn((double)d, 0.5), scale), 0.5));
-  int s = (int)floorf(f);
-  float fr = __fsub_rn(f, (float)s);
-  if (reset_border) {
-    if (s < 0) fr = 0.f, s = 0;
-    if (s >= src - 1) fr = 0.f, s = src - 1;
-  }
-  LinTap t;
-  t.c0 = __float2int_rn(__fmul_rn(__fsub_rn(1.f, fr), 2048.f));
-  t.c1 = __float2int_rn(__fmul_rn(fr, 2048.f));
-  t.s0 = min(max(s, 0), src - 1);
-  t.s1 = min(max(s + 1, 0), src - 1);
-  return t;
-}
 
 // geo [B][YV6_LB_GEO] = (src_off, h0, w0, nh, nw, top, left, 0); thread = 16 consecutive pixels of one canvas row.
 __global__ void __launch_bounds__(256) letterbox_kernel(const uint8_t* __restrict__ src, const int32_t* __restrict__ geo, int H, int W,
@@ -70,8 +50,8 @@ __global__ void __launch_bounds__(256) letterbox_kernel(const uint8_t* __restric
       for (int c = 0; c < 3; ++c) o[c][i] = in ? __ldg(row + xs * 3 + 2 - c) : (uint8_t)114;
     }
   } else {
-    const double sy_scale = __ddiv_rn(1.0, __ddiv_rn((double)nh, (double)h0));
-    const double sx_scale = __ddiv_rn(1.0, __ddiv_rn((double)nw, (double)w0));
+    const double sy_scale = lin_scale(nh, h0);
+    const double sx_scale = lin_scale(nw, w0);
     const LinTap v = lin_tap(ys, sy_scale, h0, false);
     const uint8_t* r0 = im + (int64_t)v.s0 * w0 * 3;
     const uint8_t* r1 = im + (int64_t)v.s1 * w0 * 3;
@@ -84,13 +64,7 @@ __global__ void __launch_bounds__(256) letterbox_kernel(const uint8_t* __restric
       }
       const LinTap hz = lin_tap(xs, sx_scale, w0, true);
 #pragma unroll
-      for (int c = 0; c < 3; ++c) {
-        const int ch = 2 - c;                  // BGR -> RGB
-        const int S0 = __ldg(r0 + hz.s0 * 3 + ch) * hz.c0 + __ldg(r0 + hz.s1 * 3 + ch) * hz.c1;
-        const int S1 = __ldg(r1 + hz.s0 * 3 + ch) * hz.c0 + __ldg(r1 + hz.s1 * 3 + ch) * hz.c1;
-        const int t = (((v.c0 * (S0 >> 4)) >> 16) + ((v.c1 * (S1 >> 4)) >> 16) + 2) >> 2;
-        o[c][i] = (uint8_t)min(max(t, 0), 255);
-      }
+      for (int c = 0; c < 3; ++c) o[c][i] = lin_pixel(r0, r1, v, hz, 2 - c);      // BGR -> RGB
     }
   }
   const int64_t plane = (int64_t)H * W;
