@@ -196,6 +196,42 @@ int yv6_eval_boxes(yv6_handle* h, const float* det, const int32_t* count, const 
                    float* out, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Precision / recall metric of the Evaler (do_pr_metric, core/evaler.py:109-226; utils/metrics.py:13-215) over a dataset.
+ * The accumulators live in device buffers the caller owns, described by yv6_pr_state; the caller zeroes nt, npred,
+ * matrix and flags before the first image.  Slot s = image * max_det + row of conf / cls / correct.
+ *
+ * yv6_pr_match: one launch per batch, images first_image .. first_image + B - 1 of the dataset.  det [B,max_det,6] / count
+ *   [B] as yv6_nms_batched writes them (max_det <= state max_det); targets [n_targets,6] fp32 (image in the batch, cls, x, y,
+ *   w, h normalised), any row order; meta [B,6] as for yv6_eval_boxes; H, W the letterboxed canvas; iouv [10] fp32 device
+ *   table (torch.linspace(0.5, 0.95, 10)).  Writes each row's conf, cls and correct bits (bit t: correct at iouv[t], the
+ *   rule of metrics.process_batch), ndet[image], adds label and prediction counts per class and, with confusion != 0,
+ *   ConfusionMatrix.process_batch to matrix[pred][true] ((nc+1) x (nc+1), row / column nc = background).  flags[0] gets
+ *   error bits (1: label class outside [0, nc) or not whole, 2: same for a detection, 4: an image has more labels than
+ *   fit in shared memory), flags[1] = 1 once any row is correct.
+ * yv6_pr_metric: ap_per_class + compute_ap + the Evaler's summary over images 0 .. n_images - 1, in float64.  px [1000]
+ *   and x101 [101] are np.linspace(0, 1, 1000) / np.linspace(0, 1, 101) (device).  out (device, YV6_PR_OUT_SIZE(nc)
+ *   doubles): p [nc][1000], r [nc][1000], f1 [nc][1000], ap [nc][10] (rows of classes without labels stay 0), nt [nc],
+ *   matrix [(nc+1)^2] (0 without confusion), then map50, map, mp, mr, i* (last arg-max of f1.mean(0)), ok (0: no row is
+ *   correct at any threshold -- map50 = map = mp = mr = 0 and i* = -1), flags[0], number of classes with labels.
+ * ---------------------------------------------------------------------------------------------- */
+typedef struct yv6_pr_state {
+  int32_t max_images, max_det, nc, confusion;
+  float* conf; float* cls;                              /* [max_images][max_det]                                          */
+  uint16_t* correct;                                    /* [max_images][max_det]                                          */
+  int32_t* ndet;                                        /* [max_images] rows per image                                     */
+  int32_t* nt; int32_t* npred;                          /* [nc] labels / predictions per class                            */
+  int32_t* matrix;                                      /* [(nc+1)*(nc+1)], may be NULL when confusion == 0               */
+  int32_t* flags;                                       /* [2]                                                            */
+} yv6_pr_state;
+#define YV6_PR_OUT_SIZE(nc) ((int64_t)(nc) * 3010 + (int64_t)(nc) + ((int64_t)(nc) + 1) * ((int64_t)(nc) + 1) + 8)
+int64_t yv6_pr_workspace_bytes(int32_t max_images, int32_t max_det);
+int yv6_pr_match(yv6_handle* h, const yv6_pr_state* st, const float* det, const int32_t* count, int32_t B, int32_t max_det,
+                 const float* targets, int32_t n_targets, const float* meta, int32_t H, int32_t W, const float* iouv,
+                 int32_t first_image, void* stream);
+int yv6_pr_metric(yv6_handle* h, const yv6_pr_state* st, int32_t n_images, const double* px, const double* x101, void* workspace,
+                  int64_t workspace_bytes, double* out, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Serving from decoded frames: the two steps of the reference's Inferer around the model, for a whole batch per launch.
  * Per-image geometry table geo [B][YV6_LB_GEO] int32 (device) = (src_off, h0, w0, nh, nw, top, left, 0):
  *   src_off   byte offset of the image in `src` (images packed back to back, each uint8 HWC BGR [h0][w0][3]);

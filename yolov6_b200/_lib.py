@@ -112,6 +112,15 @@ class XformSeg(C.Structure):
     ]
 
 
+class PrState(C.Structure):
+    """Mirror of `yv6_pr_state` (include/yv6.h)."""
+    _fields_ = [
+        ("max_images", C.c_int32), ("max_det", C.c_int32), ("nc", C.c_int32), ("confusion", C.c_int32),
+        ("conf", C.c_void_p), ("cls", C.c_void_p), ("correct", C.c_void_p), ("ndet", C.c_void_p),
+        ("nt", C.c_void_p), ("npred", C.c_void_p), ("matrix", C.c_void_p), ("flags", C.c_void_p),
+    ]
+
+
 XF_F32, XF_F64, XF_BF16 = 0, 1, 2
 XFORM_CHUNK = 4096
 
@@ -187,6 +196,11 @@ _SIGNATURES = {
     "yv6_xform": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p]),
     "yv6_sgd_ema_step": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
                                    C.c_void_p, C.c_void_p]),
+    "yv6_pr_workspace_bytes": (C.c_int64, [C.c_int32, C.c_int32]),
+    "yv6_pr_match": (C.c_int, [C.c_void_p, C.POINTER(PrState), C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32,
+                               C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p]),
+    "yv6_pr_metric": (C.c_int, [C.c_void_p, C.POINTER(PrState), C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p,
+                                C.c_void_p]),
     "yv6_nms_workspace_bytes": (C.c_int64, [C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
     "yv6_nms_batched": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_float, C.c_double,
                                   C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,

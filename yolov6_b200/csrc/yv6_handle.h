@@ -20,7 +20,7 @@ struct yv6_handle {
   int max_clusters;                // co-resident 2-CTA clusters of the conv kernel (one CTA per SM); 0 = pairs unavailable
 };
 
-enum { YV6_CFG_CONV = 1u, YV6_CFG_WGRAD = 2u, YV6_CFG_NMS = 4u, YV6_CFG_BN = 8u, YV6_CFG_TRAIN2 = 16u, YV6_CFG_POOL = 32u, YV6_CFG_SELROWS = 64u, YV6_CFG_POOL16 = 128u, YV6_CFG_STEM = 256u };
+enum { YV6_CFG_CONV = 1u, YV6_CFG_WGRAD = 2u, YV6_CFG_NMS = 4u, YV6_CFG_BN = 8u, YV6_CFG_TRAIN2 = 16u, YV6_CFG_POOL = 32u, YV6_CFG_SELROWS = 64u, YV6_CFG_POOL16 = 128u, YV6_CFG_STEM = 256u, YV6_CFG_METRICS = 512u };
 
 // Every entry point runs on the handle's device whatever the caller's current device is, and leaves the
 // caller's current device untouched (several handles / GPUs in one process, nn.DataParallel-style callers).

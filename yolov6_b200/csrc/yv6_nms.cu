@@ -20,6 +20,7 @@
 
 #include "yv6_common.cuh"
 #include "yv6_handle.h"
+#include "yv6_scale_coords.cuh"
 
 namespace yv6 {
 
@@ -761,12 +762,8 @@ __global__ void eval_boxes_kernel(const float* __restrict__ det, const int32_t* 
     return;
   }
   const float* r = det + (int64_t)i * 6;
-  const float* m = meta + b * 6;
-  const float gh = m[0], gw = m[1], px = m[2], py = m[3], h0 = m[4], w0 = m[5];
-  const float x1 = fminf(fmaxf(__fdiv_rn(__fsub_rn(r[0], px), gw), 0.f), w0);
-  const float y1 = fminf(fmaxf(__fdiv_rn(__fsub_rn(r[1], py), gh), 0.f), h0);
-  const float x2 = fminf(fmaxf(__fdiv_rn(__fsub_rn(r[2], px), gw), 0.f), w0);
-  const float y2 = fminf(fmaxf(__fdiv_rn(__fsub_rn(r[3], py), gh), 0.f), h0);
+  const float4 s = scale_coords_rn(r[0], r[1], r[2], r[3], meta + b * 6);
+  const float x1 = s.x, y1 = s.y, x2 = s.z, y2 = s.w;
   const float xc = __fdiv_rn(__fadd_rn(x1, x2), 2.f), yc = __fdiv_rn(__fadd_rn(y1, y2), 2.f);
   const float w = __fsub_rn(x2, x1), hh = __fsub_rn(y2, y1);
   o[0] = __fsub_rn(xc, __fdiv_rn(w, 2.f));
