@@ -1,0 +1,96 @@
+"""Throughput of every built-in model on one GPU: bf16 inference images/s and the CUDA-graph training step.
+
+    python tools/bench_models.py [--steps 30] [--warmup 10] [--models yolov6n,yolov6s_mbla,...] [--no-train]
+
+Inference runs bench.py's own `bench_infer` (the DetectFarm pipeline bench.py times: one CUDA graph per batch -- network,
+decode and batched NMS at the Evaler's settings -- from device-resident inputs, seeded synthetic weights): 640 px batch 32
+for the P5 models, 1280 px batch 8 for the P6 ones.  Each line also carries the conv GFLOP per image of the graph (2 x MACs
+of every conv, transposed conv and prediction conv at that size).  The training step (TrainStep, CUDA graph, TAL or ATSS by
+the config's atss_warmup_epoch at epoch 0, no optimizer) is timed for YOLOv6-S-MBLA (640, bs32) and YOLOv6-N6 (1280, bs8).
+One JSON line per measurement; the first line names the card, its power limit and its maximum SM clock, read in the same run.
+"""
+import argparse
+import json
+import os
+import sys
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+import torch  # noqa: E402
+
+import bench  # noqa: E402
+from yolov6_b200 import configs  # noqa: E402
+from yolov6_b200.arch import build_graph  # noqa: E402
+
+TRAIN_CASES = [("yolov6s_mbla", 640, 32), ("yolov6n6", 1280, 8)]
+
+
+def native(name):
+    """(size, batch) of the measurement: 640 / 32 for P5 models, 1280 / 8 for P6 models."""
+    return (1280, 8) if len(configs.CONFIGS[name]["head"]["strides"]) == 4 else (640, 32)
+
+
+def conv_gflop_per_image(g, size):
+    """2 x multiply-accumulates of every conv of graph g (inference forward, eval head) on one size x size image."""
+    flop = 0
+    for op in g.ops:
+        if op.kind == "pool" or (op.kind == "pred" and op.head[0] not in ("cls", "reg")):
+            continue
+        if op.kind == "stem":
+            lvl = 1
+        elif op.kind == "pred":
+            lvl = g.bufs[op.src.buf].level
+        else:
+            lvl = g.bufs[op.dst.buf].level
+        hw = (size >> lvl) ** 2
+        k = 2 if op.kind == "convT" else op.k        # a 2x2 stride-2 transposed conv: 4 taps per input pixel = 1 per output pixel
+        flop += 2 * hw * op.cout * op.cin * (1 if op.kind == "convT" else k * k)
+    return flop / 1e9
+
+
+def bench_train_step(name, size, batch, steps, warmup, dev):
+    from yolov6_b200.loss import ComputeLoss
+    from yolov6_b200.model import build_model
+    from yolov6_b200.step import TrainStep
+    from yolov6_b200.synth import synthetic_targets
+    torch.manual_seed(0)
+    model = build_model(name, 80, dev).train()
+    hd = configs.CONFIGS[name]["head"]
+    crit = ComputeLoss(fpn_strides=hd["strides"], num_classes=80, ori_img_size=size, warmup_epoch=hd["atss_warmup_epoch"],
+                       use_dfl=hd["use_dfl"], reg_max=hd["reg_max"], iou_type=hd["iou_type"])
+    step = TrainStep(model, crit, batch, size, size, in_dtype=torch.uint8, max_gt=64, graph=True)
+    g = torch.Generator().manual_seed(1)
+    step.load((torch.rand(batch, 3, size, size, generator=g) * 255).to(torch.uint8), synthetic_targets(batch, seed=100))
+    ms = bench.timed(lambda i: step.run(epoch_num=0), steps, warmup, 1, dev)
+    assert not step.overflowed()
+    return {"model": name, "mode": "train", "size": size, "batch": batch, "ms_per_step": ms, "images_per_s": batch / (ms * 1e-3),
+            "assigner": "ATSS" if hd["atss_warmup_epoch"] > 0 else "TAL", "step": "TrainStep (CUDA graph), no optimizer"}
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--steps", type=int, default=30)
+    ap.add_argument("--warmup", type=int, default=10)
+    ap.add_argument("--models", default=",".join(configs.CONFIGS))
+    ap.add_argument("--no-train", action="store_true")
+    args = ap.parse_args()
+    dev = torch.device("cuda:0")
+    torch.cuda.set_device(dev)
+    print(json.dumps({"gpu": bench.gpu_info(0)}), flush=True)
+    for name in args.models.split(","):
+        size, batch = native(name)
+        r = bench.bench_infer(name, batch, size, args.steps, args.warmup, 0, 1, dev, precision="bf16", e2e=False, roofline=False)
+        print(json.dumps({"model": name, "mode": "infer bf16", "size": size, "batch": batch, "images_per_s": r["value"],
+                          "ms_per_step": r["ms_per_step"], "launches_per_step": r["launches_per_step"],
+                          "conv_gflop_per_image": conv_gflop_per_image(build_graph(configs.get_config(name), 80), size)}), flush=True)
+        del r
+        torch.cuda.empty_cache()
+    if not args.no_train:
+        for name, size, batch in TRAIN_CASES:
+            print(json.dumps(bench_train_step(name, size, batch, args.steps, args.warmup, dev)), flush=True)
+            torch.cuda.empty_cache()
+
+
+if __name__ == "__main__":
+    main()

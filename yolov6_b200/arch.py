@@ -11,7 +11,7 @@ activation buffers, emitted once per (config, num_classes):
     (reppan.py:228,232, common.py:650,718 -> `dst=T(buf, c_off, c)`);
   * the engine (engine.py) walks the list and issues one kernel per op through the C ABI.
 
-Op kinds: stem | conv (rep / cba / plain parameter layouts) | convT | pool.
+Op kinds: stem | conv (rep / cba / cm / plain parameter layouts) | convT | pool.
 """
 import math
 from dataclasses import dataclass, field
@@ -37,7 +37,7 @@ class Buf:
 class Op:
     kind: str                 # 'stem' | 'conv' | 'convT' | 'pool' | 'pred'
     name: str                 # reference parameter prefix
-    layout: str = ""          # 'rep' | 'cba' | 'plain' | 'convT'
+    layout: str = ""          # 'rep' | 'cba' | 'cm' (bare ConvModule) | 'plain' | 'convT'
     src: Optional[T] = None
     dst: Optional[T] = None
     cin: int = 0
@@ -48,6 +48,14 @@ class Op:
     res: Optional[T] = None
     alpha: Optional[str] = None   # parameter name of BottleRep.alpha (common.py:600-603)
     head: Optional[tuple] = None  # ('cls' | 'reg', level index) for the prediction convs
+    # an op that computes output rows [w_row0, w_row0 + cout) of a parameter with w_rows output rows (0: the whole parameter);
+    # the op with w_row0 == 0 owns the parameter.  BatchNorm is per output channel, so the rows fold and train on their own.
+    w_row0: int = 0
+    w_rows: int = 0
+
+    @property
+    def param_rows(self):
+        return self.w_rows or self.cout
 
 
 @dataclass
@@ -77,12 +85,12 @@ class Graph:
     def level(self, t):
         return self.bufs[t.buf].level
 
-    def conv(self, name, layout, src, cout, k=1, s=1, act="relu", dst=None, res=None, alpha=None):
+    def conv(self, name, layout, src, cout, k=1, s=1, act="relu", dst=None, res=None, alpha=None, rows=(0, 0)):
         lvl = self.level(src) + (1 if s == 2 else 0)
         if dst is None:
             dst = self.new(lvl, cout, name)
         assert dst.c == cout and self.level(dst) == lvl, (name, dst, cout, lvl)
-        self.ops.append(Op("conv", name, layout, src, dst, src.c, cout, k, s, act, res, alpha))
+        self.ops.append(Op("conv", name, layout, src, dst, src.c, cout, k, s, act, res, alpha, w_row0=rows[0], w_rows=rows[1]))
         return dst
 
     def block(self, name, src, cout, s=1, dst=None, res=None, alpha=None):
@@ -136,32 +144,83 @@ def _bepc3(g, name, src, cout, n, e, dst=None):
     return g.conv(name + ".cv3", "cba", T(cat, 0, 2 * c_), cout, 1, 1, g.act, dst=dst)
 
 
-def _sppf(g, name, src, cout):
+def mbla_branches(n):
+    """MBLABlock's BottleRep3 chain lengths (common.py:657-668): n // 2 (at least 1) blocks in the longest branch, plus one
+    branch of the largest power of two below half of that when there are more than one."""
+    n = max(n // 2, 1)
+    if n == 1:
+        return [0, 1]
+    e = 1
+    while 2 * e < n:
+        e *= 2
+    return [0, e, n]
+
+
+def _mbla(g, name, src, cout, n, e, dst=None):
+    """MBLABlock (common.py:653-692): cv2(cat(y0, y1, m0(y1)..., y2, m1(y2)...)) with y = split(cv1(x)), where branch i is
+    a chain of BottleRep3 blocks (common.py:611-631), each conv3(conv2(conv1(x))) + alpha * x; every block reads the
+    previous block's output.  cv1 / cv2 are bare ConvModules.  The concat is one buffer; the y_i are not adjacent in it
+    once there is a third branch, so cv1 runs as one launch per contiguous run of concat slots, each over its rows of
+    the parameter."""
+    n_list = mbla_branches(n)
+    c = int(cout * e)
+    ctot = (sum(n_list) + len(n_list)) * c
+    cat = g.buf(g.level(src), ctot, name + ".cat")
+    slot = [i + sum(n_list[:i]) for i in range(len(n_list))]     # concat slot (in units of c) of y_i
+    b0 = 0
+    for b in range(1, len(n_list) + 1):
+        if b == len(n_list) or slot[b] != slot[b - 1] + 1:
+            g.conv(name + ".cv1", "cm", src, (b - b0) * c, 1, 1, g.act, dst=T(cat, slot[b0] * c, (b - b0) * c),
+                   rows=(b0 * c, len(n_list) * c))
+            b0 = b
+    for i, k in enumerate(n_list[1:]):
+        x = T(cat, slot[i + 1] * c, c)
+        for j in range(k):
+            p = f"{name}.m.{i}.{j}"
+            t = g.block(p + ".conv2", g.block(p + ".conv1", x, c), c)
+            x = g.block(p + ".conv3", t, c, dst=T(cat, x.c_off + c, c), res=x, alpha=p + ".alpha")
+    return g.conv(name + ".cv2", "cm", T(cat, 0, ctot), cout, 1, 1, g.act, dst=dst)
+
+
+STAGE_BLOCKS = ("BepC3", "MBLABlock")
+
+
+def _stage(g, kind, name, src, cout, n, e, dst=None):
+    """The stage block of the backbones and necks: RepBlock (EfficientRep*, RepBiFPANNeck*) or, on the CSP variants, the
+    `stage_block_type` of the config (yolo.py:75-96, efficientrep.py:271-274, reppan.py:684-687)."""
+    if kind == "RepBlock":
+        return _rep_block(g, name, src, cout, n, dst)
+    if kind == "BepC3":
+        return _bepc3(g, name, src, cout, n, e, dst)
+    return _mbla(g, name, src, cout, n, e, dst)
+
+
+def _sppf(g, name, src, cout, act):
     """SimSPPF / SPPF (common.py:97-133)."""
     p = name + ".sppf"
     c_ = src.c // 2
     lvl = g.level(src)
     cat = g.buf(lvl, 4 * c_, p + ".cat")
-    g.conv(p + ".cv1", "cba", src, c_, 1, 1, g.act, dst=T(cat, 0, c_))
+    g.conv(p + ".cv1", "cba", src, c_, 1, 1, act, dst=T(cat, 0, c_))
     g.ops.append(Op("pool", p + ".m", src=T(cat, 0, c_), dst=T(cat, 0, 4 * c_), cin=c_, cout=c_))
-    return g.conv(p + ".cv2", "cba", T(cat, 0, 4 * c_), cout, 1, 1, g.act)
+    return g.conv(p + ".cv2", "cba", T(cat, 0, 4 * c_), cout, 1, 1, act)
 
 
-def _cspsppf(g, name, src, cout):
+def _cspsppf(g, name, src, cout, act):
     """SimCSPSPPF / CSPSPPF (common.py:135-178), e = 0.5."""
     p = name + ".cspsppf"
     c_ = int(cout * 0.5)
     lvl = g.level(src)
     cat4 = g.buf(lvl, 4 * c_, p + ".cat4")
     cat2 = g.buf(lvl, 2 * c_, p + ".cat2")
-    a = g.conv(p + ".cv1", "cba", src, c_, 1, 1, g.act)
-    a = g.conv(p + ".cv3", "cba", a, c_, 3, 1, g.act)
-    g.conv(p + ".cv4", "cba", a, c_, 1, 1, g.act, dst=T(cat4, 0, c_))
-    g.conv(p + ".cv2", "cba", src, c_, 1, 1, g.act, dst=T(cat2, 0, c_))
+    a = g.conv(p + ".cv1", "cba", src, c_, 1, 1, act)
+    a = g.conv(p + ".cv3", "cba", a, c_, 3, 1, act)
+    g.conv(p + ".cv4", "cba", a, c_, 1, 1, act, dst=T(cat4, 0, c_))
+    g.conv(p + ".cv2", "cba", src, c_, 1, 1, act, dst=T(cat2, 0, c_))
     g.ops.append(Op("pool", p + ".m", src=T(cat4, 0, c_), dst=T(cat4, 0, 4 * c_), cin=c_, cout=c_))
-    b = g.conv(p + ".cv5", "cba", T(cat4, 0, 4 * c_), c_, 1, 1, g.act)
-    g.conv(p + ".cv6", "cba", b, c_, 3, 1, g.act, dst=T(cat2, c_, c_))
-    return g.conv(p + ".cv7", "cba", T(cat2, 0, 2 * c_), cout, 1, 1, g.act)
+    b = g.conv(p + ".cv5", "cba", T(cat4, 0, 4 * c_), c_, 1, 1, act)
+    g.conv(p + ".cv6", "cba", b, c_, 3, 1, act, dst=T(cat2, c_, c_))
+    return g.conv(p + ".cv7", "cba", T(cat2, 0, 2 * c_), cout, 1, 1, act)
 
 
 def _bifusion(g, name, x0, x1, x2, cout):
@@ -190,12 +249,16 @@ def build_graph(cfg, num_classes=80, name="yolov6", fuse_ab=False, distill_ns=Fa
     if distill_ns and (fuse_ab or nl != 3):
         raise ValueError("distill_ns is the 3-level N / S student head (yolo.py:113-120); it excludes fuse_ab")
     csp = "CSP" in bb["type"]
-    p6 = bb["type"].endswith("P6")
+    p6 = bb["type"] in ("EfficientRep6", "CSPBepBackbone_P6")
     nstage = 6 if p6 else 5
-    if bb["type"] not in ("EfficientRep", "CSPBepBackbone", "CSPBepBackbone_P6"):
+    if bb["type"] not in ("EfficientRep", "EfficientRep6", "CSPBepBackbone", "CSPBepBackbone_P6"):
         raise NotImplementedError(f"backbone {bb['type']} is outside the hot-path scope (SURVEY.md section 2)")
-    if nk["type"] not in ("RepBiFPANNeck", "CSPRepBiFPANNeck", "CSPRepBiFPANNeck_P6"):
+    if nk["type"] not in ("RepBiFPANNeck", "RepBiFPANNeck6", "CSPRepBiFPANNeck", "CSPRepBiFPANNeck_P6"):
         raise NotImplementedError(f"neck {nk['type']} is outside the hot-path scope (SURVEY.md section 2)")
+    # the CSP variants take the backbone's stage_block_type for the backbone AND the neck (yolo.py:75-96)
+    stage_kind = bb.get("stage_block_type", "BepC3") if csp else "RepBlock"
+    if stage_kind not in STAGE_BLOCKS + ("RepBlock",):
+        raise ValueError(f"stage_block_type {stage_kind!r} is not one of {STAGE_BLOCKS} (efficientrep.py:271-276)")
 
     # ---- backbone (efficientrep.py:7-118, 250-374, 377-516) ----
     layout = "rep" if g.mode == "repvgg" else "cba"
@@ -206,12 +269,11 @@ def build_graph(cfg, num_classes=80, name="yolov6", fuse_ab=False, distill_ns=Fa
     for s in range(2, nstage + 1):
         p = f"backbone.ERBlock_{s}"
         x = g.block(p + ".0", x, ch[s - 1], s=2)
-        if csp:
-            x = _bepc3(g, p + ".1", x, ch[s - 1], reps[s - 1], bb["csp_e"])
-        else:
-            x = _rep_block(g, p + ".1", x, ch[s - 1], reps[s - 1])
+        x = _stage(g, stage_kind, p + ".1", x, ch[s - 1], reps[s - 1], bb.get("csp_e"))
         if s == nstage:
-            x = _cspsppf(g, p + ".2", x, ch[s - 1]) if bb.get("cspsppf") else _sppf(g, p + ".2", x, ch[s - 1])
+            # EfficientRep6 always takes the ReLU variants (efficientrep.py:209), the others SiLU ones with ConvBNSiLU blocks
+            act = "relu" if bb["type"] == "EfficientRep6" else g.act
+            x = (_cspsppf if bb.get("cspsppf") else _sppf)(g, p + ".2", x, ch[s - 1], act)
         if s > 2 or bb.get("fuse_P2"):
             outs.append(x)
     if not bb.get("fuse_P2"):
@@ -221,9 +283,7 @@ def build_graph(cfg, num_classes=80, name="yolov6", fuse_ab=False, distill_ns=Fa
     nb = len(bb["num_repeats"])
 
     def stage(name, src, cout, n, dst=None):
-        if csp:
-            return _bepc3(g, name, src, cout, n, nk["csp_e"], dst)
-        return _rep_block(g, name, src, cout, n, dst)
+        return _stage(g, stage_kind, name, src, cout, n, nk.get("csp_e"), dst)
 
     if not p6:
         x3, x2, x1, x0 = outs
@@ -317,6 +377,10 @@ def param_specs(g):
         elif op.layout == "cba":
             specs.append((n + ".block.conv.weight", (op.cout, op.cin, op.k, op.k), "conv"))
             bn(n + ".block.bn", op.cout)
+        elif op.layout == "cm":
+            if op.w_row0 == 0:
+                specs.append((n + ".conv.weight", (op.param_rows, op.cin, op.k, op.k), "conv"))
+                bn(n + ".bn", op.param_rows)
         elif op.layout == "plain":
             specs.append((n + ".weight", (op.cout, op.cin, 1, 1), "conv"))
             specs.append((n + ".bias", (op.cout,), "bias"))

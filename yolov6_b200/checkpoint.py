@@ -10,15 +10,15 @@ compatibility; BN folding / RepVGG re-parameterisation happen inside the inferen
 """
 import torch
 
-from . import configs
+from . import arch, configs
 from .model import Model
 
 
 def _matching_config(sd, num_classes):
+    """The built-in configuration whose state_dict has exactly these keys and shapes (each built-in layout is unique)."""
     want = {k: tuple(v.shape) for k, v in sd.items()}
     for name in configs.CONFIGS:
-        m = Model(name, num_classes=num_classes)
-        have = {k: tuple(v.shape) for k, v in m.state_dict().items()}
+        have = {k: tuple(shape) for k, shape, _ in arch.param_specs(arch.build_graph(configs.get_config(name), num_classes))}
         if have == want:
             return name
     return None
@@ -42,7 +42,8 @@ def from_reference(module, cfg=None, device=None):
     if cfg is None:
         cfg = _matching_config(sd, nc)
         if cfg is None:
-            raise RuntimeError("no built-in configuration (yolov6n/s/m/l6) has this state_dict layout; pass the reference Config as `cfg`")
+            raise RuntimeError(f"no built-in configuration ({', '.join(configs.CONFIGS)}) has this state_dict layout; "
+                               "pass the reference Config as `cfg`")
     m = Model(cfg, num_classes=nc)
     m.load_state_dict(sd, strict=True)
     if device is None:

@@ -1,4 +1,5 @@
-"""Built-in model configurations (the `model` dict of reference configs/yolov6{n,s,m,l6}.py) so that
+"""Built-in model configurations (the `model` dict and `training_mode` of reference configs/yolov6{n,s,m,l,n6,s6,m6,l6}.py and
+configs/mbla/yolov6{s,m,l,x}_mbla.py; `training_mode` defaults to "repvgg" as tools/train.py:99-100 does) so that
 tests, smoke() and bench.py run where /root/reference is not mounted, plus a normaliser that accepts
 the reference's own mmcv-style Config object (yolov6/utils/config.py) for drop-in use."""
 import copy
@@ -6,6 +7,8 @@ import copy
 _P5_HEAD = dict(type="EffiDeHead", in_channels=[128, 256, 512], num_layers=3, begin_indices=24, anchors=3,
                 anchors_init=[[10, 13, 19, 19, 33, 23], [30, 61, 59, 59, 59, 119], [116, 90, 185, 185, 373, 326]],   # fuse_ab head
                 out_indices=[17, 20, 23], strides=[8, 16, 32], atss_warmup_epoch=0)
+_P6_HEAD = dict(type="EffiDeHead", in_channels=[128, 256, 512, 1024], num_layers=4, anchors=1, strides=[8, 16, 32, 64],
+                atss_warmup_epoch=4)
 
 CONFIGS = {
     "yolov6n": dict(
@@ -27,15 +30,55 @@ CONFIGS = {
         neck=dict(type="CSPRepBiFPANNeck", num_repeats=[12, 12, 12, 12], out_channels=[256, 128, 128, 256, 256, 512],
                   csp_e=2.0 / 3),
         head=dict(_P5_HEAD, iou_type="giou", use_dfl=True, reg_max=16)),
+    "yolov6l": dict(
+        training_mode="conv_silu", depth_multiple=1.0, width_multiple=1.0,
+        backbone=dict(type="CSPBepBackbone", num_repeats=[1, 6, 12, 18, 6], out_channels=[64, 128, 256, 512, 1024],
+                      csp_e=0.5, fuse_P2=True),
+        neck=dict(type="CSPRepBiFPANNeck", num_repeats=[12, 12, 12, 12], out_channels=[256, 128, 128, 256, 256, 512],
+                  csp_e=0.5),
+        head=dict(_P5_HEAD, iou_type="giou", use_dfl=True, reg_max=16)),
+    "yolov6n6": dict(
+        training_mode="repvgg", depth_multiple=0.33, width_multiple=0.25,
+        backbone=dict(type="EfficientRep6", num_repeats=[1, 6, 12, 18, 6, 6], out_channels=[64, 128, 256, 512, 768, 1024],
+                      fuse_P2=True, cspsppf=True),
+        neck=dict(type="RepBiFPANNeck6", num_repeats=[12, 12, 12, 12, 12, 12], out_channels=[512, 256, 128, 256, 512, 1024]),
+        head=dict(_P6_HEAD, iou_type="siou", use_dfl=False, reg_max=0)),
+    "yolov6s6": dict(
+        training_mode="repvgg", depth_multiple=0.33, width_multiple=0.50,
+        backbone=dict(type="EfficientRep6", num_repeats=[1, 6, 12, 18, 6, 6], out_channels=[64, 128, 256, 512, 768, 1024],
+                      fuse_P2=True, cspsppf=True),
+        neck=dict(type="RepBiFPANNeck6", num_repeats=[12, 12, 12, 12, 12, 12], out_channels=[512, 256, 128, 256, 512, 1024]),
+        head=dict(_P6_HEAD, iou_type="giou", use_dfl=False, reg_max=0)),
+    "yolov6m6": dict(
+        training_mode="repvgg", depth_multiple=0.60, width_multiple=0.75,
+        backbone=dict(type="CSPBepBackbone_P6", num_repeats=[1, 6, 12, 18, 6, 6],
+                      out_channels=[64, 128, 256, 512, 768, 1024], csp_e=2.0 / 3, fuse_P2=True),
+        neck=dict(type="CSPRepBiFPANNeck_P6", num_repeats=[12, 12, 12, 12, 12, 12],
+                  out_channels=[512, 256, 128, 256, 512, 1024], csp_e=2.0 / 3),
+        head=dict(_P6_HEAD, iou_type="giou", use_dfl=True, reg_max=16)),
     "yolov6l6": dict(
         training_mode="conv_silu", depth_multiple=1.0, width_multiple=1.0,
         backbone=dict(type="CSPBepBackbone_P6", num_repeats=[1, 6, 12, 18, 6, 6],
                       out_channels=[64, 128, 256, 512, 768, 1024], csp_e=0.5, fuse_P2=True),
         neck=dict(type="CSPRepBiFPANNeck_P6", num_repeats=[12, 12, 12, 12, 12, 12],
                   out_channels=[512, 256, 128, 256, 512, 1024], csp_e=0.5),
-        head=dict(type="EffiDeHead", in_channels=[128, 256, 512, 1024], num_layers=4, anchors=1,
-                  strides=[8, 16, 32, 64], atss_warmup_epoch=4, iou_type="giou", use_dfl=True, reg_max=16)),
+        head=dict(_P6_HEAD, iou_type="giou", use_dfl=True, reg_max=16)),
 }
+
+
+def _mbla(depth, width):
+    """configs/mbla/yolov6{s,m,l,x}_mbla.py: CSP networks with MBLABlock stages, which differ only in depth and width."""
+    return dict(
+        training_mode="conv_silu", depth_multiple=depth, width_multiple=width,
+        backbone=dict(type="CSPBepBackbone", num_repeats=[1, 4, 8, 8, 4], out_channels=[64, 128, 256, 512, 1024],
+                      csp_e=0.5, fuse_P2=True, stage_block_type="MBLABlock"),
+        neck=dict(type="CSPRepBiFPANNeck", num_repeats=[8, 8, 8, 8], out_channels=[256, 128, 128, 256, 256, 512],
+                  csp_e=0.5, stage_block_type="MBLABlock"),
+        head=dict(_P5_HEAD, iou_type="giou", use_dfl=True, reg_max=16))
+
+
+CONFIGS.update({"yolov6s_mbla": _mbla(0.5, 0.5), "yolov6m_mbla": _mbla(0.5, 0.75), "yolov6l_mbla": _mbla(0.5, 1.0),
+                "yolov6x_mbla": _mbla(1.0, 1.0)})
 
 
 def get_config(name):

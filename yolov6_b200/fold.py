@@ -42,6 +42,10 @@ def fold_op(sd, op):
     if op.layout == "cba":
         k, b = fold_conv_bn(sd, n + ".block")
         return k.permute(0, 2, 3, 1).contiguous(), b
+    if op.layout == "cm":       # rows [w_row0, w_row0 + cout) of a bare ConvModule (arch.Op.w_row0)
+        k, b = fold_conv_bn(sd, n)
+        r = slice(op.w_row0, op.w_row0 + op.cout)
+        return k[r].permute(0, 2, 3, 1).contiguous(), b[r]
     if op.layout == "plain":
         return sd[n + ".weight"].double().permute(0, 2, 3, 1).contiguous(), sd[n + ".bias"].double()
     if op.layout == "convT":

@@ -160,6 +160,11 @@ class Model(nn.Module):
                 b = _ensure(root, path[1:] + ["block"])
                 b.add_module("conv", nn.Conv2d(op.cin, op.cout, op.k, op.s, op.k // 2, bias=False))
                 b.add_module("bn", nn.BatchNorm2d(op.cout))
+            elif op.layout == "cm":
+                if op.w_row0 == 0:
+                    node = _ensure(root, path[1:])
+                    node.add_module("conv", nn.Conv2d(op.cin, op.param_rows, op.k, op.s, op.k // 2, bias=False))
+                    node.add_module("bn", nn.BatchNorm2d(op.param_rows))
             elif op.layout == "plain":
                 _ensure(root, path[1:-1]).add_module(path[-1], nn.Conv2d(op.cin, op.cout, 1))
             elif op.layout == "convT":

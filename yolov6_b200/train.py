@@ -51,12 +51,16 @@ def op_branches(op):
         if op.kind != "stem" and op.cin == op.cout and op.s == 1:
             br.append((op.name + ".rbr_identity", 0))
         return br
+    if op.layout == "cm":        # bare ConvModule (MBLABlock.cv1 / cv2, common.py:671-677)
+        return [(op.name, op.k)]
     return [(op.name + ".block", op.k)]
 
 
 def op_param_names(op):
-    """Trainable parameters owned by a graph op, in the order their gradients are produced."""
-    if op.kind == "pool":
+    """Trainable parameters owned by a graph op, in the order their gradients are produced.  An op over rows w_row0 > 0 of a
+    parameter (arch.Op.w_row0) writes its rows of the gradients, but the parameter belongs to the op over row 0: that op
+    comes first in the forward pass, so the parameter's gradient is complete once that op's backward ran."""
+    if op.kind == "pool" or op.w_row0:
         return []
     if op.kind == "pred":
         return [op.name + ".weight", op.name + ".bias"]
@@ -227,7 +231,7 @@ class TrainEngine:
                 if k == 0:
                     W["br"].append(ent)
                     continue
-                wsrc = fl.ptr(prefix + ".conv.weight")                           # [Cout][Cin][k][k]
+                wsrc = fl.ptr(prefix + ".conv.weight") + 4 * op.w_row0 * ci * k * k   # [Cout][Cin][k][k]
                 if op.kind == "stem":
                     ent["w"] = torch.zeros(3, 3, 3, co, dtype=torch.float32, device=dev)   # [r][s][c][Cout], fp32 math
                     if k == 3:
@@ -261,7 +265,7 @@ class TrainEngine:
         self.pack_table = XformTable(pack, dev)
 
         # ---- gradient unpack table, in backward order = flat gradient order; buckets = contiguous op ranges
-        ops_with_params = [i for i in range(len(g.ops) - 1, -1, -1) if op_param_names(g.ops[i])]
+        ops_with_params = [i for i in range(len(g.ops) - 1, -1, -1) if g.ops[i].kind != "pool"]
         total = fl.n_train
         bounds, acc, k = [], 0, 0
         per_bucket = [[] for _ in range(self.n_buckets)]
@@ -274,7 +278,7 @@ class TrainEngine:
             per_bucket[k].extend(segs)
             self.bucket_of_op[i] = k
             acc += size
-            if k < self.n_buckets - 1 and acc >= total * (k + 1) / self.n_buckets:
+            if k < self.n_buckets - 1 and acc >= total * (k + 1) / self.n_buckets and op_param_names(op):
                 hi = fl.slots[op_param_names(op)[-1]][0] + (fl.slots[op_param_names(op)[-1]][1] + 3) // 4 * 4
                 self.bucket_range.append((lo, hi))
                 lo = hi
@@ -305,6 +309,7 @@ class TrainEngine:
             return segs
         br = op_branches(op)
         co, ci = op.cout, op.cin
+        r0 = 4 * op.w_row0          # byte offset of the op's first row in per-channel vectors
         for b, (prefix, k) in enumerate(br):
             bn = prefix + (".bn" if k else "")
             if k:
@@ -316,10 +321,10 @@ class TrainEngine:
                         segs.append(_seg(fl.grad_ptr(prefix + ".conv.weight"), z(i, "dw", b) + 4 * 12, [co, 3], [3, 1], [32, 1], XF_F32, XF_F32))
                 else:
                     kk = k * k      # dw [Cout][kk][Cin] -> [Cout][Cin][kk]
-                    segs.append(_seg(fl.grad_ptr(prefix + ".conv.weight"), z(i, "dw", b), [co, ci, kk], [ci * kk, kk, 1],
+                    segs.append(_seg(fl.grad_ptr(prefix + ".conv.weight") + r0 * ci * kk, z(i, "dw", b), [co, ci, kk], [ci * kk, kk, 1],
                                      [kk * ci, 1, ci], XF_F32, XF_F32))
-            segs.append(_seg(fl.grad_ptr(bn + ".weight"), z(i, "s2") + 8 * b * co, [co], [1], [1], XF_F32, XF_F64))   # dgamma = sum dz * xhat
-            segs.append(_seg(fl.grad_ptr(bn + ".bias"), z(i, "s1"), [co], [1], [1], XF_F32, XF_F64))                 # dbeta = sum dz
+            segs.append(_seg(fl.grad_ptr(bn + ".weight") + r0, z(i, "s2") + 8 * b * co, [co], [1], [1], XF_F32, XF_F64))   # dgamma = sum dz * xhat
+            segs.append(_seg(fl.grad_ptr(bn + ".bias") + r0, z(i, "s1"), [co], [1], [1], XF_F32, XF_F64))                 # dbeta = sum dz
         if op.alpha:
             segs.append(_seg(fl.grad_ptr(op.alpha), z(i, "dalpha"), [1], [1], [1], XF_F32, XF_F64))
         return segs
@@ -343,8 +348,9 @@ class TrainEngine:
         d.dw = dw_ptr
         return d
 
-    def _stats_desc(self, xs, c, pixels, sums_ptr, cnt_ptr, finalize=None):
-        """xs: [(tensor, channel offset)]; finalize: [(bn prefix, stats tensor [4][C])] or None (sums only)."""
+    def _stats_desc(self, xs, c, pixels, sums_ptr, cnt_ptr, finalize=None, row0=0):
+        """xs: [(tensor, channel offset)]; finalize: [(bn prefix, stats tensor [4][C])] or None (sums only); row0: the channels
+        are rows [row0, row0 + c) of the BatchNorm."""
         d = BnStatsDesc()
         d.nb, d.C, d.pixels = len(xs), c, pixels
         for b, (t, off) in enumerate(xs):
@@ -355,8 +361,9 @@ class TrainEngine:
         if finalize is not None:
             fl = self.flat
             for b, (prefix, st) in enumerate(finalize):
-                d.gamma[b], d.beta[b] = fl.ptr(prefix + ".weight"), fl.ptr(prefix + ".bias")
-                d.running_mean[b], d.running_var[b] = fl.ptr(prefix + ".running_mean"), fl.ptr(prefix + ".running_var")
+                d.gamma[b], d.beta[b] = fl.ptr(prefix + ".weight") + 4 * row0, fl.ptr(prefix + ".bias") + 4 * row0
+                d.running_mean[b] = fl.ptr(prefix + ".running_mean") + 4 * row0
+                d.running_var[b] = fl.ptr(prefix + ".running_var") + 4 * row0
                 d.stats[b] = st.data_ptr()
         return d
 
@@ -531,7 +538,7 @@ class TrainEngine:
                     fwd.append(("conv", self._conv_desc(src, op.src.c_off, ent["w"], raw, stride=op.s)))
                 xs.append((raw, 0))
             fin = [(ent["prefix"] + (".bn" if ent["k"] else ""), st[b]) for b, ent in enumerate(br)]
-            fwd.append(("stats", self._stats_desc(xs, op.cout, count, z(i, "fsum"), z(i, "fcnt"), fin)))
+            fwd.append(("stats", self._stats_desc(xs, op.cout, count, z(i, "fsum"), z(i, "fcnt"), fin, op.w_row0)))
             d = BnDesc()
             d.nb, d.act, d.C, d.pixels = nb, ACT_CODES[op.act], op.cout, count
             dcs = []
