@@ -31,7 +31,8 @@ enum {
   YV6_ERR_STATE = -3    /* handle not usable (wrong device, destroyed, ...) */
 };
 
-enum { YV6_ACT_NONE = 0, YV6_ACT_RELU = 1, YV6_ACT_SILU = 2, YV6_ACT_SIGMOID = 3 };
+/* HARDSWISH = x * min(max(x + 3, 0), 6) / 6 (nn.Hardswish), HARDSIGMOID = min(max(x + 3, 0), 6) / 6 (nn.Hardsigmoid) */
+enum { YV6_ACT_NONE = 0, YV6_ACT_RELU = 1, YV6_ACT_SILU = 2, YV6_ACT_SIGMOID = 3, YV6_ACT_HARDSWISH = 4, YV6_ACT_HARDSIGMOID = 5 };
 enum { YV6_DT_BF16 = 0, YV6_DT_F32 = 1, YV6_DT_U8 = 2 };
 #define YV6_PAD_SAME (-1000000)
 
@@ -151,6 +152,50 @@ int yv6_stem_fwd(yv6_handle* h, const yv6_stem_desc* d, void* stream);
  * maxima (= three chained MaxPool2d(5,1,2)) into slices [C,2C), [2C,3C), [3C,4C). */
 int yv6_sppf_pool(yv6_handle* h, void* buf, int32_t N, int32_t H, int32_t W, int32_t C, int32_t c_total,
                   int32_t nsplit, int64_t plane_stride, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * YOLOv6Lite (reference yolov6/models/yolo_lite.py; layers/common.py:740-934): the layers that are not dense convolutions.
+ * The 1x1 ConvBNHS convs run on yv6_conv_fwd with act = YV6_ACT_HARDSWISH, `conv_0` on yv6_stem_fwd.
+ * Activations are NHWC bf16 channel slices: x / y point at the slice's first channel, *_c_total / *_pitch is the channel
+ * pitch of the buffer; nsplit = 3: three bf16 planes *_plane_stride elements apart, computed on as their fp32 sum.
+ *
+ * yv6_dwconv_fwd: depthwise conv (groups = C), k in {3, 5}, stride 1 or 2, padding k / 2, output ((H-1)/s+1) x ((W-1)/s+1);
+ *   y = act(conv(x, w) + bias), act NONE or HARDSWISH.  w fp32 [k*k][C] (tap-major, channel innermost), bias fp32 [C] or NULL.
+ *   Any C and slice offset; channels of y outside the slice are not written.
+ * yv6_se_fwd: SEBlock in place on x: s = hardsigmoid(W2 relu(W1 mean_hw(x) + b1) + b2), x *= s per (image, channel).
+ *   w1 fp32 [Cr][C], b1 [Cr], w2 [C][Cr], b2 [C]; C <= 512, Cr <= 128.  Deterministic: fixed summation order, no atomics.
+ * yv6_channel_shuffle: channel_shuffle(cat(a, b), 2) of two C-channel slices: y[.., 2j] = a[.., j], y[.., 2j+1] = b[.., j].
+ * yv6_upsample2x: nearest 2x upsample of an [N, H, W, C] slice into a [N, 2H, 2W, .] slice.
+ * ---------------------------------------------------------------------------------------------- */
+typedef struct yv6_dw_desc {
+  const void* x;
+  int32_t N, H, W, C;
+  int32_t x_c_total, y_c_total;
+  int64_t x_plane_stride, y_plane_stride;
+  const float* w;
+  const float* bias;
+  int32_t k, stride, act, nsplit;
+  void* y;
+} yv6_dw_desc;
+int yv6_dwconv_fwd(yv6_handle* h, const yv6_dw_desc* d, void* stream);
+
+typedef struct yv6_se_desc {
+  void* x;
+  int32_t N, HW, C, Cr;
+  int64_t c_total, plane_stride;
+  const float* w1;
+  const float* b1;
+  const float* w2;
+  const float* b2;
+  int32_t nsplit, reserved0;
+} yv6_se_desc;
+int yv6_se_fwd(yv6_handle* h, const yv6_se_desc* d, void* stream);
+
+int yv6_channel_shuffle(yv6_handle* h, const void* a, int64_t a_pitch, int64_t a_plane, const void* b, int64_t b_pitch,
+                        int64_t b_plane, int64_t pixels, int32_t C, void* y, int64_t y_pitch, int64_t y_plane, int32_t nsplit,
+                        void* stream);
+int yv6_upsample2x(yv6_handle* h, const void* x, int64_t x_pitch, int64_t x_plane, int32_t N, int32_t H, int32_t W, int32_t C,
+                   void* y, int64_t y_pitch, int64_t y_plane, int32_t nsplit, void* stream);
 
 /* Eval-mode head decode (reference yolov6/models/effidehead.py:106-139, assigners/anchor_generator.py
  * :13-33, utils/general.py:32-43): cls [B,A,nc] fp32 (post-sigmoid), reg [B,A,reg_ch] fp32 (ltrb, or

@@ -4,7 +4,10 @@
 
 Inference runs bench.py's own `bench_infer` (the DetectFarm pipeline bench.py times: one CUDA graph per batch -- network,
 decode and batched NMS at the Evaler's settings -- from device-resident inputs, seeded synthetic weights): 640 px batch 32
-for the P5 models, 1280 px batch 8 for the P6 ones.  Each line also carries the conv GFLOP per image of the graph (2 x MACs
+for the P5 models, 1280 px batch 8 for the P6 ones, and 320 px (the Lite models' deploy size) at batch 32 and batch 1 for
+YOLOv6Lite.  For each Lite model two more lines: the device time of every launch of one bf16 forward timed on its own,
+summed per kind (wgmma convs against the depthwise / squeeze-excite / shuffle / upsample kernels), and the same network run
+eagerly through PyTorch / cuDNN (oracle/lite.py in bf16, channels_last) on the same GPU, as the comparison point.  Each line also carries the conv GFLOP per image of the graph (2 x MACs
 of every conv, transposed conv and prediction conv at that size).  The training step (TrainStep, CUDA graph, TAL or ATSS by
 the config's atss_warmup_epoch at epoch 0, no optimizer) is timed for YOLOv6-S-MBLA (640, bs32) and YOLOv6-N6 (1280, bs8).
 One JSON line per measurement; the first line names the card, its power limit and its maximum SM clock, read in the same run.
@@ -21,21 +24,23 @@ import torch  # noqa: E402
 
 import bench  # noqa: E402
 from yolov6_b200 import configs  # noqa: E402
-from yolov6_b200.arch import build_graph  # noqa: E402
+from yolov6_b200.arch import build_graph, is_lite  # noqa: E402
 
 TRAIN_CASES = [("yolov6s_mbla", 640, 32), ("yolov6n6", 1280, 8)]
 
 
 def native(name):
-    """(size, batch) of the measurement: 640 / 32 for P5 models, 1280 / 8 for P6 models."""
-    return (1280, 8) if len(configs.CONFIGS[name]["head"]["strides"]) == 4 else (640, 32)
+    """[(size, batch)] of the measurements: 640 / 32 for P5 models, 1280 / 8 for P6 models, 320 / 32 and 320 / 1 for Lite."""
+    if is_lite(configs.CONFIGS[name]):
+        return [(320, 32), (320, 1)]
+    return [(1280, 8) if len(configs.CONFIGS[name]["head"]["strides"]) == 4 else (640, 32)]
 
 
 def conv_gflop_per_image(g, size):
     """2 x multiply-accumulates of every conv of graph g (inference forward, eval head) on one size x size image."""
     flop = 0
     for op in g.ops:
-        if op.kind == "pool" or (op.kind == "pred" and op.head[0] not in ("cls", "reg")):
+        if op.kind in ("pool", "se", "shuffle", "up") or (op.kind == "pred" and op.head[0] not in ("cls", "reg")):
             continue
         if op.kind == "stem":
             lvl = 1
@@ -45,8 +50,41 @@ def conv_gflop_per_image(g, size):
             lvl = g.bufs[op.dst.buf].level
         hw = (size >> lvl) ** 2
         k = 2 if op.kind == "convT" else op.k        # a 2x2 stride-2 transposed conv: 4 taps per input pixel = 1 per output pixel
-        flop += 2 * hw * op.cout * op.cin * (1 if op.kind == "convT" else k * k)
+        flop += 2 * hw * op.cout * (1 if op.kind == "dw" else op.cin) * (1 if op.kind == "convT" else k * k)
     return flop / 1e9
+
+
+def lite_split(name, size, batch, dev):
+    """Device ms of one bf16 forward, every launch timed alone: wgmma convs (stem included) against the Lite kernels."""
+    from yolov6_b200.model import build_model
+    from yolov6_b200.synth import randomize_
+    eng = randomize_(build_model(name, 80, dev), seed=0).eval().set_precision("bf16").engine()
+    x = torch.rand(batch, 3, size, size, device=dev)
+    rows = eng.profile_calls(x)
+    per_kind = {}
+    for kind, _, ms in rows:
+        per_kind[kind] = per_kind.get(kind, 0.0) + ms
+    top = sorted(rows, key=lambda r: -r[2])[:8]
+    return {"model": name, "mode": "launch split bf16", "size": size, "batch": batch, "launches": len(rows),
+            "ms_by_kind": {k: round(v, 4) for k, v in per_kind.items()}, "slowest": [[k, n, round(ms, 4)] for k, n, ms in top]}
+
+
+def lite_eager(name, size, batch, steps, warmup, dev):
+    """The same network eagerly through PyTorch / cuDNN: oracle/lite.py's forward up to the head outputs (train-form weights,
+    BN applied as its own ops; no decode and no NMS, which the kernel path's figure includes) in bf16, channels_last, seeded
+    synthetic weights."""
+    from oracle import fabricate as fab
+    from oracle import lite
+    from yolov6_b200.arch import param_specs
+    keys = [(k, shape) for k, shape, _ in param_specs(build_graph(configs.get_config(name), 80))]
+    sd = {k: v.to(dev, torch.bfloat16) if v.is_floating_point() else v for k, v in fab.fabricate_state_dict(keys).items()}
+    sd = {k: v.contiguous(memory_format=torch.channels_last) if v.dim() == 4 else v for k, v in sd.items()}
+    x = torch.rand(batch, 3, size, size, device=dev, dtype=torch.bfloat16).contiguous(memory_format=torch.channels_last)
+    torch.backends.cudnn.benchmark = True
+    with torch.no_grad():
+        ms = bench.timed(lambda i: lite.forward(sd, lite.CONFIGS[name], x, train_outputs=True), steps, warmup, 1, dev)
+    return {"model": name, "mode": "eager PyTorch/cuDNN bf16 channels_last, network only", "size": size, "batch": batch, "ms_per_step": ms,
+            "images_per_s": batch / (ms * 1e-3)}
 
 
 def bench_train_step(name, size, batch, steps, warmup, dev):
@@ -79,13 +117,17 @@ def main():
     torch.cuda.set_device(dev)
     print(json.dumps({"gpu": bench.gpu_info(0)}), flush=True)
     for name in args.models.split(","):
-        size, batch = native(name)
-        r = bench.bench_infer(name, batch, size, args.steps, args.warmup, 0, 1, dev, precision="bf16", e2e=False, roofline=False)
-        print(json.dumps({"model": name, "mode": "infer bf16", "size": size, "batch": batch, "images_per_s": r["value"],
-                          "ms_per_step": r["ms_per_step"], "launches_per_step": r["launches_per_step"],
-                          "conv_gflop_per_image": conv_gflop_per_image(build_graph(configs.get_config(name), 80), size)}), flush=True)
-        del r
-        torch.cuda.empty_cache()
+        for size, batch in native(name):
+            r = bench.bench_infer(name, batch, size, args.steps, args.warmup, 0, 1, dev, precision="bf16", e2e=False, roofline=False)
+            print(json.dumps({"model": name, "mode": "infer bf16", "size": size, "batch": batch, "images_per_s": r["value"],
+                              "ms_per_step": r["ms_per_step"], "launches_per_step": r["launches_per_step"],
+                              "conv_gflop_per_image": conv_gflop_per_image(build_graph(configs.get_config(name), 80), size)}), flush=True)
+            del r
+            torch.cuda.empty_cache()
+            if is_lite(configs.CONFIGS[name]):
+                print(json.dumps(lite_eager(name, size, batch, args.steps, args.warmup, dev)), flush=True)
+                print(json.dumps(lite_split(name, size, batch, dev)), flush=True)
+                torch.cuda.empty_cache()
     if not args.no_train:
         for name, size, batch in TRAIN_CASES:
             print(json.dumps(bench_train_step(name, size, batch, args.steps, args.warmup, dev)), flush=True)

@@ -10,10 +10,10 @@ import threading
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libyolov6_b200.so")
 
-ACT_NONE, ACT_RELU, ACT_SILU, ACT_SIGMOID = 0, 1, 2, 3
+ACT_NONE, ACT_RELU, ACT_SILU, ACT_SIGMOID, ACT_HARDSWISH = 0, 1, 2, 3, 4
 DT_BF16, DT_F32, DT_U8 = 0, 1, 2
 PAD_SAME = -1000000
-ACT_CODES = {None: ACT_NONE, "none": ACT_NONE, "relu": ACT_RELU, "silu": ACT_SILU, "sigmoid": ACT_SIGMOID}
+ACT_CODES = {None: ACT_NONE, "none": ACT_NONE, "relu": ACT_RELU, "silu": ACT_SILU, "sigmoid": ACT_SIGMOID, "hardswish": ACT_HARDSWISH}
 
 
 class ConvDesc(C.Structure):
@@ -121,6 +121,25 @@ class PrState(C.Structure):
     ]
 
 
+class DwDesc(C.Structure):
+    """Mirror of `yv6_dw_desc` (include/yv6.h)."""
+    _fields_ = [
+        ("x", C.c_void_p), ("N", C.c_int32), ("H", C.c_int32), ("W", C.c_int32), ("C", C.c_int32),
+        ("x_c_total", C.c_int32), ("y_c_total", C.c_int32), ("x_plane_stride", C.c_int64), ("y_plane_stride", C.c_int64),
+        ("w", C.c_void_p), ("bias", C.c_void_p), ("k", C.c_int32), ("stride", C.c_int32), ("act", C.c_int32), ("nsplit", C.c_int32),
+        ("y", C.c_void_p),
+    ]
+
+
+class SeDesc(C.Structure):
+    """Mirror of `yv6_se_desc` (include/yv6.h)."""
+    _fields_ = [
+        ("x", C.c_void_p), ("N", C.c_int32), ("HW", C.c_int32), ("C", C.c_int32), ("Cr", C.c_int32),
+        ("c_total", C.c_int64), ("plane_stride", C.c_int64),
+        ("w1", C.c_void_p), ("b1", C.c_void_p), ("w2", C.c_void_p), ("b2", C.c_void_p), ("nsplit", C.c_int32), ("reserved0", C.c_int32),
+    ]
+
+
 XF_F32, XF_F64, XF_BF16 = 0, 1, 2
 XFORM_CHUNK = 4096
 
@@ -201,6 +220,12 @@ _SIGNATURES = {
                                C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p]),
     "yv6_pr_metric": (C.c_int, [C.c_void_p, C.POINTER(PrState), C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p,
                                 C.c_void_p]),
+    "yv6_dwconv_fwd": (C.c_int, [C.c_void_p, C.POINTER(DwDesc), C.c_void_p]),
+    "yv6_se_fwd": (C.c_int, [C.c_void_p, C.POINTER(SeDesc), C.c_void_p]),
+    "yv6_channel_shuffle": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_int32,
+                                      C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_void_p]),
+    "yv6_upsample2x": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
+                                 C.c_int64, C.c_int64, C.c_int32, C.c_void_p]),
     "yv6_nms_workspace_bytes": (C.c_int64, [C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
     "yv6_nms_batched": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_float, C.c_double,
                                   C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,

@@ -11,7 +11,9 @@ activation buffers, emitted once per (config, num_classes):
     (reppan.py:228,232, common.py:650,718 -> `dst=T(buf, c_off, c)`);
   * the engine (engine.py) walks the list and issues one kernel per op through the C ABI.
 
-Op kinds: stem | conv (rep / cba / cm / plain parameter layouts) | convT | pool.
+Op kinds: stem | conv (rep / cba / cm / plain / dp parameter layouts) | convT | pool, and for the YOLOv6Lite networks
+(build_lite_graph) dw (depthwise conv) | se (squeeze-excite, in place) | shuffle (channel_shuffle of two slices) | up (nearest
+2x upsample).
 """
 import math
 from dataclasses import dataclass, field
@@ -35,9 +37,9 @@ class Buf:
 
 @dataclass
 class Op:
-    kind: str                 # 'stem' | 'conv' | 'convT' | 'pool' | 'pred'
+    kind: str                 # 'stem' | 'conv' | 'convT' | 'pool' | 'pred' | 'dw' | 'se' | 'shuffle' | 'up'
     name: str                 # reference parameter prefix
-    layout: str = ""          # 'rep' | 'cba' | 'cm' (bare ConvModule) | 'plain' | 'convT'
+    layout: str = ""          # 'rep' | 'cba' | 'cm' (bare ConvModule) | 'plain' | 'convT' | 'dp' (a DPBlock conv: bias, bn_1 / bn_2)
     src: Optional[T] = None
     dst: Optional[T] = None
     cin: int = 0
@@ -52,6 +54,7 @@ class Op:
     # the op with w_row0 == 0 owns the parameter.  BatchNorm is per output channel, so the rows fold and train on their own.
     w_row0: int = 0
     w_rows: int = 0
+    src2: Optional[T] = None  # shuffle: the second source (y[2j] = src[j], y[2j+1] = src2[j])
 
     @property
     def param_rows(self):
@@ -70,6 +73,7 @@ class Graph:
     ops: List[Op] = field(default_factory=list)
     feat: List[T] = field(default_factory=list)   # neck outputs (reference `featmaps`, yolo.py:37-39)
     fuse_ab: bool = False
+    lite: bool = False                            # a YOLOv6Lite network (build_lite_graph): no DFL projection in the head
     anchors_init: Optional[list] = None           # fuse_ab: per level [w0, h0, w1, h1, w2, h2] in pixels
     distill_ns: bool = False
     dist_reg_ch: int = 0                          # distill_ns: channels of the DFL (reg_preds_dist) branch
@@ -235,10 +239,16 @@ def _bifusion(g, name, x0, x1, x2, cout):
 
 
 def build_graph(cfg, num_classes=80, name="yolov6", fuse_ab=False, distill_ns=False):
-    """cfg: dict with the fields of the reference's `config.model` (see configs.py / config_from_reference).
+    """The network of a normalised config (configs.normalize): build_lite_graph for the Lite_EffiBackbone ones, else below.
+
+    cfg: dict with the fields of the reference's `config.model` (see configs.py / config_from_reference).
     fuse_ab: add the anchor-aided training branch of effidehead_fuseab.py (two more 1x1 pred convs per level).
     distill_ns: the N / S student head of effidehead_distill_ns.py -- `reg_preds` emits the 4 (l, r, t, b) distances used at
     inference, `reg_preds_dist` the 4 * (reg_max + 1) DFL logits used by the distillation loss (training only)."""
+    if is_lite(cfg):
+        if fuse_ab or distill_ns:
+            raise ValueError("YOLOv6Lite has no fuse_ab or distill_ns head (yolo_lite.py builds only the Lite Detect)")
+        return build_lite_graph(cfg, num_classes, name)
     depth, width = cfg["depth_multiple"], cfg["width_multiple"]
     bb, nk, hd = cfg["backbone"], cfg["neck"], cfg["head"]
     reps = [(max(round(i * depth), 1) if i > 1 else i) for i in bb["num_repeats"] + nk["num_repeats"]]   # yolo.py:66
@@ -347,6 +357,150 @@ def build_graph(cfg, num_classes=80, name="yolov6", fuse_ab=False, distill_ns=Fa
     return g
 
 
+# ------------------------------------------------------------------------------------------------------------- YOLOv6Lite
+def is_lite(cfg):
+    return cfg["backbone"]["type"] == "Lite_EffiBackbone"
+
+
+def lite_divisible(v, divisor=16):
+    """make_divisible of yolo_lite.py (not arch.make_divisible): round to the nearest multiple, at least `divisor`, and not
+    below 90 % of v."""
+    new_v = max(divisor, int(v + divisor / 2) // divisor * divisor)
+    return new_v + divisor if new_v < 0.9 * v else new_v
+
+
+def lite_channels(cfg):
+    """(backbone out channels, backbone mid channels, neck in channels) of yolo_lite.build_network; the backbone forces
+    out[0] = 24 after the mid channels are computed (efficientrep.py:526)."""
+    width, bb = cfg["width_multiple"], cfg["backbone"]
+    out = [lite_divisible(i * width) for i in bb["out_channels"]]
+    mid = [lite_divisible(int(i * bb["scale_size"]), 8) for i in out]
+    out[0] = 24
+    return out, mid, [lite_divisible(i * width) for i in cfg["neck"]["in_channels"]]
+
+
+def _ceil16(c):
+    return (c + 15) // 16 * 16
+
+
+class LiteGraph(Graph):
+    """Every activation buffer has a channel pitch that is a multiple of 16 and zero pad channels, so a 1x1 conv can read the
+    16-aligned channel window around any slice (engine.conv_window) with zero weight columns outside it."""
+
+    def buf(self, level, c_total, name=""):
+        return super().buf(level, _ceil16(c_total), name)
+
+    def new(self, level, c, name=""):
+        return T(self.buf(level, c, name), 0, c)
+
+    def hs(self, name, src, cout, dst=None, res=None):
+        """ConvBNHS 1x1 (common.py:87-94)."""
+        return self.conv(name, "cba", src, cout, 1, 1, "hardswish", dst=dst, res=res)
+
+    def dw(self, name, layout, src, k, s, act, dst=None):
+        """Depthwise conv: ConvBN / ConvBNHS with groups = C ('cba') or DPBlock.conv_dw_1 ('dp')."""
+        lvl = self.level(src) + (1 if s == 2 else 0)
+        if dst is None:
+            dst = self.new(lvl, src.c, name)
+        assert dst.c == src.c and self.level(dst) == lvl, (name, dst, src)
+        self.ops.append(Op("dw", name, layout, src, dst, src.c, src.c, k, s, act))
+        return dst
+
+    def se(self, name, t):
+        """SEBlock (common.py:740-768), in place on slice t; reduction 4."""
+        self.ops.append(Op("se", name, "se", t, t, t.c, t.c // 4))
+
+    def dp(self, name, src, k, s, dst=None, res=None):
+        """DPBlock (common.py:900-934): hardswish(BN(dw k x k + bias)) -> hardswish(BN(1x1 + bias)) [+ res]."""
+        t = self.dw(name + ".conv_dw_1", "dp", src, k, s, "hardswish")
+        return self.conv(name + ".conv_pw_1", "dp", t, src.c, 1, 1, "hardswish", dst=dst, res=res)
+
+
+def _lite_s2(g, p, x, mid, out):
+    """Lite_EffiBlockS2 (common.py:826-897), stride 2: cat(conv_1(dw_1 x), conv_2(se(dw_2(pw_2 x)))) -> dw_3 -> pw_3."""
+    cat = g.buf(g.level(x) + 1, out, p + ".cat")
+    g.hs(p + ".conv_1", g.dw(p + ".conv_dw_1", "cba", x, 3, 2, None), out // 2, dst=T(cat, 0, out // 2))
+    t = g.dw(p + ".conv_dw_2", "cba", g.hs(p + ".conv_pw_2", x, mid // 2), 3, 2, None)
+    g.se(p + ".se", t)
+    g.hs(p + ".conv_2", t, out // 2, dst=T(cat, out // 2, out // 2))
+    return g.hs(p + ".conv_pw_3", g.dw(p + ".conv_dw_3", "cba", T(cat, 0, out), 3, 1, "hardswish"), out)
+
+
+def _lite_s1(g, p, x, mid):
+    """Lite_EffiBlockS1 (common.py:783-823): x1, x2 = split(x); channel_shuffle(cat(x1, conv_1(se(dw_1(pw_1 x2)))), 2)."""
+    h = x.c // 2
+    t = g.dw(p + ".conv_dw_1", "cba", g.hs(p + ".conv_pw_1", T(x.buf, x.c_off + h, h), mid), 3, 1, None)
+    g.se(p + ".se", t)
+    x3 = g.hs(p + ".conv_1", t, h)
+    y = g.new(g.level(x), x.c, p)
+    g.ops.append(Op("shuffle", p + ".shuffle", src=T(x.buf, x.c_off, h), src2=x3, dst=y, cin=h, cout=x.c))
+    return y
+
+
+def _csp_lite(g, p, x, cout, dst=None):
+    """CSPBlock(k=5, e=0.5) of Lite_EffiNeck (common.py:937-985): conv_3(cat(DarknetBlock(conv_1 x), conv_2 x))."""
+    m = int(cout * 0.5)
+    cat = g.buf(g.level(x), 2 * m, p + ".cat")
+    g.dp(p + ".blocks.conv_2", g.hs(p + ".blocks.conv_1", g.hs(p + ".conv_1", x, m), m), 5, 1, dst=T(cat, 0, m))
+    g.hs(p + ".conv_2", x, m, dst=T(cat, m, m))
+    return g.hs(p + ".conv_3", T(cat, 0, 2 * m), cout, dst=dst)
+
+
+def build_lite_graph(cfg, num_classes=80, name="yolov6lite"):
+    """YOLOv6Lite (yolo_lite.py:49-76): Lite_EffiBackbone (efficientrep.py:518-582), Lite_EffiNeck (reppan.py:1118-1226) and the
+    Lite decoupled head (effidehead_lite.py): k5 DPBlock stems / cls / reg convs, 1x1 preds, reg used directly as ltrb distances.
+    Physical channel order is the reference's order, so torch.split is a slice and every intermediate compares directly."""
+    bb, nk, hd = cfg["backbone"], cfg["neck"], cfg["head"]
+    if nk["type"] != "Lite_EffiNeck" or hd["num_layers"] != 4:
+        raise NotImplementedError(f"Lite_EffiBackbone with neck {nk['type']} / {hd['num_layers']} levels is outside the hot-path scope")
+    out, mid, neck_in = lite_channels(cfg)
+    g = LiteGraph(name, num_classes, list(hd["strides"]), False, 0, "lite")
+    g.lite = True
+    stem = g.new(1, out[0], "backbone.conv_0")
+    g.ops.append(Op("stem", "backbone.conv_0", "cba", None, stem, 3, out[0], 3, 2, "hardswish"))
+    x, feats = stem, []
+    for s in range(1, 5):
+        p = f"backbone.lite_effiblock_{s}"
+        for i in range(bb["num_repeats"][s - 1]):
+            x = _lite_s2(g, f"{p}.{i}", x, mid[s], out[s]) if i == 0 else _lite_s1(g, f"{p}.{i}", x, mid[s])
+        if s >= 2:
+            feats.append(x)
+    x2, x1, x0 = feats
+    assert [x0.c, x1.c, x2.c] == neck_in, (neck_in, [x0.c, x1.c, x2.c])
+    U = nk["unified_channels"]
+    f_cat0 = g.buf(g.level(x1), 2 * U, "neck.f_concat_layer0")      # [upsample_feat0, reduce_layer1(x1)]
+    f_cat1 = g.buf(g.level(x2), 2 * U, "neck.f_concat_layer1")      # [upsample_feat1, reduce_layer2(x2)]
+    p_cat1 = g.buf(g.level(x1), 2 * U, "neck.p_concat_layer1")      # [down_feat1, f_out1]
+    p_cat2 = g.buf(g.level(x0), 2 * U, "neck.p_concat_layer2")      # [down_feat0, fpn_out0]
+    fpn0 = g.hs("neck.reduce_layer0", x0, U, dst=T(p_cat2, U, U))
+    g.hs("neck.reduce_layer1", x1, U, dst=T(f_cat0, U, U))
+    g.hs("neck.reduce_layer2", x2, U, dst=T(f_cat1, U, U))
+    g.ops.append(Op("up", "neck.upsample0", src=fpn0, dst=T(f_cat0, 0, U), cin=U, cout=U))
+    f_out1 = _csp_lite(g, "neck.Csp_p4", T(f_cat0, 0, 2 * U), U, dst=T(p_cat1, U, U))
+    g.ops.append(Op("up", "neck.upsample1", src=f_out1, dst=T(f_cat1, 0, U), cin=U, cout=U))
+    pan3 = _csp_lite(g, "neck.Csp_p3", T(f_cat1, 0, 2 * U), U)
+    g.dp("neck.downsample2", pan3, 5, 2, dst=T(p_cat1, 0, U))
+    pan2 = _csp_lite(g, "neck.Csp_n3", T(p_cat1, 0, 2 * U), U)
+    g.dp("neck.downsample1", pan2, 5, 2, dst=T(p_cat2, 0, U))
+    pan1 = _csp_lite(g, "neck.Csp_n4", T(p_cat2, 0, 2 * U), U)
+    top = g.dp("neck.p6_conv_1", fpn0, 5, 2)
+    pan0 = g.dp("neck.p6_conv_2", pan1, 5, 2, res=top)               # top_features + p6_conv_2(pan_out1): hardswish, then add
+    g.feat = [pan3, pan2, pan1, pan0]
+    for i, f in enumerate(g.feat):
+        st = g.dp(f"detect.stems.{i}", f, 5, 1)
+        cf = g.dp(f"detect.cls_convs.{i}", st, 5, 1)
+        rf = g.dp(f"detect.reg_convs.{i}", st, 5, 1)
+        g.ops.append(Op("pred", f"detect.cls_preds.{i}", "plain", cf, None, U, num_classes, 1, 1, "sigmoid", head=("cls", i)))
+        g.ops.append(Op("pred", f"detect.reg_preds.{i}", "plain", rf, None, U, 4, 1, 1, None, head=("reg", i)))
+    return g
+
+
+def dp_bn(name):
+    """The BatchNorm of a DPBlock conv: conv_dw_1 -> bn_1, conv_pw_1 -> bn_2 (common.py:908-923)."""
+    parent, leaf = name.rsplit(".", 1)
+    return parent + (".bn_1" if leaf == "conv_dw_1" else ".bn_2")
+
+
 def param_specs(g):
     """(name, shape, kind) of every tensor in the reference state_dict that this graph owns.
     kind in {'conv', 'bn', 'bias', 'alpha', 'buffer', 'const'}; BN expands to its five tensors."""
@@ -362,7 +516,12 @@ def param_specs(g):
     seen_alpha = set()
     for op in g.ops:
         n = op.name
-        if op.kind == "pool":
+        if op.kind in ("pool", "shuffle", "up"):
+            continue
+        if op.kind == "se":
+            cr = op.cin // 4
+            specs += [(n + ".conv1.weight", (cr, op.cin, 1, 1), "conv"), (n + ".conv1.bias", (cr,), "bias"),
+                      (n + ".conv2.weight", (op.cin, cr, 1, 1), "conv"), (n + ".conv2.bias", (op.cin,), "bias")]
             continue
         if op.alpha and op.alpha not in seen_alpha:
             seen_alpha.add(op.alpha)
@@ -375,8 +534,12 @@ def param_specs(g):
             specs.append((n + ".rbr_1x1.conv.weight", (op.cout, op.cin, 1, 1), "conv"))
             bn(n + ".rbr_1x1.bn", op.cout)
         elif op.layout == "cba":
-            specs.append((n + ".block.conv.weight", (op.cout, op.cin, op.k, op.k), "conv"))
+            specs.append((n + ".block.conv.weight", (op.cout, 1 if op.kind == "dw" else op.cin, op.k, op.k), "conv"))
             bn(n + ".block.bn", op.cout)
+        elif op.layout == "dp":
+            specs.append((n + ".weight", (op.cout, 1 if op.kind == "dw" else op.cin, op.k, op.k), "conv"))
+            specs.append((n + ".bias", (op.cout,), "bias"))
+            bn(dp_bn(n), op.cout)
         elif op.layout == "cm":
             if op.w_row0 == 0:
                 specs.append((n + ".conv.weight", (op.param_rows, op.cin, op.k, op.k), "conv"))
@@ -387,6 +550,8 @@ def param_specs(g):
         elif op.layout == "convT":
             specs.append((n + ".upsample_transpose.weight", (op.cin, op.cout, 2, 2), "conv"))
             specs.append((n + ".upsample_transpose.bias", (op.cout,), "bias"))
+    if g.lite:       # the Lite Detect has no DFL projection (effidehead_lite.py:10-45)
+        return specs
     # build_network does not forward reg_max to Detect (yolo.py:130-131), so its DFL projection always
     # has Detect's default reg_max = 16 entries even for the N/S models that predict 4 reg channels.
     specs.append(("detect.proj", (DETECT_DEFAULT_REG_MAX + 1,), "const"))

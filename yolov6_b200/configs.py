@@ -1,5 +1,6 @@
 """Built-in model configurations (the `model` dict and `training_mode` of reference configs/yolov6{n,s,m,l,n6,s6,m6,l6}.py and
-configs/mbla/yolov6{s,m,l,x}_mbla.py; `training_mode` defaults to "repvgg" as tools/train.py:99-100 does) so that
+configs/mbla/yolov6{s,m,l,x}_mbla.py, and the YOLOv6Lite models of configs/yolov6_lite/yolov6_lite_{s,m,l}.py under their release
+names yolov6lite_{s,m,l}; `training_mode` defaults to "repvgg" as tools/train.py:99-100 does) so that
 tests, smoke() and bench.py run where /root/reference is not mounted, plus a normaliser that accepts
 the reference's own mmcv-style Config object (yolov6/utils/config.py) for drop-in use."""
 import copy
@@ -81,16 +82,30 @@ CONFIGS.update({"yolov6s_mbla": _mbla(0.5, 0.5), "yolov6m_mbla": _mbla(0.5, 0.75
                 "yolov6x_mbla": _mbla(1.0, 1.0)})
 
 
+def _lite(kind, width):
+    """configs/yolov6_lite/yolov6_lite_{s,m,l}.py: one network at three widths; no depth_multiple, no training_mode."""
+    return dict(
+        type=f"YOLOv6-lite-{kind}", width_multiple=width,
+        backbone=dict(type="Lite_EffiBackbone", num_repeats=[1, 3, 7, 3], out_channels=[24, 32, 64, 128, 256], scale_size=0.5),
+        neck=dict(type="Lite_EffiNeck", in_channels=[256, 128, 64], unified_channels=96),
+        head=dict(type="Lite_EffideHead", in_channels=[96, 96, 96, 96], num_layers=4, anchors=1, strides=[8, 16, 32, 64],
+                  atss_warmup_epoch=4, iou_type="siou", use_dfl=False, reg_max=0))
+
+
+CONFIGS.update({"yolov6lite_s": _lite("s", 0.7), "yolov6lite_m": _lite("m", 1.1), "yolov6lite_l": _lite("l", 1.5)})
+
+
 def get_config(name):
     return copy.deepcopy(CONFIGS[name])
 
 
 def normalize(cfg):
     """Accept a built-in name, one of the dicts above, or the reference's Config (attribute access,
-    `.model.{depth_multiple,width_multiple,backbone,neck,head}`, `.training_mode`) -> plain dict."""
+    `.model.{depth_multiple,width_multiple,backbone,neck,head}`, `.training_mode`; the Lite configs have `.model.type` and
+    no depth_multiple) -> plain dict."""
     if isinstance(cfg, str):
         return get_config(cfg)
-    if isinstance(cfg, dict) and "depth_multiple" in cfg:
+    if isinstance(cfg, dict) and "backbone" in cfg:
         return copy.deepcopy(cfg)
     model = cfg["model"] if isinstance(cfg, dict) else cfg.model
     get = (lambda o, k, d=None: o.get(k, d)) if hasattr(model, "get") else (lambda o, k, d=None: getattr(o, k, d))
@@ -98,4 +113,7 @@ def normalize(cfg):
     out = dict(training_mode=mode, depth_multiple=get(model, "depth_multiple"), width_multiple=get(model, "width_multiple"))
     for part in ("backbone", "neck", "head"):
         out[part] = {k: (list(v) if isinstance(v, (list, tuple)) else v) for k, v in dict(get(model, part)).items()}
+    if "YOLOv6-lite" in str(get(model, "type", "")):      # the trainer's Lite dispatch (core/engine.py:413-416)
+        out = dict(type=get(model, "type"), width_multiple=out["width_multiple"], backbone=out["backbone"], neck=out["neck"],
+                   head=out["head"])
     return out

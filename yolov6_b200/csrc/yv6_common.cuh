@@ -163,6 +163,8 @@ __device__ __forceinline__ float act_apply(float v, int act) {
     case YV6_ACT_RELU: return fmaxf(v, 0.f);
     case YV6_ACT_SILU: return v / (1.f + expf(-v));
     case YV6_ACT_SIGMOID: return 1.f / (1.f + expf(-v));
+    case YV6_ACT_HARDSWISH: return v * fminf(fmaxf(v + 3.f, 0.f), 6.f) * (1.f / 6.f);
+    case YV6_ACT_HARDSIGMOID: return fminf(fmaxf(v + 3.f, 0.f), 6.f) * (1.f / 6.f);
     default: return v;
   }
 }

@@ -258,6 +258,9 @@ __device__ __forceinline__ void epilogue_math(const ConvKParams& p, const float*
   } else if (p.act == YV6_ACT_SIGMOID) {
 #pragma unroll
     for (int j = 0; j < 16; ++j) v[j] = rcp_ftz(1.f + ex2_ftz(-1.4426950408889634f * v[j]));
+  } else if (p.act == YV6_ACT_HARDSWISH) {  // the YOLOv6Lite ConvBNHS convs
+#pragma unroll
+    for (int j = 0; j < 16; ++j) v[j] = v[j] * fminf(fmaxf(v[j] + 3.f, 0.f), 6.f) * (1.f / 6.f);   // no division: it would bring a CALL
   }
   if (p.res != nullptr && valid && ncol > 0) {
     for (int pl = 0; pl < p.res_planes; ++pl) {

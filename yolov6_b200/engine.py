@@ -17,7 +17,7 @@ import torch
 
 from . import _lib, ops
 from ._lib import ConvDesc
-from .fold import fold_op
+from .fold import fold_op, se_weights
 
 
 def siblings(g):
@@ -71,6 +71,31 @@ def pair_view(d, w_pair, plan_fn):
     return v if d.Cin <= 32 or plan_fn(v)["halo"] == 2 else d
 
 
+def conv_window(g, op):
+    """Input channels [lo, hi) a conv / pred launch reads.  On the Lite graphs (arch.LiteGraph: 16-aligned pitches, zero pad
+    channels) that is the 16-aligned window around the op's slice, so that the conv kernel's Cin % 16 == 0 and 16-byte
+    alignment hold for any slice; window_weights gives the columns outside the slice zero weight.  Elsewhere it is the slice."""
+    a, c = op.src.c_off, op.src.c
+    if not g.lite:
+        return a, a + c
+    return a // 16 * 16, (a + c + 15) // 16 * 16
+
+
+def window_weights(g, op, w):
+    """KRSC weights [Cout, k, k, Cin] of a conv / pred op -> [Cout, k, k, hi - lo] over its conv_window, zero outside the slice."""
+    lo, hi = conv_window(g, op)
+    if (lo, hi) == (op.src.c_off, op.src.c_off + op.src.c):
+        return w
+    out = w.new_zeros(w.shape[:3] + (hi - lo,))
+    out[..., op.src.c_off - lo:op.src.c_off - lo + op.src.c] = w
+    return out
+
+
+def stem_channels(g, op):
+    """Channels the stem writes: its buffer's pitch (the Lite stem: 24 real + 8 zero-weight channels, Hardswish(0) = 0)."""
+    return g.bufs[op.dst.buf].c_total
+
+
 def conv_launches(g, N, H, W, nsplit, sibling, addr, plan_fn):
     """Descriptors of the conv launches of one inference forward of graph g over an [N, 3, H, W] input, in launch order:
     {op index: [ConvDesc, ...]} -- four 1x1 quadrant launches for a transposed conv, one otherwise; the first conv of a sibling pair
@@ -105,7 +130,11 @@ def conv_launches(g, N, H, W, nsplit, sibling, addr, plan_fn):
         fused = i in sibling
         x, x_off, xs = view(op.src)
         k, s = (1, 1) if op.kind == "convT" else (op.k, op.s)
-        ws = (2 * op.cout if fused else op.cout, k, k, op.cin)
+        cin = op.cin
+        if op.kind != "convT":
+            lo, hi = conv_window(g, op)
+            x_off, cin = x_off - op.src.c_off + lo, hi - lo
+        ws = (2 * op.cout if fused else op.cout, k, k, cin)
         kw = dict(x_c_off=x_off, bias=addr("bias_fused" if fused else "bias", i), stride=s, act=op.act, nsplit=nsplit)
         if op.res is not None:
             r, r_off, (_, rh, rw, rct) = view(op.res)
@@ -160,14 +189,24 @@ class InferEngine:
 
         self.sibling = siblings(self.g) if self.fuse_siblings else {}
         for i, op in enumerate(self.g.ops):
-            if op.kind == "pool" or (op.kind == "pred" and op.head[0] not in ("cls", "reg")):   # fuse_ab / distillation preds: training only
+            if op.kind in ("pool", "shuffle", "up") or (op.kind == "pred" and op.head[0] not in ("cls", "reg")):   # fuse_ab / distillation preds: training only
+                continue
+            if op.kind == "se":
+                self.weights[i] = dict(zip(("w1", "b1", "w2", "b2"), (t.float().contiguous().to(dev) for t in se_weights(sd, op))))
                 continue
             w, b = fold_op(sd, op)
             ent = {}
             if op.kind == "stem":
+                cp = stem_channels(self.g, op)
+                w, b = torch.cat([w, w.new_zeros((cp - op.cout,) + w.shape[1:])]), torch.cat([b, b.new_zeros(cp - op.cout)])
                 ent["w_dev"] = w.float().permute(1, 2, 3, 0).contiguous().to(dev)       # [3][3][3][Cout]
                 ent["b_dev"] = b.float().contiguous().to(dev)
+            elif op.kind == "dw":
+                # fp32 [k*k][C]: the exact folded weights serve both precision modes and cost k*k*C*4 bytes per launch
+                ent["w_dev"] = w[..., 0].permute(1, 2, 0).reshape(op.k * op.k, op.cin).float().contiguous().to(dev)
+                ent["b_dev"] = b.float().contiguous().to(dev)
             else:
+                w = w if op.kind == "convT" else window_weights(self.g, op, w)
                 ws = w if isinstance(w, list) else [w]
                 ent["w"] = [planes(wi) for wi in ws]
                 if pair_view_candidate(op):      # [Cout][3][2][2*Cin] weights of the column-pair view (see pair_view)
@@ -247,12 +286,20 @@ class InferEngine:
             return (t[q] if kind == "w" else t).data_ptr()
 
         launches = conv_launches(g, N, H, W, P, self.sibling, addr, lambda d: ops.plan_of(d, dev.index or 0))
+
+        def slice_args(t):
+            """(address of the slice's first channel, channel pitch, plane stride) of a graph tensor slice."""
+            buf, c0 = view(t)
+            return buf.data_ptr() + 2 * c0, buf.shape[-1], buf.stride(0) if P == 3 else 0
+
+        plan["call_names"] = []
         for i, op in enumerate(g.ops):
+            lvl = g.bufs[op.src.buf].level if op.src is not None else 0
             if op.kind == "stem":
                 buf, _ = view(op.dst)
                 ent = self.weights[i]
-                d = ops.stem_desc(0, N, H, W, in_dtype == torch.uint8, ent["w_dev"].data_ptr(), ent["b_dev"].data_ptr(), op.cout, op.act,
-                                  buf.data_ptr(), P, buf.stride(0) if P == 3 else 0)
+                d = ops.stem_desc(0, N, H, W, in_dtype == torch.uint8, ent["w_dev"].data_ptr(), ent["b_dev"].data_ptr(), stem_channels(g, op),
+                                  op.act, buf.data_ptr(), P, buf.stride(0) if P == 3 else 0)
                 plan["stem"] = d
                 plan["calls"].append(("stem", d))
                 plan["deps"].append(dict(reads=[], writes=[span(op.dst)]))
@@ -261,6 +308,29 @@ class InferEngine:
                 h, w, ct = buf.shape[-3:]
                 plan["calls"].append(("pool", (buf.data_ptr(), N, h, w, op.cin, ct, P, buf.stride(0) if P == 3 else 0)))
                 plan["deps"].append(dict(reads=[(id(buf), 0, op.cin)], writes=[(id(buf), op.cin, 4 * op.cin)]))
+            elif op.kind == "dw":
+                ent = self.weights[i]
+                (x, xp, xpl), (y, yp, ypl) = slice_args(op.src), slice_args(op.dst)
+                d = ops.dw_desc(x, (N, H >> lvl, W >> lvl, xp), xpl, ent["w_dev"].data_ptr(), ent["b_dev"].data_ptr(), op.cin, op.k, op.s,
+                                op.act, y, yp, ypl, P)
+                plan["calls"].append(("dw", d))
+                plan["deps"].append(dict(reads=[span(op.src)], writes=[span(op.dst)]))
+            elif op.kind == "se":
+                ent = self.weights[i]
+                x, xp, xpl = slice_args(op.src)
+                d = ops.se_desc(x, N, (H >> lvl) * (W >> lvl), op.cin, op.cout, xp, xpl, *(ent[k].data_ptr() for k in ("w1", "b1", "w2", "b2")),
+                                nsplit=P)
+                plan["calls"].append(("se", d))
+                plan["deps"].append(dict(reads=[span(op.src)], writes=[span(op.src)]))
+            elif op.kind == "shuffle":
+                (a, ap, apl), (b, bp, bpl), (y, yp, ypl) = slice_args(op.src), slice_args(op.src2), slice_args(op.dst)
+                plan["calls"].append(("shuffle", (a, ap, apl, b, bp, bpl, N * (H >> lvl) * (W >> lvl), op.cin, y, yp, ypl, P)))
+                plan["deps"].append(dict(reads=[span(op.src), span(op.src2)], writes=[span(op.dst)]))
+            elif op.kind == "up":
+                (x, xp, xpl), (y, yp, ypl) = slice_args(op.src), slice_args(op.dst)
+                plan["calls"].append(("up", (x, xp, xpl, N, H >> lvl, W >> lvl, op.cin, y, yp, ypl, P)))
+                plan["deps"].append(dict(reads=[span(op.src)], writes=[span(op.dst)]))
+            plan["call_names"] += [op.name] * (len(plan["calls"]) - len(plan["call_names"]))
             for q, d in enumerate(launches.get(i, ())):
                 lvl = g.bufs[op.src.buf].level
                 sh, sw, k, s = H >> lvl, W >> lvl, d.kh, d.stride      # (of the 3x3 stride-2 conv, also on the column-pair view)
@@ -280,6 +350,7 @@ class InferEngine:
                     plan["neck_start"] = len(plan["calls"])     # first launch after the backbone (pipeline.DetectStream forks here)
                 plan["calls"].append(("conv", d))
                 plan["deps"].append(dict(reads=reads, writes=writes))
+                plan["call_names"].append(op.name)
         self._schedule(plan)
         self._plans[key] = plan
         return plan
@@ -385,12 +456,7 @@ class InferEngine:
                 for j in waits[i]:
                     streams[t].wait_event(events[j])
                 sp = sps[t]
-            if kind == "conv":
-                chk(lib.yv6_conv_fwd(h, C.byref(d), sp))
-            elif kind == "stem":
-                chk(lib.yv6_stem_fwd(h, C.byref(d), sp))
-            else:
-                chk(lib.yv6_sppf_pool(h, C.c_void_p(d[0]), d[1], d[2], d[3], d[4], d[5], d[6], d[7], sp))
+            self._launch(kind, d, sp)
             if multi and i in events:
                 events[i].record(streams[lane[i]])
         if multi:                                  # join: the caller's stream continues after every lane
@@ -406,6 +472,47 @@ class InferEngine:
                                 C.c_void_p(plan["pred"].data_ptr()), N, g.num_classes, 4 * (g.reg_max + 1),
                                 len(g.strides), plan["lvl_h"], plan["lvl_w"], plan["lvl_s"], sp))
         return plan["pred"]
+
+    def _launch(self, kind, d, sp):
+        lib, h, chk = self.lib, self.handle, _lib.check
+        if kind == "conv":
+            chk(lib.yv6_conv_fwd(h, C.byref(d), sp))
+        elif kind == "stem":
+            chk(lib.yv6_stem_fwd(h, C.byref(d), sp))
+        elif kind == "pool":
+            chk(lib.yv6_sppf_pool(h, C.c_void_p(d[0]), d[1], d[2], d[3], d[4], d[5], d[6], d[7], sp))
+        elif kind == "dw":
+            chk(lib.yv6_dwconv_fwd(h, C.byref(d), sp))
+        elif kind == "se":
+            chk(lib.yv6_se_fwd(h, C.byref(d), sp))
+        elif kind == "shuffle":
+            chk(lib.yv6_channel_shuffle(h, *d, sp))
+        elif kind == "up":
+            chk(lib.yv6_upsample2x(h, *d, sp))
+        else:
+            raise RuntimeError(f"no kernel for launch kind {kind!r}")
+
+    def profile_calls(self, x, steps=20, stream=None):
+        """Device time of every launch of one forward, each launched alone between CUDA events (serial, one stream):
+        [(kind, op name, ms)], the median over `steps` runs."""
+        x = x.contiguous()
+        N, _, H, W = x.shape
+        plan = self._plan(N, H, W, x.dtype if x.dtype == torch.uint8 else torch.float32)
+        self.forward(x, stream)
+        torch.cuda.synchronize()
+        sp = _lib.stream_ptr(stream)
+        rows = []
+        for (kind, d), name in zip(plan["calls"], plan["call_names"]):
+            ts = []
+            for _ in range(steps):
+                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                e0.record()
+                self._launch(kind, d, sp)
+                e1.record()
+                torch.cuda.synchronize()
+                ts.append(e0.elapsed_time(e1))
+            rows.append((kind, name, sorted(ts)[len(ts) // 2]))
+        return rows
 
     def head_outputs(self, N, H, W, in_dtype=torch.float32):
         """(cls [N,A,nc] post-sigmoid, reg [N,A,R] raw) of the last forward with this shape."""

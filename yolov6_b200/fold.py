@@ -8,6 +8,8 @@ final cast (the reference's own fold drifts its outputs by ~1e-4, SURVEY.md A.2)
 """
 import torch
 
+from .arch import dp_bn
+
 BN_EPS = 1e-3  # torch_utils.py:41-43
 
 
@@ -26,8 +28,13 @@ def fold_conv_bn(sd, p):
 
 
 def fold_op(sd, op):
-    """Returns (weight fp64 [Cout,kh,kw,Cin] (KRSC), bias fp64 [Cout]); convT returns 4 KRSC 1x1 weights."""
+    """Returns (weight fp64 [Cout,kh,kw,Cin] (KRSC), bias fp64 [Cout]); convT returns 4 KRSC 1x1 weights; a depthwise conv
+    (op.kind 'dw') returns [C,k,k,1]."""
     n = op.name
+    if op.layout == "dp":       # DPBlock conv with bias, then BN: scale * (conv + b) + shift (common.py:926-929)
+        scale, shift = _bn_affine(sd, dp_bn(n))
+        w = sd[n + ".weight"].double() * scale.view(-1, 1, 1, 1)
+        return w.permute(0, 2, 3, 1).contiguous(), sd[n + ".bias"].double() * scale + shift
     if op.layout == "rep":
         k3, b3 = fold_conv_bn(sd, n + ".rbr_dense")
         k1, b1 = fold_conv_bn(sd, n + ".rbr_1x1")
@@ -53,3 +60,10 @@ def fold_op(sd, op):
         quads = [w[:, :, dy, dx].t().contiguous().view(op.cout, 1, 1, op.cin) for dy in range(2) for dx in range(2)]
         return quads, sd[n + ".upsample_transpose.bias"].double()
     raise ValueError(op.layout)
+
+
+def se_weights(sd, op):
+    """SEBlock FCs, unfolded (common.py:745-757): (w1 [Cr, C], b1 [Cr], w2 [C, Cr], b2 [C]) in fp64."""
+    n = op.name
+    return (sd[n + ".conv1.weight"].double().flatten(1), sd[n + ".conv1.bias"].double(),
+            sd[n + ".conv2.weight"].double().flatten(1), sd[n + ".conv2.bias"].double())

@@ -88,6 +88,36 @@ class Detect(Node):
         self.proj_conv.weight.data.copy_(self.proj.view(1, self.reg_max + 1, 1, 1))
 
 
+class LiteDetect(Node):
+    """The YOLOv6Lite head (effidehead_lite.py:10-56): no DFL, so no use_dfl / reg_max / proj / proj_conv."""
+    export = False
+
+    def __init__(self, num_classes=80, num_layers=4):
+        super().__init__()
+        self.nc = num_classes
+        self.no = num_classes + 5
+        self.nl = num_layers
+        self.grid = [torch.zeros(1)] * num_layers
+        self.prior_prob = 1e-2
+        self.inplace = True
+        self.stride = torch.tensor([8, 16, 32] if num_layers == 3 else [8, 16, 32, 64])
+        self.grid_cell_offset = 0.5
+        self.grid_cell_size = 5.0
+
+    def initialize_biases(self):
+        """effidehead_lite.py:46-56: cls bias = -log((1-p)/p), reg bias = 1, pred weights = 0."""
+        for conv in self.cls_preds:
+            conv.bias.data.fill_(-math.log((1 - self.prior_prob) / self.prior_prob))
+            conv.weight.data.fill_(0.)
+        for conv in self.reg_preds:
+            conv.bias.data.fill_(1.0)
+            conv.weight.data.fill_(0.)
+
+
+LITE_TRAINING = ("training a YOLOv6Lite model is not supported: yolov6_b200 runs the Lite networks for inference only "
+                 "(no backward kernels for the depthwise, squeeze-excite, Hardswish and channel-shuffle layers)")
+
+
 class Model(nn.Module):
     export = False
 
@@ -102,8 +132,10 @@ class Model(nn.Module):
         g = self.graph
         hd = self.cfg["head"]
         self.backbone, self.neck = Node(), Node()
-        # build_network passes use_dfl but not reg_max to Detect (yolo.py:130-131)
-        self.detect = Detect(self.num_classes, hd["num_layers"], bool(hd["use_dfl"]), arch.DETECT_DEFAULT_REG_MAX)
+        if g.lite:
+            self.detect = LiteDetect(self.num_classes, hd["num_layers"])
+        else:   # build_network passes use_dfl but not reg_max to Detect (yolo.py:130-131)
+            self.detect = Detect(self.num_classes, hd["num_layers"], bool(hd["use_dfl"]), arch.DETECT_DEFAULT_REG_MAX)
         for name in (("stems", "cls_convs", "reg_convs", "cls_preds") + (("reg_preds_dist",) if self.distill_ns else ()) + ("reg_preds",) +
                      (("cls_preds_ab", "reg_preds_ab") if self.fuse_ab else ())):
             self.detect.add_module(name, Node())
@@ -140,7 +172,7 @@ class Model(nn.Module):
 
     def _materialize(self, g):
         for op in g.ops:
-            if op.kind == "pool":
+            if op.kind in ("pool", "shuffle", "up"):
                 continue
             path = op.name.split(".")
             root = getattr(self, path[0])
@@ -156,10 +188,19 @@ class Model(nn.Module):
                     b = _ensure(node, [br])
                     b.add_module("conv", nn.Conv2d(op.cin, op.cout, k, op.s, k // 2, bias=False))
                     b.add_module("bn", nn.BatchNorm2d(op.cout))
+            elif op.kind == "se":
+                node = _ensure(root, path[1:])
+                node.add_module("conv1", nn.Conv2d(op.cin, op.cin // 4, 1))
+                node.add_module("conv2", nn.Conv2d(op.cin // 4, op.cin, 1))
             elif op.layout == "cba":
                 b = _ensure(root, path[1:] + ["block"])
-                b.add_module("conv", nn.Conv2d(op.cin, op.cout, op.k, op.s, op.k // 2, bias=False))
+                b.add_module("conv", nn.Conv2d(op.cin, op.cout, op.k, op.s, op.k // 2, bias=False,
+                                               groups=op.cin if op.kind == "dw" else 1))
                 b.add_module("bn", nn.BatchNorm2d(op.cout))
+            elif op.layout == "dp":
+                node = _ensure(root, path[1:-1])
+                node.add_module(path[-1], nn.Conv2d(op.cin, op.cout, op.k, op.s, op.k // 2, groups=op.cin if op.kind == "dw" else 1))
+                node.add_module(arch.dp_bn(op.name).rsplit(".", 1)[1], nn.BatchNorm2d(op.cout))
             elif op.layout == "cm":
                 if op.w_row0 == 0:
                     node = _ensure(root, path[1:])
@@ -169,6 +210,8 @@ class Model(nn.Module):
                 _ensure(root, path[1:-1]).add_module(path[-1], nn.Conv2d(op.cin, op.cout, 1))
             elif op.layout == "convT":
                 _ensure(root, path[1:]).add_module("upsample_transpose", nn.ConvTranspose2d(op.cin, op.cout, 2, 2, bias=True))
+        if g.lite:
+            return
         R = arch.DETECT_DEFAULT_REG_MAX
         self.detect.proj = nn.Parameter(torch.linspace(0, R, R + 1), requires_grad=False)
         self.detect.add_module("proj_conv", nn.Conv2d(R + 1, 1, 1, bias=False))
@@ -205,6 +248,8 @@ class Model(nn.Module):
     def train_engine(self, n_buckets=None, rebuild=False):
         """The training engine of this model (train.py).  `n_buckets` > 1 splits the flat gradient buffer into that many
         contiguous buckets, completed one after the other during the backward pass (overlapped all-reduce, dist.py)."""
+        if self.graph.lite:
+            raise NotImplementedError(LITE_TRAINING)
         eng = self.__dict__.get("_train_engine")
         stale = eng is not None and (eng.dev != next(self.parameters()).device or not eng.flat.valid() or
                                      (n_buckets is not None and eng.n_buckets != n_buckets))
@@ -216,6 +261,8 @@ class Model(nn.Module):
 
     def forward(self, x):
         if self.training:
+            if self.graph.lite:
+                raise NotImplementedError(LITE_TRAINING)
             # train form (batch-stat BatchNorm, three-branch RepVGG) through the sm_90a training engine;
             # returns the reference's train-mode structure [(feats, cls, reg), featmaps] (yolo.py:33-41,
             # effidehead.py:72-92); `feats` carry only the level shapes ComputeLoss needs (loss.py:63-68)

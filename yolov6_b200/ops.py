@@ -7,7 +7,7 @@ import ctypes as C
 import torch
 
 from . import _lib
-from ._lib import ACT_CODES, DT_BF16, DT_F32, DT_U8, ConvDesc, StemDesc
+from ._lib import ACT_CODES, DT_BF16, DT_F32, DT_U8, ConvDesc, DwDesc, SeDesc, StemDesc
 
 # Names of the yv6_conv_plan (10) / yv6_conv_plan_host (12) output words.  a_res = A stages * 100 + CTA pair * 10 + B resident.
 PLAN_KEYS = ("BW", "BH", "BI", "BN", "KB", "stages", "grid", "tiles", "halo", "a_res", "smem", "threads")
@@ -113,6 +113,47 @@ def stem_desc(x, N, H, W, u8, w, bias, cout, act, y, nsplit=1, y_plane_stride=0,
     d.w, d.bias, d.Cout, d.act = w, bias, cout, ACT_CODES[act]
     d.y, d.y_plane_stride, d.nsplit, d.fp32_math = y, y_plane_stride, nsplit, fp32_math
     return d
+
+
+def dw_desc(x, x_shape, x_plane, w, bias, C, k, stride, act, y, y_pitch, y_plane=0, nsplit=1):
+    """yv6_dw_desc from device addresses: x / y point at the first channel of their slices; x_shape = (N, H, W, channel pitch);
+    w fp32 [k*k][C], bias fp32 [C] or 0."""
+    d = DwDesc()
+    d.x, (d.N, d.H, d.W, d.x_c_total), d.C = x, x_shape, C
+    d.y, d.y_c_total = y, y_pitch
+    d.x_plane_stride, d.y_plane_stride = (x_plane, y_plane) if nsplit == 3 else (0, 0)
+    d.w, d.bias, d.k, d.stride, d.act, d.nsplit = w, bias, k, stride, ACT_CODES[act], nsplit
+    return d
+
+
+def se_desc(x, N, HW, C, Cr, pitch, plane, w1, b1, w2, b2, nsplit=1):
+    """yv6_se_desc from device addresses: x is the first channel of the slice scaled in place."""
+    d = SeDesc()
+    d.x, d.N, d.HW, d.C, d.Cr, d.c_total, d.plane_stride = x, N, HW, C, Cr, pitch, plane if nsplit == 3 else 0
+    d.w1, d.b1, d.w2, d.b2, d.nsplit = w1, b1, w2, b2, nsplit
+    return d
+
+
+def dwconv_fwd(x, w, bias, y, *, k, stride=1, act=None, x_c_offset=0, y_c_offset=0, nsplit=1, stream=None):
+    """y[..., y_c_offset:+C] = act(depthwise_conv(x[..., x_c_offset:+C], w) + bias).  x / y: [N,H,W,pitch] bf16 ([3,...] when
+    nsplit=3); w fp32 [k*k][C]; bias fp32 [C] or None."""
+    planes = nsplit == 3
+    xs, ys = (x.shape[1:], y.shape[1:]) if planes else (x.shape, y.shape)
+    d = dw_desc(x.data_ptr() + 2 * x_c_offset, tuple(xs), x.stride(0) if planes else 0, w.data_ptr(),
+                bias.data_ptr() if bias is not None else 0, w.shape[1], k, stride, act, y.data_ptr() + 2 * y_c_offset, ys[-1],
+                y.stride(0) if planes else 0, nsplit)
+    _lib.check(_lib.lib().yv6_dwconv_fwd(_lib.handle(x.device.index or 0), C.byref(d), _lib.stream_ptr(stream)))
+    return y
+
+
+def se_fwd(x, w1, b1, w2, b2, *, c_offset=0, nsplit=1, stream=None):
+    """SEBlock in place on x[..., c_offset:+C] (x: [N,H,W,pitch] bf16, [3,...] when nsplit=3); w1 [Cr, C], w2 [C, Cr] fp32."""
+    planes = nsplit == 3
+    N, H, W, pitch = x.shape[1:] if planes else x.shape
+    d = se_desc(x.data_ptr() + 2 * c_offset, N, H * W, w1.shape[1], w1.shape[0], pitch, x.stride(0) if planes else 0,
+                w1.data_ptr(), b1.data_ptr(), w2.data_ptr(), b2.data_ptr(), nsplit)
+    _lib.check(_lib.lib().yv6_se_fwd(_lib.handle(x.device.index or 0), C.byref(d), _lib.stream_ptr(stream)))
+    return x
 
 
 def conv_fwd(x, w, bias, y, *, cin=None, x_c_offset=0, stride=1, act=None, y_c_offset=0,
