@@ -19,8 +19,10 @@
 //   * warpgroup 0 = TMA producer (one warp), warpgroups 1 and 2 = consumers in a ping-pong schedule: each owns
 //     every other tile of the CTA, issues wgmma m64nBNk16 for all 128 rows of it and keeps its accumulators in
 //     registers.  The two take turns on the tensor cores, so one's epilogue runs under the other's MMAs.
-//     The epilogue stages the fp32 tile in shared memory and writes it with coalesced 16-channel
-//     chunks (bias / activation / residual / dtype / bf16x3 planes / channel slices fused there).
+//     The epilogue adds the bias and applies the activation in registers, stages the tile in the output dtype and
+//     writes it with TMA bulk tensor stores through a third tensor map over the destination view (channel slice,
+//     ConvTranspose quadrant, head anchors).  Residual adds, bf16x3 output planes and views no tensor map can describe
+//     take the chunk epilogue: an fp32 staging tile written out in coalesced 16-channel chunks.
 //   * persistent CTAs (grid = #SMs) over a static tile schedule; smem ring of `stages` K-blocks
 //     (the producer runs ahead across tiles, so the next tile's loads overlap this tile's epilogue).
 //   * bf16x3 mode (nsplit=3): same kernel, K loop additionally runs over six (plane_a, plane_b)
@@ -68,6 +70,8 @@ struct ConvKParams {
   // L2 once per pair instead of once per CTA.  A ring stage may only be refilled once the consumers of BOTH CTAs released it.
   int32_t cpair, m_tiles, b_rows;
   int32_t fast_act;                        // bf16 outputs: SiLU through tanh.approx (rel. error 2^-11 < bf16 ulp)
+  // 1: the epilogue writes the tile through the output tensor map tmY (conditions in plan_conv); 0: in 16-channel chunks
+  int32_t tma_store;
 };
 
 constexpr int kHaloW = 10, kHaloH = 18;                   // BW = 8, BH = 16 output tile + 1-pixel border
@@ -84,9 +88,12 @@ struct HaloGeom {
 constexpr int kMaxAStages = 6, kMaxBStages = 40;
 
 // fp32 staging tile of the epilogue: 128 rows x BN columns, rows padded by 4 floats (16-byte aligned, fewer bank conflicts);
-// each consumer warpgroup owns 64 of the rows and writes its tile out through them in two passes
+// each consumer warpgroup owns 64 of the rows and writes its tile out through them in two passes.  The TMA-store epilogue
+// uses the same half differently: its first 256 x BN bytes hold the whole tile in bf16 (or 64 rows of it in fp32) for the
+// bulk tensor store, the 1 KB after them the tile's bias.
 __host__ __device__ constexpr int stage_pitch(int bn) { return bn + 4; }
 __host__ __device__ constexpr int staging_bytes(int bn) { return kTileRows * stage_pitch(bn) * 4; }
+static_assert(staging_bytes(32) / 2 == 256 * 32 + 1024, "the TMA-store tile and its bias fill one staging half");
 
 __device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* m, uint64_t* bar, int c0,
                                             int c1, int c2) {
@@ -106,6 +113,18 @@ __device__ __forceinline__ void tma_load_3d_mc(void* dst, const CUtensorMap* m, 
       "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "h"(mask)
       : "memory");
 }
+// Bulk tensor store of a shared-memory box to (c0, c1, c2, c3) of the output map (elements out of bounds are not written), in
+// the issuing thread's bulk async-group.
+__device__ __forceinline__ void tma_store_4d(const CUtensorMap* m, const void* src, int c0, int c1, int c2, int c3) {
+  asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];" ::"l"(
+                   reinterpret_cast<uint64_t>(m)), "r"(smem_u32(src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// the stores this thread committed have finished reading shared memory
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+// this thread's shared-memory writes become visible to the async proxy (the TMA unit)
+__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void warpgroup_bar_sync(int wg) {  // the 128 threads of consumer warpgroup wg (named barrier 1 + wg)
   asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
 }
@@ -223,15 +242,39 @@ __device__ __forceinline__ float tanh_fast(float x) {
   return y;
 }
 
+// the layer's activation on n values (after the bias), shared by both epilogues so that they round alike
+template <int N>
+__device__ __forceinline__ void activate(const ConvKParams& p, float (&v)[N]) {
+  if (p.act == YV6_ACT_RELU) {
+#pragma unroll
+    for (int j = 0; j < N; ++j) v[j] = fmaxf(v[j], 0.f);
+  } else if (p.act == YV6_ACT_SILU) {
+    if (p.fast_act) {                       // x * sigmoid(x) = h + h * tanh(h), h = x / 2: one MUFU per element
+#pragma unroll
+      for (int j = 0; j < N; ++j) {
+        const float h = 0.5f * v[j];
+        v[j] = fmaf(h, tanh_fast(h), h);
+      }
+    } else {                                // ex2 / rcp approximations are ~1e-7 relative
+#pragma unroll
+      for (int j = 0; j < N; ++j) v[j] = v[j] * rcp_ftz(1.f + ex2_ftz(-1.4426950408889634f * v[j]));
+    }
+  } else if (p.act == YV6_ACT_SIGMOID) {
+#pragma unroll
+    for (int j = 0; j < N; ++j) v[j] = rcp_ftz(1.f + ex2_ftz(-1.4426950408889634f * v[j]));
+  } else if (p.act == YV6_ACT_HARDSWISH) {  // the YOLOv6Lite ConvBNHS convs
+#pragma unroll
+    for (int j = 0; j < N; ++j) v[j] = v[j] * fminf(fmaxf(v[j] + 3.f, 0.f), 6.f) * (1.f / 6.f);   // no division: it would bring a CALL
+  }
+}
+
 // bias + activation (+ residual) for 16 consecutive output channels of one pixel
-__device__ __forceinline__ void epilogue_math(const ConvKParams& p, const float* sbias, const uint32_t (&r)[16], int n, int ncol,
-                                              bool valid, int64_t roff, float (&v)[16]) {
+__device__ __forceinline__ void epilogue_math(const ConvKParams& p, const uint32_t (&r)[16], int n, int ncol, int64_t roff,
+                                              float (&v)[16]) {
   if (p.bias != nullptr) {
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
-      // shared-memory copy (broadcast LDS) when staged; the global path costs an exposed L2 round trip per chunk
-      const float4 b = sbias ? *reinterpret_cast<const float4*>(sbias + n + 4 * j)
-                             : __ldg(reinterpret_cast<const float4*>(p.bias + n) + j);
+      const float4 b = __ldg(reinterpret_cast<const float4*>(p.bias + n) + j);
       v[4 * j + 0] = __uint_as_float(r[4 * j + 0]) + b.x;
       v[4 * j + 1] = __uint_as_float(r[4 * j + 1]) + b.y;
       v[4 * j + 2] = __uint_as_float(r[4 * j + 2]) + b.z;
@@ -241,28 +284,8 @@ __device__ __forceinline__ void epilogue_math(const ConvKParams& p, const float*
 #pragma unroll
     for (int j = 0; j < 16; ++j) v[j] = __uint_as_float(r[j]);
   }
-  if (p.act == YV6_ACT_RELU) {
-#pragma unroll
-    for (int j = 0; j < 16; ++j) v[j] = fmaxf(v[j], 0.f);
-  } else if (p.act == YV6_ACT_SILU) {
-    if (p.fast_act) {                       // x * sigmoid(x) = h + h * tanh(h), h = x / 2: one MUFU per element
-#pragma unroll
-      for (int j = 0; j < 16; ++j) {
-        const float h = 0.5f * v[j];
-        v[j] = fmaf(h, tanh_fast(h), h);
-      }
-    } else {                                // ex2 / rcp approximations are ~1e-7 relative
-#pragma unroll
-      for (int j = 0; j < 16; ++j) v[j] = v[j] * rcp_ftz(1.f + ex2_ftz(-1.4426950408889634f * v[j]));
-    }
-  } else if (p.act == YV6_ACT_SIGMOID) {
-#pragma unroll
-    for (int j = 0; j < 16; ++j) v[j] = rcp_ftz(1.f + ex2_ftz(-1.4426950408889634f * v[j]));
-  } else if (p.act == YV6_ACT_HARDSWISH) {  // the YOLOv6Lite ConvBNHS convs
-#pragma unroll
-    for (int j = 0; j < 16; ++j) v[j] = v[j] * fminf(fmaxf(v[j] + 3.f, 0.f), 6.f) * (1.f / 6.f);   // no division: it would bring a CALL
-  }
-  if (p.res != nullptr && valid && ncol > 0) {
+  activate(p, v);
+  if (p.res != nullptr) {
     for (int pl = 0; pl < p.res_planes; ++pl) {
       const __nv_bfloat16* rp = p.res + pl * p.res_plane_stride + roff + n;
       if (ncol == 16 && ((reinterpret_cast<uintptr_t>(rp) & 15) == 0)) {
@@ -280,6 +303,43 @@ __device__ __forceinline__ void epilogue_math(const ConvKParams& p, const float*
         for (int j = 0; j < 16; ++j)
           if (j < ncol) v[j] += p.alpha * __bfloat162float(rp[j]);
       }
+    }
+  }
+}
+
+// TMA-store epilogue: the output box is (y_box_bytes / element size) channels x the output tile, and its rows are y_box_bytes
+// long, which is also the swizzle span of the map (the widest of 128 / 64 bytes that divides a BN-wide row)
+__host__ __device__ constexpr int y_box_bytes(int bn, int esz) { return (bn * esz) % 128 == 0 ? 128 : 64; }
+
+// TMA-store epilogue: bias + activation on one accumulator half (rows row0 + 8 i, columns 8 j + c0, + 1 of this thread), rounded
+// to the output dtype and written to the staging half as the boxes of the output map: column group g (kCols channels) is a
+// [rows][kBox bytes] block at g * kGroupBytes in the map's swizzle, which XORs the 16-byte unit of a row with address bits 7+.
+template <int BN, bool F32>
+__device__ __forceinline__ void stage_out_tile(const ConvKParams& p, float (&acc)[BN / 2], const float* sbias, uint8_t* stage,
+                                               int row0, int c0) {
+  constexpr int kEsz = F32 ? 4 : 2, kBox = y_box_bytes(BN, kEsz), kCols = kBox / kEsz;
+  constexpr int kGroupBytes = (F32 ? 64 : 128) * kBox;
+  // this thread's rows are 8 apart and the staging half is 1024-byte aligned, so the XOR term is the same for all of them;
+  // the empty asm keeps the 16 per-column offsets below from being hoisted out of the tile loop and held in registers
+  int xr = (((row0 * kBox) >> 7) & (kBox / 16 - 1)) << 4;
+  asm volatile("" : "+r"(xr));
+  uint8_t* base = stage + row0 * kBox;
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j) {
+    float v[4] = {acc[4 * j], acc[4 * j + 1], acc[4 * j + 2], acc[4 * j + 3]};
+    if (p.bias != nullptr) {
+      const float2 b = *reinterpret_cast<const float2*>(sbias + 8 * j + c0);
+      v[0] += b.x;
+      v[1] += b.y;
+      v[2] += b.x;
+      v[3] += b.y;
+    }
+    activate(p, v);
+    uint8_t* dst = base + (8 * j / kCols) * kGroupBytes + ((((8 * j) % kCols + c0) * kEsz) ^ xr);
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      if (F32) *reinterpret_cast<float2*>(dst + 8 * i * kBox) = make_float2(v[2 * i], v[2 * i + 1]);
+      else *reinterpret_cast<uint32_t*>(dst + 8 * i * kBox) = pack_bf16x2(v[2 * i], v[2 * i + 1]);
     }
   }
 }
@@ -305,7 +365,8 @@ __device__ __forceinline__ void mma_kblock(float (&acc)[2][BN / 2], uint64_t ad,
 //       All are compile-time so that each variant carries only its own loops.
 template <int BN, int MODE, bool CP>
 __global__ void __launch_bounds__(kConvThreads, 1)
-conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const ConvKParams p) {
+conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                  const __grid_constant__ CUtensorMap tmY, const ConvKParams p) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_addr = smem_u32(smem_raw);
   uint8_t* smem = smem_raw + ((1024u - (raw_addr & 1023u)) & 1023u);
@@ -341,6 +402,7 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     if (lane == 0) {
       tma_prefetch_desc(&tmA);
       tma_prefetch_desc(&tmB);
+      if (p.tma_store) tma_prefetch_desc(&tmY);
     }
     // full barriers: the producer's expect_tx arrival; empty barriers: one arrival from the warpgroup that owns the stage's
     // tile (in both CTAs when the weight stages are multicast; the input-only a_empty ring of the halo modes stays per CTA);
@@ -471,7 +533,11 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     uint32_t pha = 0, phb = 0, turn_ph = 0;
     bool first = true;
     float* sCw = sC + wg * 64 * stage_pitch(BN);         // this warpgroup's half of the staging tile
+    float* sbias = sCw + 64 * BN;                        // TMA-store epilogue: the tile's bias, after the staged tile
     for (int tile = unit0 + wg * ustep; tile < num_tiles; tile += 2 * ustep) {
+      // TMA-store epilogue: the tile's bias goes to shared memory before the MMAs (this warpgroup's last epilogue read its
+      // previous contents before its final barrier), so that its load latency hides under the wait for the tensor cores
+      if (p.tma_store && p.bias != nullptr && ct < BN) sbias[ct] = __ldg(p.bias + coord(tile).n0 + ct);
       if (tile != unit0) {                               // the other warpgroup owns the preceding tile
         if constexpr (HALO) {
           skip_stages(sa, pha, pcs, p.a_stages);
@@ -565,12 +631,42 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       wgmma_fence_operand(acc[1]);
       first = false;
 
-      // ---- epilogue, in two 64-row passes: fragment -> this warpgroup's staging half -> coalesced 16-channel chunks
-      //      with the fused tail ----
       const TileCoord t = coord(tile);
+      const int r0 = (warp & 3) * 16 + (lane >> 2);      // this thread's fragment rows r0 + 8 i (+ 64 for acc[1]) and
+      const int c0 = 2 * (lane & 3);                     // columns 8 j + c0, + 1
+      if (p.tma_store) {
+        // ---- epilogue through the output tensor map: bias, activation and rounding in registers, the tile staged in the
+        //      output dtype (bf16: all 128 rows in one pass; fp32: one 64-row pass per accumulator half), one bulk tensor
+        //      store per column group.  The stores clip at the output's edges. ----
+        const bool f32 = p.y_dtype == YV6_DT_F32;
+        uint8_t* stage = reinterpret_cast<uint8_t*>(sCw);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          if (h == 1 && !f32) break;
+          if (ct == 0) bulk_wait_read();               // the last store has read the staging half
+          warpgroup_bar_sync(wg);
+          if (f32) {
+            stage_out_tile<BN, true>(p, acc[h], sbias, stage, r0, c0);
+          } else {
+            stage_out_tile<BN, false>(p, acc[0], sbias, stage, r0, c0);
+            stage_out_tile<BN, false>(p, acc[1], sbias, stage, r0 + 64, c0);
+          }
+          fence_proxy_async();
+          warpgroup_bar_sync(wg);
+          if (ct == 0) {
+            const int gcols = y_box_bytes(BN, f32 ? 4 : 2) / (f32 ? 4 : 2);
+            const int group_bytes = (f32 ? 64 : 128) * y_box_bytes(BN, f32 ? 4 : 2);
+            for (int g = 0; g * gcols < BN; ++g)
+              tma_store_4d(&tmY, stage + g * group_bytes, t.n0 + g * gcols, t.w0, t.h0 + h * (p.BH / 2), t.i0);
+            bulk_commit();
+            if (tile + 2 * ustep >= num_tiles) bulk_wait_read();   // the CTA's shared memory outlives the last store's reads
+          }
+        }
+        continue;
+      }
+      // ---- chunk epilogue (residual, bf16x3 planes, outputs a tensor map cannot describe), in two 64-row passes:
+      //      fragment -> this warpgroup's staging half -> coalesced 16-channel chunks with the fused tail ----
       constexpr int kChunks = BN / 16;
-      const int r0 = (warp & 3) * 16 + (lane >> 2);
-      const int c0 = 2 * (lane & 3);
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const int rows = min(64, p.rows - 64 * h);
@@ -608,7 +704,7 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             r[4 * q + 3] = __float_as_uint(f.w);
           }
           float v[16];
-          epilogue_math(p, nullptr, r, n, ncol, true, roff, v);
+          epilogue_math(p, r, n, ncol, roff, v);
           store_chunk(p, off, n, ncol, v);
         }
       }
@@ -848,6 +944,18 @@ static int plan_conv(const yv6_handle* h, const yv6_conv_desc* d, ConvPlan* plan
   k.res_plane_stride = d->res_plane_stride;
   k.bias = d->bias;
 
+  // Output through a tensor map (C, W, H, N) with boxes of (box_bytes / element size) channels x the BW x BH x BI tile:
+  // needs one output plane, no residual, a 16-byte aligned base and strides, and in fp32 (where one staging half holds 64
+  // rows) a 128-row tile split into two 64-row boxes along H.
+  {
+    const int esz = d->y_dtype == YV6_DT_F32 ? 4 : 2;
+    const int64_t strides[3] = {d->y_w_stride * esz, d->y_h_stride * esz, d->y_img_stride * esz};
+    bool ok = k.out_planes == 1 && d->res == nullptr && (reinterpret_cast<uintptr_t>(d->y) & 15) == 0;
+    for (int64_t s : strides) ok = ok && s > 0 && s % 16 == 0 && s < (1ll << 40);
+    if (esz == 4) ok = ok && k.BI == 1 && k.BH % 2 == 0 && k.BW * k.BH == kTileRows;
+    k.tma_store = ok ? 1 : 0;
+  }
+
   if (k.cpair) {   // grid counts CTAs: two per unit
     int clusters = std::min(k.num_tiles, h->max_clusters);
     if (d->force_grid > 0) clusters = std::min(k.num_tiles, std::max(1, d->force_grid / 2));
@@ -863,7 +971,7 @@ static int plan_conv(const yv6_handle* h, const yv6_conv_desc* d, ConvPlan* plan
 
 using namespace yv6;
 
-using ConvKernelFn = void (*)(const CUtensorMap, const CUtensorMap, const ConvKParams);
+using ConvKernelFn = void (*)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const ConvKParams);
 #define YV6_CONV_MODES(BN, CP)                                                                                      \
   {conv_igemm_kernel<BN, 0, CP>, conv_igemm_kernel<BN, 1, CP>, conv_igemm_kernel<BN, 2, CP>, conv_igemm_kernel<BN, 3, CP>, \
    conv_igemm_kernel<BN, 4, CP>}
@@ -1007,6 +1115,27 @@ extern "C" int yv6_conv_fwd(yv6_handle* h, const yv6_conv_desc* d, void* stream)
       return YV6_ERR_CUDA;
     }
   }
+  // Y: (C, W, H, N) over the destination view, for the TMA-store epilogue (unused, left zero, otherwise)
+  CUtensorMap tmY;
+  memset(&tmY, 0, sizeof(tmY));
+  if (k.tma_store) {
+    const bool f32 = d->y_dtype == YV6_DT_F32;
+    const uint64_t esz = f32 ? 4 : 2;
+    cuuint64_t dims[4] = {(cuuint64_t)d->Cout, (cuuint64_t)k.Wo, (cuuint64_t)k.Ho, (cuuint64_t)d->N};
+    cuuint64_t strides[3] = {(cuuint64_t)d->y_w_stride * esz, (cuuint64_t)d->y_h_stride * esz, (cuuint64_t)d->y_img_stride * esz};
+    const int box_bytes = y_box_bytes(k.BN, (int)esz);
+    cuuint32_t box[4] = {(cuuint32_t)(box_bytes / esz), (cuuint32_t)k.BW, (cuuint32_t)(f32 ? k.BH / 2 : k.BH), (cuuint32_t)k.BI};
+    cuuint32_t estr[4] = {1, 1, 1, 1};
+    CUresult cr = h->encode_tiled(&tmY, f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, d->y, dims,
+                                  strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                                  box_bytes == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
+                                  CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (cr != CUDA_SUCCESS) {
+      yv6_set_error("conv: cuTensorMapEncodeTiled(Y) failed with %d (C=%d W=%d H=%d N=%d strides=%lld,%lld,%lld)", (int)cr, d->Cout,
+                    k.Wo, k.Ho, d->N, (long long)d->y_w_stride, (long long)d->y_h_stride, (long long)d->y_img_stride);
+      return YV6_ERR_CUDA;
+    }
+  }
 
   const int mode = k.halo ? (k.halo == 2 ? 3 : 1) + (k.b_resident ? 1 : 0) : 0;
   const int bn_idx = k.BN == 32 ? 0 : k.BN == 64 ? 1 : k.BN == 96 ? 2 : 3;
@@ -1026,7 +1155,7 @@ extern "C" int yv6_conv_fwd(yv6_handle* h, const yv6_conv_desc* d, void* stream)
     cfg.attrs = attr;
     cfg.numAttrs = 1;
   }
-  YV6_CHECK_CUDA(cudaLaunchKernelEx(&cfg, fn, tmA, tmB, k));
+  YV6_CHECK_CUDA(cudaLaunchKernelEx(&cfg, fn, tmA, tmB, tmY, k));
   YV6_CHECK_CUDA(cudaGetLastError());
   return YV6_OK;
 }
