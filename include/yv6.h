@@ -510,6 +510,33 @@ typedef struct yv6_bn_stats_desc {
 int yv6_bn_stats_finalize(yv6_handle* h, const yv6_bn_stats_desc* d, void* stream);
 int yv6_bn_bwd(yv6_handle* h, const yv6_bn_desc* d, void* stream);
 
+/* QARepVGGBlock / QARepVGGBlockV2 (layers/common.py:322-477): the branch sum in front of the block's post-sum BatchNorm,
+ *   t = scale_d * u + shift_d + v [+ x [+ avg3x3(x)]]
+ * with u the raw 3x3 conv (BN_d = rbr_dense.bn), v the bare 1x1 conv, x the block input (identity, Cin == C at stride 1) and
+ * avg3x3 = AvgPool2d(3, 1, 1), which divides by 9 at the border too.  Any C and channel pitch; channels outside [0, C) are
+ * not written.
+ * yv6_qa_fwd: writes t (bf16) and, in the same launch, the float64 per-channel sum / sum of squares of the ROUNDED t into
+ *   sums [2][C] (zero on entry when zeroed != 0); the thread block that finishes last writes stats [4][C] = mean, invstd,
+ *   scale = gamma * invstd, shift = beta - mean * scale of the post-sum bn and updates its running statistics (may be NULL),
+ *   as yv6_bn_stats_finalize does.
+ * yv6_qa_bwd: the identity / avg part of the input gradient, dx (+)= dt + avg3x3^T(dt) (accumulate != 0: +=). */
+typedef struct yv6_qa_desc {
+  int32_t N, H, W, C;
+  const void* u; int64_t u_pitch;
+  const void* v; int64_t v_pitch;
+  const float* scale_d; const float* shift_d;           /* [C] each                                                        */
+  const void* x; int64_t x_pitch;                       /* NULL: no identity / avg branch                                  */
+  int32_t avg, accumulate;
+  void* t; int64_t t_pitch;
+  double* sums; uint32_t* counter; int32_t zeroed; float eps;
+  const float* gamma; const float* beta;
+  float* running_mean; float* running_var; float* stats; float momentum; int32_t reserved0;
+  const void* dt; int64_t dt_pitch;                     /* backward: gradient w.r.t. t                                     */
+  void* dx; int64_t dx_pitch;                           /* backward: gradient w.r.t. the block input                       */
+} yv6_qa_desc;
+int yv6_qa_fwd(yv6_handle* h, const yv6_qa_desc* d, void* stream);
+int yv6_qa_bwd(yv6_handle* h, const yv6_qa_desc* d, void* stream);
+
 /* Head gradients: level slice [off, off+hw) of the [B,A,ch] fp32 tensors -> dense NHWC bf16 [B,hw,ch_pad];
  * with `scores` the sigmoid backward dlogit = dscore * s * (1 - s) of effidehead.py:85 is applied. */
 int yv6_head_grad_prep(yv6_handle* h, const float* grad, const float* scores_or_null, int32_t B, int32_t A, int32_t ch,

@@ -9,7 +9,10 @@ YOLOv6Lite.  For each Lite model two more lines: the device time of every launch
 summed per kind (wgmma convs against the depthwise / squeeze-excite / shuffle / upsample kernels), and the same network run
 eagerly through PyTorch / cuDNN (oracle/lite.py in bf16, channels_last) on the same GPU, as the comparison point.  Each line also carries the conv GFLOP per image of the graph (2 x MACs
 of every conv, transposed conv and prediction conv at that size).  The training step (TrainStep, CUDA graph, TAL or ATSS by
-the config's atss_warmup_epoch at epoch 0, no optimizer) is timed for YOLOv6-S-MBLA (640, bs32) and YOLOv6-N6 (1280, bs8).
+the config's atss_warmup_epoch at epoch 0, no optimizer) is timed for YOLOv6-S-MBLA (640, bs32), YOLOv6-N6 (1280, bs8) and
+YOLOv6-S-QA next to YOLOv6-S (640, bs32).  For those two a further line splits one training step into its launches, each run
+alone and summed per kind, with the achieved bandwidth of the QA kernels (yv6_qa_fwd / yv6_qa_bwd) over the bytes their shapes
+imply, against the H100 SXM data-sheet 3.35 TB/s.
 One JSON line per measurement; the first line names the card, its power limit and its maximum SM clock, read in the same run.
 """
 import argparse
@@ -26,7 +29,9 @@ import bench  # noqa: E402
 from yolov6_b200 import configs  # noqa: E402
 from yolov6_b200.arch import build_graph, is_lite  # noqa: E402
 
-TRAIN_CASES = [("yolov6s_mbla", 640, 32), ("yolov6n6", 1280, 8)]
+TRAIN_CASES = [("yolov6s_mbla", 640, 32), ("yolov6n6", 1280, 8), ("yolov6s_qa", 640, 32), ("yolov6s", 640, 32)]
+SPLIT_CASES = [("yolov6s_qa", 640, 32), ("yolov6s", 640, 32)]
+HBM_BYTES_PER_S = 3.35e12       # H100 SXM data sheet
 
 
 def native(name):
@@ -106,17 +111,76 @@ def bench_train_step(name, size, batch, steps, warmup, dev):
             "assigner": "ATSS" if hd["atss_warmup_epoch"] > 0 else "TAL", "step": "TrainStep (CUDA graph), no optimizer"}
 
 
+def train_split(name, size, batch, dev, reps=5):
+    """Device ms of every launch of one training step (the training engine's forward and backward call lists), each run alone
+    after the per-step accumulators are cleared, median of `reps`, summed per kind.  yv6_qa_fwd moves u, v, t and (with the
+    identity branch) x once each, yv6_qa_bwd dt and dx (read too when it accumulates): 2 bytes per element."""
+    from yolov6_b200 import _lib
+    from yolov6_b200.model import build_model
+    from yolov6_b200.synth import randomize_
+    model = randomize_(build_model(name, 80, dev), seed=0).train()
+    eng = model.train_engine()
+    x = torch.rand(batch, 3, size, size, device=dev)
+    cls, reg = eng.forward(x)
+    eng.backward(torch.randn_like(cls) * 1e-3, torch.randn_like(reg) * 1e-3)
+    torch.cuda.synchronize()
+    sp = _lib.stream_ptr()
+
+    def timed(fn):
+        ts = []
+        for _ in range(reps):
+            eng.zero_arena.zero_()
+            a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            a.record()
+            fn()
+            b.record()
+            b.synchronize()
+            ts.append(a.elapsed_time(b))
+        return sorted(ts)[reps // 2]
+
+    fwd_ms, bwd_ms, qa = {}, {}, {"qa_fwd": [0.0, 0], "qa_bwd": [0.0, 0]}
+    calls = eng.fwd_calls
+    try:
+        for c in calls:
+            eng.fwd_calls = [c]
+            ms = timed(lambda: eng.run_forward(sp))
+            fwd_ms[c[0]] = fwd_ms.get(c[0], 0.0) + ms
+            if c[0] == "qa":
+                d = c[1]
+                qa["qa_fwd"][0] += ms
+                qa["qa_fwd"][1] += 2 * d.N * d.H * d.W * d.C * (3 + (1 if d.x else 0))
+    finally:
+        eng.fwd_calls = calls
+    for j, c in enumerate(eng.bwd_calls):
+        if c[0] in ("dbg", "bucket"):
+            continue
+        ms = timed(lambda: eng.backward(None, None, first=j, last=j + 1))
+        bwd_ms[c[0]] = bwd_ms.get(c[0], 0.0) + ms
+        if c[0] == "qa_bwd":
+            d = c[1]
+            qa["qa_bwd"][0] += ms
+            qa["qa_bwd"][1] += 2 * d.N * d.H * d.W * d.C * (2 + d.accumulate)
+    out = {"model": name, "mode": "train launch split", "size": size, "batch": batch,
+           "fwd_ms_by_kind": {k: round(v, 4) for k, v in fwd_ms.items()}, "bwd_ms_by_kind": {k: round(v, 4) for k, v in bwd_ms.items()}}
+    for k, (ms, nbytes) in qa.items():
+        if ms:
+            out[k] = {"ms": round(ms, 4), "bytes": nbytes, "GB_per_s": round(nbytes / (ms * 1e-3) / 1e9, 1),
+                      "frac_of_hbm_peak": round(nbytes / (ms * 1e-3) / HBM_BYTES_PER_S, 3)}
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=30)
     ap.add_argument("--warmup", type=int, default=10)
     ap.add_argument("--models", default=",".join(configs.CONFIGS))
     ap.add_argument("--no-train", action="store_true")
+    ap.add_argument("--train-only", action="store_true", help="skip the inference sweep")
     args = ap.parse_args()
     dev = torch.device("cuda:0")
     torch.cuda.set_device(dev)
     print(json.dumps({"gpu": bench.gpu_info(0)}), flush=True)
-    for name in args.models.split(","):
+    for name in ([] if args.train_only else args.models.split(",")):
         for size, batch in native(name):
             r = bench.bench_infer(name, batch, size, args.steps, args.warmup, 0, 1, dev, precision="bf16", e2e=False, roofline=False)
             print(json.dumps({"model": name, "mode": "infer bf16", "size": size, "batch": batch, "images_per_s": r["value"],
@@ -131,6 +195,9 @@ def main():
     if not args.no_train:
         for name, size, batch in TRAIN_CASES:
             print(json.dumps(bench_train_step(name, size, batch, args.steps, args.warmup, dev)), flush=True)
+            torch.cuda.empty_cache()
+        for name, size, batch in SPLIT_CASES:
+            print(json.dumps(train_split(name, size, batch, dev)), flush=True)
             torch.cuda.empty_cache()
 
 

@@ -140,6 +140,20 @@ class SeDesc(C.Structure):
     ]
 
 
+class QaDesc(C.Structure):
+    """Mirror of `yv6_qa_desc` (include/yv6.h)."""
+    _fields_ = [
+        ("N", C.c_int32), ("H", C.c_int32), ("W", C.c_int32), ("C", C.c_int32),
+        ("u", C.c_void_p), ("u_pitch", C.c_int64), ("v", C.c_void_p), ("v_pitch", C.c_int64),
+        ("scale_d", C.c_void_p), ("shift_d", C.c_void_p), ("x", C.c_void_p), ("x_pitch", C.c_int64),
+        ("avg", C.c_int32), ("accumulate", C.c_int32), ("t", C.c_void_p), ("t_pitch", C.c_int64),
+        ("sums", C.c_void_p), ("counter", C.c_void_p), ("zeroed", C.c_int32), ("eps", C.c_float),
+        ("gamma", C.c_void_p), ("beta", C.c_void_p), ("running_mean", C.c_void_p), ("running_var", C.c_void_p),
+        ("stats", C.c_void_p), ("momentum", C.c_float), ("reserved0", C.c_int32),
+        ("dt", C.c_void_p), ("dt_pitch", C.c_int64), ("dx", C.c_void_p), ("dx_pitch", C.c_int64),
+    ]
+
+
 XF_F32, XF_F64, XF_BF16 = 0, 1, 2
 XFORM_CHUNK = 4096
 
@@ -222,6 +236,8 @@ _SIGNATURES = {
                                 C.c_void_p]),
     "yv6_dwconv_fwd": (C.c_int, [C.c_void_p, C.POINTER(DwDesc), C.c_void_p]),
     "yv6_se_fwd": (C.c_int, [C.c_void_p, C.POINTER(SeDesc), C.c_void_p]),
+    "yv6_qa_fwd": (C.c_int, [C.c_void_p, C.POINTER(QaDesc), C.c_void_p]),
+    "yv6_qa_bwd": (C.c_int, [C.c_void_p, C.POINTER(QaDesc), C.c_void_p]),
     "yv6_channel_shuffle": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_int32,
                                       C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_void_p]),
     "yv6_upsample2x": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,

@@ -11,7 +11,7 @@ activation buffers, emitted once per (config, num_classes):
     (reppan.py:228,232, common.py:650,718 -> `dst=T(buf, c_off, c)`);
   * the engine (engine.py) walks the list and issues one kernel per op through the C ABI.
 
-Op kinds: stem | conv (rep / cba / cm / plain / dp parameter layouts) | convT | pool, and for the YOLOv6Lite networks
+Op kinds: stem | conv (rep / qa / cba / cm / plain / dp parameter layouts) | convT | pool, and for the YOLOv6Lite networks
 (build_lite_graph) dw (depthwise conv) | se (squeeze-excite, in place) | shuffle (channel_shuffle of two slices) | up (nearest
 2x upsample).
 """
@@ -39,7 +39,7 @@ class Buf:
 class Op:
     kind: str                 # 'stem' | 'conv' | 'convT' | 'pool' | 'pred' | 'dw' | 'se' | 'shuffle' | 'up'
     name: str                 # reference parameter prefix
-    layout: str = ""          # 'rep' | 'cba' | 'cm' (bare ConvModule) | 'plain' | 'convT' | 'dp' (a DPBlock conv: bias, bn_1 / bn_2)
+    layout: str = ""          # 'rep' | 'qa' (QARepVGGBlock[V2]) | 'cba' | 'cm' (bare ConvModule) | 'plain' | 'convT' | 'dp' (a DPBlock conv: bias, bn_1 / bn_2)
     src: Optional[T] = None
     dst: Optional[T] = None
     cin: int = 0
@@ -55,6 +55,12 @@ class Op:
     w_row0: int = 0
     w_rows: int = 0
     src2: Optional[T] = None  # shuffle: the second source (y[2j] = src[j], y[2j+1] = src2[j])
+    avg: bool = False         # 'qa': the block has QARepVGGBlockV2's 3x3 average-pool branch (common.py:406-425)
+
+    @property
+    def identity(self):
+        """A RepVGG-style block ('rep' / 'qa') with an identity branch: Cin == Cout at stride 1, not the stem."""
+        return self.layout in ("rep", "qa") and self.kind != "stem" and self.cin == self.cout and self.s == 1
 
     @property
     def param_rows(self):
@@ -98,7 +104,12 @@ class Graph:
         return dst
 
     def block(self, name, src, cout, s=1, dst=None, res=None, alpha=None):
-        """get_block(training_mode) of common.py:721-737: RepVGGBlock (relu) or ConvBNSiLU / ConvBNReLU."""
+        """get_block(training_mode) of common.py:721-737: RepVGGBlock (relu), QARepVGGBlock[V2] (relu) or ConvBNSiLU /
+        ConvBNReLU."""
+        if self.mode in QA_MODES:
+            dst = self.conv(name, "qa", src, cout, 3, s, "relu", dst, res, alpha)
+            self.ops[-1].avg = self.mode == "qarepvggv2" and src.c == cout and s == 1
+            return dst
         if self.mode == "repvgg":
             return self.conv(name, "rep", src, cout, 3, s, "relu", dst, res, alpha)
         return self.conv(name, "cba", src, cout, 3, s, "silu" if self.mode == "conv_silu" else "relu", dst, res, alpha)
@@ -108,6 +119,10 @@ class Graph:
         return "silu" if self.mode == "conv_silu" else "relu"
 
 
+QA_MODES = ("qarepvgg", "qarepvggv2")
+# get_block's modes (common.py:721-737) that build a network here; 'hyper_search' (LinearAddBlock) and 'repopt' (RealVGGBlock)
+# are not among them
+TRAINING_MODES = ("repvgg", "conv_relu", "conv_silu") + QA_MODES
 DETECT_DEFAULT_REG_MAX = 16  # effidehead.py:16
 AB_ANCHORS = 3                # build_network passes num_anchors = 3 to the fuse_ab head (yolo.py:125)
 
@@ -249,6 +264,8 @@ def build_graph(cfg, num_classes=80, name="yolov6", fuse_ab=False, distill_ns=Fa
         if fuse_ab or distill_ns:
             raise ValueError("YOLOv6Lite has no fuse_ab or distill_ns head (yolo_lite.py builds only the Lite Detect)")
         return build_lite_graph(cfg, num_classes, name)
+    if cfg["training_mode"] not in TRAINING_MODES:
+        raise ValueError(f"training_mode {cfg['training_mode']!r} is not one of {TRAINING_MODES} (get_block, common.py:721-737)")
     depth, width = cfg["depth_multiple"], cfg["width_multiple"]
     bb, nk, hd = cfg["backbone"], cfg["neck"], cfg["head"]
     reps = [(max(round(i * depth), 1) if i > 1 else i) for i in bb["num_repeats"] + nk["num_repeats"]]   # yolo.py:66
@@ -271,9 +288,9 @@ def build_graph(cfg, num_classes=80, name="yolov6", fuse_ab=False, distill_ns=Fa
         raise ValueError(f"stage_block_type {stage_kind!r} is not one of {STAGE_BLOCKS} (efficientrep.py:271-276)")
 
     # ---- backbone (efficientrep.py:7-118, 250-374, 377-516) ----
-    layout = "rep" if g.mode == "repvgg" else "cba"
+    layout = "rep" if g.mode == "repvgg" else "qa" if g.mode in QA_MODES else "cba"
     stem = T(g.buf(1, ch[0], "stem"), 0, ch[0])
-    g.ops.append(Op("stem", "backbone.stem", layout, None, stem, 3, ch[0], 3, 2, "relu" if g.mode == "repvgg" else g.act))
+    g.ops.append(Op("stem", "backbone.stem", layout, None, stem, 3, ch[0], 3, 2, "relu" if layout != "cba" else g.act))
     x = stem
     outs = []
     for s in range(2, nstage + 1):
@@ -533,6 +550,11 @@ def param_specs(g):
             bn(n + ".rbr_dense.bn", op.cout)
             specs.append((n + ".rbr_1x1.conv.weight", (op.cout, op.cin, 1, 1), "conv"))
             bn(n + ".rbr_1x1.bn", op.cout)
+        elif op.layout == "qa":     # QARepVGGBlock[V2]: identity / avg have no parameters, rbr_1x1 is a bare Conv2d
+            specs.append((n + ".rbr_dense.conv.weight", (op.cout, op.cin, 3, 3), "conv"))
+            bn(n + ".rbr_dense.bn", op.cout)
+            specs.append((n + ".rbr_1x1.weight", (op.cout, op.cin, 1, 1), "conv"))
+            bn(n + ".bn", op.cout)
         elif op.layout == "cba":
             specs.append((n + ".block.conv.weight", (op.cout, 1 if op.kind == "dw" else op.cin, op.k, op.k), "conv"))
             bn(n + ".block.bn", op.cout)

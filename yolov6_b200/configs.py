@@ -1,6 +1,7 @@
 """Built-in model configurations (the `model` dict and `training_mode` of reference configs/yolov6{n,s,m,l,n6,s6,m6,l6}.py and
 configs/mbla/yolov6{s,m,l,x}_mbla.py, and the YOLOv6Lite models of configs/yolov6_lite/yolov6_lite_{s,m,l}.py under their release
-names yolov6lite_{s,m,l}; `training_mode` defaults to "repvgg" as tools/train.py:99-100 does) so that
+names yolov6lite_{s,m,l}, and the quantization-aware RepVGG networks of configs/qarepvgg/yolov6{n,s,m}_qa.py; `training_mode`
+defaults to "repvgg" as tools/train.py:99-100 does) so that
 tests, smoke() and bench.py run where /root/reference is not mounted, plus a normaliser that accepts
 the reference's own mmcv-style Config object (yolov6/utils/config.py) for drop-in use."""
 import copy
@@ -93,6 +94,9 @@ def _lite(kind, width):
 
 
 CONFIGS.update({"yolov6lite_s": _lite("s", 0.7), "yolov6lite_m": _lite("m", 1.1), "yolov6lite_l": _lite("l", 1.5)})
+
+# configs/qarepvgg/yolov6{n,s,m}_qa.py: the N / S / M networks built from QARepVGGBlockV2 (common.py:396-477)
+CONFIGS.update({f"{n}_qa": dict(copy.deepcopy(CONFIGS[n]), training_mode="qarepvggv2") for n in ("yolov6n", "yolov6s", "yolov6m")})
 
 
 def get_config(name):

@@ -1,7 +1,7 @@
 """Weight preparation for the deploy-form kernels: BatchNorm folding and RepVGG re-parameterisation.
 
 Reference: fuse_conv_and_bn / fuse_model (yolov6/utils/torch_utils.py:50-94) and
-RepVGGBlock.get_equivalent_kernel_bias / switch_to_deploy (yolov6/layers/common.py:257-319).  The
+RepVGGBlock / QARepVGGBlock[V2].get_equivalent_kernel_bias / switch_to_deploy (yolov6/layers/common.py:257-477).  The
 reference does this by mutating modules in fp32; here it is a pure function from the train-form
 state_dict to per-op (weight KRSC, bias) pairs, computed in fp64 so the only rounding left is the
 final cast (the reference's own fold drifts its outputs by ~1e-4, SURVEY.md A.2).
@@ -46,6 +46,19 @@ def fold_op(sd, op):
             k[idx, idx, 1, 1] += scale
             b = b + shift
         return k.permute(0, 2, 3, 1).contiguous(), b
+    if op.layout == "qa":
+        # QARepVGGBlock[V2].get_equivalent_kernel_bias (common.py:348-360, 427-442): K = fold(W3, BN_d) + pad(W1) + I (+ 1/9 on
+        # every tap of the diagonal: AvgPool2d(3, 1, 1) counts the zero padding), bias b_d; then the post-sum bn in eval mode
+        k, b = fold_conv_bn(sd, n + ".rbr_dense")
+        k = k + torch.nn.functional.pad(sd[n + ".rbr_1x1.weight"].double(), [1, 1, 1, 1])
+        if op.identity:
+            idx = torch.arange(op.cin)
+            k[idx, idx, 1, 1] += 1.0
+            if op.avg:
+                k[idx, idx] += 1.0 / 9.0
+        scale, shift = _bn_affine(sd, n + ".bn")
+        k = k * scale.view(-1, 1, 1, 1)
+        return k.permute(0, 2, 3, 1).contiguous(), b * scale + shift
     if op.layout == "cba":
         k, b = fold_conv_bn(sd, n + ".block")
         return k.permute(0, 2, 3, 1).contiguous(), b

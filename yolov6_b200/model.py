@@ -188,6 +188,13 @@ class Model(nn.Module):
                     b = _ensure(node, [br])
                     b.add_module("conv", nn.Conv2d(op.cin, op.cout, k, op.s, k // 2, bias=False))
                     b.add_module("bn", nn.BatchNorm2d(op.cout))
+            elif op.layout == "qa":     # QARepVGGBlock[V2] (common.py:322-477): rbr_dense ConvModule, bare rbr_1x1, post-sum bn
+                node = _ensure(root, path[1:])
+                b = _ensure(node, ["rbr_dense"])
+                b.add_module("conv", nn.Conv2d(op.cin, op.cout, 3, op.s, 1, bias=False))
+                b.add_module("bn", nn.BatchNorm2d(op.cout))
+                node.add_module("rbr_1x1", nn.Conv2d(op.cin, op.cout, 1, op.s, 0, bias=False))
+                node.add_module("bn", nn.BatchNorm2d(op.cout))
             elif op.kind == "se":
                 node = _ensure(root, path[1:])
                 node.add_module("conv1", nn.Conv2d(op.cin, op.cin // 4, 1))

@@ -34,7 +34,7 @@ import numpy as np
 import torch
 
 from . import _lib, ops
-from ._lib import ACT_CODES, DT_F32, DT_U8, XF_BF16, XF_F32, XF_F64, XFORM_CHUNK, BnDesc, BnStatsDesc, WgradDesc, XformSeg
+from ._lib import ACT_CODES, DT_F32, DT_U8, XF_BF16, XF_F32, XF_F64, XFORM_CHUNK, BnDesc, BnStatsDesc, QaDesc, WgradDesc, XformSeg
 from .flat import FlatState
 
 BN_EPS, BN_MOMENTUM = 1e-3, 0.03
@@ -45,7 +45,10 @@ def _p(t):
 
 
 def op_branches(op):
-    """(prefix, kernel size) of the conv branches of a BN-ed block; k = 0 marks RepVGG's identity BatchNorm."""
+    """(prefix, kernel size) of the conv branches of a BN-ed block; k = 0 marks RepVGG's identity BatchNorm.  A QA block
+    ('qa') has the two conv branches only: its identity / average-pool branches have no parameters (yv6_qa_fwd / _bwd)."""
+    if op.layout == "qa":
+        return [(op.name + ".rbr_dense", 3), (op.name + ".rbr_1x1", 1)]
     if op.layout == "rep":
         br = [(op.name + ".rbr_dense", 3), (op.name + ".rbr_1x1", 1)]
         if op.kind != "stem" and op.cin == op.cout and op.s == 1:
@@ -54,6 +57,18 @@ def op_branches(op):
     if op.layout == "cm":        # bare ConvModule (MBLABlock.cv1 / cv2, common.py:671-677)
         return [(op.name, op.k)]
     return [(op.name + ".block", op.k)]
+
+
+def conv_weight_name(op, prefix):
+    """The weight of a conv branch: a ConvModule's `.conv.weight`, or the bare Conv2d `rbr_1x1.weight` of a QA block."""
+    return prefix + (".weight" if op.layout == "qa" and prefix.endswith(".rbr_1x1") else ".conv.weight")
+
+
+def branch_bn_names(op):
+    """The BatchNorm of each conv branch of op_branches (None: none of its own) and, for a QA block, the post-sum BatchNorm."""
+    if op.layout == "qa":
+        return [op.name + ".rbr_dense.bn", None], op.name + ".bn"
+    return [prefix + (".bn" if k else "") for prefix, k in op_branches(op)], None
 
 
 def op_param_names(op):
@@ -67,11 +82,14 @@ def op_param_names(op):
     if op.kind == "convT":
         return [op.name + ".upsample_transpose.weight", op.name + ".upsample_transpose.bias"]
     names = []
-    for prefix, k in op_branches(op):
-        bn = prefix + (".bn" if k else "")
+    bns, post = branch_bn_names(op)
+    for (prefix, k), bn in zip(op_branches(op), bns):
         if k:
-            names.append(prefix + ".conv.weight")
-        names += [bn + ".weight", bn + ".bias"]
+            names.append(conv_weight_name(op, prefix))
+        if bn is not None:
+            names += [bn + ".weight", bn + ".bias"]
+    if post is not None:
+        names += [post + ".weight", post + ".bias"]
     if op.alpha:
         names.append(op.alpha)
     return names
@@ -174,6 +192,11 @@ class TrainEngine:
                 ztake((i, "s2"), 8 * nb * c)
                 ztake((i, "dalpha"), 16)
                 ztake((i, "bcnt"), 16)
+                if op.layout == "qa":     # the post-sum BN's forward sums, and the backward of BN_d (rbr_dense.bn) on its own
+                    ztake((i, "qsum"), 16 * c)
+                    ztake((i, "qcnt"), 16)
+                    for key, nbytes in (("s1d", 8 * c), ("s2d", 8 * c), ("workd", 8 * c), ("bcntd", 16)):
+                        ztake((i, key), nbytes)
                 for b, (prefix, k) in enumerate(br):
                     if k == 0:
                         continue
@@ -223,6 +246,7 @@ class TrainEngine:
             # ---- BN-ed blocks
             br = op_branches(op)
             nb, co, ci = len(br), op.cout, op.cin
+            # QA blocks: stats [0] = BN_d (rbr_dense.bn), [1] = the post-sum bn; coef [0] / [1] = their backward coefficients
             self.stat_out[i] = torch.zeros(nb, 4, co, dtype=torch.float32, device=dev)
             self.coef_out[i] = torch.zeros(nb, 2, co, dtype=torch.float32, device=dev)
             W["br"] = []
@@ -231,7 +255,7 @@ class TrainEngine:
                 if k == 0:
                     W["br"].append(ent)
                     continue
-                wsrc = fl.ptr(prefix + ".conv.weight") + 4 * op.w_row0 * ci * k * k   # [Cout][Cin][k][k]
+                wsrc = fl.ptr(conv_weight_name(op, prefix)) + 4 * op.w_row0 * ci * k * k   # [Cout][Cin][k][k]
                 if op.kind == "stem":
                     ent["w"] = torch.zeros(3, 3, 3, co, dtype=torch.float32, device=dev)   # [r][s][c][Cout], fp32 math
                     if k == 3:
@@ -310,21 +334,31 @@ class TrainEngine:
         br = op_branches(op)
         co, ci = op.cout, op.cin
         r0 = 4 * op.w_row0          # byte offset of the op's first row in per-channel vectors
+        bns, post = branch_bn_names(op)
         for b, (prefix, k) in enumerate(br):
-            bn = prefix + (".bn" if k else "")
+            wname = conv_weight_name(op, prefix)
             if k:
                 if op.kind == "stem":
                     if k == 3:      # dw [Cout][32]: column (r*3+s)*3 + c -> [Cout][c][r][s]
-                        segs.append(_seg(fl.grad_ptr(prefix + ".conv.weight"), z(i, "dw", b), [co, 3, 9], [27, 9, 1], [32, 1, 3],
+                        segs.append(_seg(fl.grad_ptr(wname), z(i, "dw", b), [co, 3, 9], [27, 9, 1], [32, 1, 3],
                                          XF_F32, XF_F32))
                     else:           # the 1x1 stride-2 branch sees the centre tap (r = s = 1): columns 12..14
-                        segs.append(_seg(fl.grad_ptr(prefix + ".conv.weight"), z(i, "dw", b) + 4 * 12, [co, 3], [3, 1], [32, 1], XF_F32, XF_F32))
+                        segs.append(_seg(fl.grad_ptr(wname), z(i, "dw", b) + 4 * 12, [co, 3], [3, 1], [32, 1], XF_F32, XF_F32))
                 else:
                     kk = k * k      # dw [Cout][kk][Cin] -> [Cout][Cin][kk]
-                    segs.append(_seg(fl.grad_ptr(prefix + ".conv.weight") + r0 * ci * kk, z(i, "dw", b), [co, ci, kk], [ci * kk, kk, 1],
+                    segs.append(_seg(fl.grad_ptr(wname) + r0 * ci * kk, z(i, "dw", b), [co, ci, kk], [ci * kk, kk, 1],
                                      [kk * ci, 1, ci], XF_F32, XF_F32))
+            if post is not None:    # QA block: BN_d's sums come from its own backward launch
+                if bns[b] is not None:
+                    segs.append(_seg(fl.grad_ptr(bns[b] + ".weight"), z(i, "s2d"), [co], [1], [1], XF_F32, XF_F64))
+                    segs.append(_seg(fl.grad_ptr(bns[b] + ".bias"), z(i, "s1d"), [co], [1], [1], XF_F32, XF_F64))
+                continue
+            bn = bns[b]
             segs.append(_seg(fl.grad_ptr(bn + ".weight") + r0, z(i, "s2") + 8 * b * co, [co], [1], [1], XF_F32, XF_F64))   # dgamma = sum dz * xhat
             segs.append(_seg(fl.grad_ptr(bn + ".bias") + r0, z(i, "s1"), [co], [1], [1], XF_F32, XF_F64))                 # dbeta = sum dz
+        if post is not None:
+            segs.append(_seg(fl.grad_ptr(post + ".weight"), z(i, "s2"), [co], [1], [1], XF_F32, XF_F64))
+            segs.append(_seg(fl.grad_ptr(post + ".bias"), z(i, "s1"), [co], [1], [1], XF_F32, XF_F64))
         if op.alpha:
             segs.append(_seg(fl.grad_ptr(op.alpha), z(i, "dalpha"), [1], [1], [1], XF_F32, XF_F64))
         return segs
@@ -366,6 +400,20 @@ class TrainEngine:
                 d.running_var[b] = fl.ptr(prefix + ".running_var") + 4 * row0
                 d.stats[b] = st.data_ptr()
         return d
+
+    def _qa_desc(self, op, u, v, st, t, sums_ptr, cnt_ptr):
+        """yv6_qa_fwd of a QA block: t = BN_d(u) + v (x / avg set by the caller), the post-sum bn finalised into st[1]."""
+        fl, bn = self.flat, op.name + ".bn"
+        q = QaDesc()
+        q.N, q.H, q.W, q.C = t.shape
+        q.u, q.u_pitch, q.v, q.v_pitch = u.data_ptr(), u.shape[3], v.data_ptr(), v.shape[3]
+        q.scale_d, q.shift_d = st[0, 2].data_ptr(), st[0, 3].data_ptr()
+        q.avg = int(op.avg)
+        q.t, q.t_pitch = t.data_ptr(), t.shape[3]
+        q.sums, q.counter, q.zeroed, q.eps, q.momentum = sums_ptr, cnt_ptr, 1, BN_EPS, BN_MOMENTUM
+        q.gamma, q.beta = fl.ptr(bn + ".weight"), fl.ptr(bn + ".bias")
+        q.running_mean, q.running_var, q.stats = fl.ptr(bn + ".running_mean"), fl.ptr(bn + ".running_var"), st[1].data_ptr()
+        return q
 
     def _dgrad_descs(self, dc, ent, k, stride, gsrc, g_off):
         """g(src)[..., g_off:+Cin] += conv_transpose(dc, w) as one (stride 1) or up to four (stride 2) accumulating convs."""
@@ -537,10 +585,25 @@ class TrainEngine:
                     src, _ = view(op.src)
                     fwd.append(("conv", self._conv_desc(src, op.src.c_off, ent["w"], raw, stride=op.s)))
                 xs.append((raw, 0))
-            fin = [(ent["prefix"] + (".bn" if ent["k"] else ""), st[b]) for b, ent in enumerate(br)]
-            fwd.append(("stats", self._stats_desc(xs, op.cout, count, z(i, "fsum"), z(i, "fcnt"), fin, op.w_row0)))
+            qa = op.layout == "qa"
+            if qa:
+                # BN_d statistics of u, then t = BN_d(u) + v [+ x [+ avg3x3 x]] with the post-sum bn's statistics in one launch;
+                # from here on the block is a one-branch BatchNorm over t
+                u, v = xs[0][0], xs[1][0]
+                fwd.append(("stats", self._stats_desc([xs[0]], op.cout, count, z(i, "fsum"), z(i, "fcnt"), [(op.name + ".rbr_dense.bn", st[0])])))
+                tq = bf(n, ho, wo, op.cout)
+                q = self._qa_desc(op, u, v, st, tq, z(i, "qsum"), z(i, "qcnt"))
+                if op.identity:
+                    src, _ = view(op.src)
+                    q.x, q.x_pitch = src.data_ptr() + op.src.c_off * 2, src.shape[3]
+                fwd.append(("qa", q))
+                self.ctx[i].update(u=u, v=v, t=tq, stats_d=st[0], stats_p=st[1])
+                xs, st = [(tq, 0)], st[1:]
+            else:
+                fin = [(ent["prefix"] + (".bn" if ent["k"] else ""), st[b]) for b, ent in enumerate(br)]
+                fwd.append(("stats", self._stats_desc(xs, op.cout, count, z(i, "fsum"), z(i, "fcnt"), fin, op.w_row0)))
             d = BnDesc()
-            d.nb, d.act, d.C, d.pixels = nb, ACT_CODES[op.act], op.cout, count
+            d.nb, d.act, d.C, d.pixels = len(xs), ACT_CODES[op.act], op.cout, count
             dcs = []
             for b, (t, off) in enumerate(xs):
                 d.x[b], d.x_pitch[b] = t.data_ptr() + off * 2, t.shape[3]
@@ -576,6 +639,28 @@ class TrainEngine:
             par = bn_ops & 1
             bn_ops += 1
             calls.append(("bn_bwd", d, wr, par))
+            if qa:
+                # dt (d.dx[0]) -> BN_d backward (no activation) -> du; dt also feeds the 1x1 branch and the parameter-free identity /
+                # average-pool branches (yv6_qa_bwd into g(x)); the conv branches below then read dcs = [du, dt]
+                dt = dcs[0]
+                du = dc_pool[2 * par + 1][:count * op.cout].view(n, ho, wo, op.cout)
+                sd_ = self.stat_out[i][0]
+                d2 = BnDesc()
+                d2.nb, d2.act, d2.C, d2.pixels = 1, ACT_CODES[None], op.cout, count
+                d2.x[0], d2.x_pitch[0] = u.data_ptr(), op.cout
+                d2.mean[0], d2.invstd[0], d2.scale[0], d2.shift[0] = (sd_[r].data_ptr() for r in range(4))
+                d2.s2[0], d2.s1 = z(i, "s2d"), z(i, "s1d")
+                d2.dx[0], d2.dx_pitch[0], d2.accumulate[0] = du.data_ptr(), op.cout, 0
+                d2.dy, d2.dy_pitch = dt.data_ptr(), op.cout
+                d2.work, d2.counter, d2.coef, d2.zeroed = z(i, "workd"), z(i, "bcntd"), self.coef_out[i][1].data_ptr(), 1
+                calls.append(("bn_bwd", d2, [], par))
+                if op.identity:
+                    _, gsrc = view(op.src)
+                    qb = self._qa_desc(op, u, v, self.stat_out[i], tq, 0, 0)
+                    qb.dt, qb.dt_pitch = dt.data_ptr(), op.cout
+                    qb.dx, qb.dx_pitch = gsrc.data_ptr() + op.src.c_off * 2, gsrc.shape[3]
+                    calls.append(("qa_bwd", qb, dict(buf=op.src.buf, off=op.src.c_off, n=op.cin, full=True)))
+                dcs = [du, dt]
             if op.kind == "stem":       # im2col once, then one tensor-core wgrad GEMM per branch
                 patches, patches_lo = bf(n, ho, wo, 32), bf(n, ho, wo, 32)     # image = hi + lo (bf16 planes)
                 self._stem_patches = (patches, patches_lo)
@@ -651,6 +736,8 @@ class TrainEngine:
                         d.dres_assign = 1 if assign else 0
             elif kind == "pool_bwd":
                 c[1][11] = 0 if decide(c[2]) else 1
+            elif kind == "qa_bwd":
+                c[1].accumulate = 0 if decide(c[2]) else 1
         for i, cv in enumerate(cov):        # slices nobody writes are read as zero gradients
             if not cv.all():
                 need_zero.add(i)
@@ -705,6 +792,8 @@ class TrainEngine:
                 chk(lib.yv6_bn_apply_fwd(h, C.byref(d), sp))
             elif kind == "stem":
                 chk(lib.yv6_stem_fwd(h, C.byref(d), sp))
+            elif kind == "qa":
+                chk(lib.yv6_qa_fwd(h, C.byref(d), sp))
             elif kind == "abp":
                 self._ab_call(d, False, sp)
             else:
@@ -797,6 +886,8 @@ class TrainEngine:
                 chk(lib.yv6_bn_bwd(h, C.byref(d), sp))
             elif kind == "stats":
                 chk(lib.yv6_bn_stats_finalize(h, C.byref(d), sp))
+            elif kind == "qa_bwd":
+                chk(lib.yv6_qa_bwd(h, C.byref(d), sp))
             elif kind == "copy":
                 if overlap:
                     wait_pending()
