@@ -356,9 +356,8 @@ def check_hgp(lib, h, sp, mem, args, gen):
 def check_pool_chain(lib, h, sp, eng, calls, gen):
     """The three chained MaxPool2d(5, 1, 2) backward launches of one SPPF against torch's max-pool backward in float64 (scatter to
     the first maximum in row-major window order), on operands quantised to a few levels so that ties are everywhere."""
-    a = calls[0][1]
-    n, hh, ww, c = a[4], a[5], a[6], a[7]
-    bi = calls[0][2]["buf"]
+    n, hh, ww, c = calls[0].args[4:8]
+    bi = calls[0].writes[0].buf
     buf, gbuf = eng.bufs[bi], eng.gbufs[bi]
     ys = [torch.randint(0, 4, (n, c, hh, ww), generator=gen).double()]
     for _ in range(3):
@@ -369,10 +368,10 @@ def check_pool_chain(lib, h, sp, eng, calls, gen):
     gbuf.copy_(prior)
     G = [nchw(prior[..., j * c:(j + 1) * c]) for j in range(4)]
     for call in calls:
-        d = call[1]
-        j = call[2]["off"] // c + 1
+        d = call.args
+        j = call.writes[0].off // c + 1
         assert d[0] == buf.data_ptr() + (j - 1) * c * 2 and d[2] == gbuf.data_ptr() + j * c * 2
-        check(lib.yv6_maxpool5_bwd(h, d[0], d[1], d[2], d[3], d[4], d[5], d[6], d[7], d[8].data_ptr(), d[9], d[10], d[11], sp), lib)
+        check(lib.yv6_maxpool5_bwd(h, *d, sp), lib)
         y = ys[j - 1].clone().requires_grad_(True)
         F.max_pool2d(y, 5, 1, 2).backward(G[j])
         G[j - 1] = (G[j - 1] * d[11] + y.grad).to(BF16).double()
@@ -427,13 +426,12 @@ def _engine(name):
 
 
 def engine_mem(eng):
-    dc_pool, pool_scr, dq_pool = eng._keep
+    sc = eng.scratch
     named = [("buf", t) for t in eng.bufs] + [("gbuf", t) for t in eng.gbufs] + [("arena", eng.zero_arena)]
-    named += [("dc", t) for t in dc_pool] + [("dq", t) for t in (dq_pool or [])] + [("poolscr", pool_scr)]
+    named += [("dc", t) for t in sc.dc] + [("dq", t) for q in sc.quad for t in q] + [("poolscr", t) for p in sc.pool for t in p]
     named += [("stat", t) for t in eng.stat_out.values()] + [("coef", t) for t in eng.coef_out.values()]
     named += [("head", t) for t in (eng.cls, eng.reg, eng.grad_cls, eng.grad_reg)] + [("img", eng.x_static)]
-    named += [("dl", c[2]) for c in eng.bwd_calls if c[0] == "hgp"]
-    named += [("dq", c[1][0]) for c in eng.bwd_calls if c[0] == "copy"]       # ConvTranspose quadrants (earlier, smaller pools)
+    named += [("dl", t) for t in sc.dl]
     named += [("patch", t) for t in getattr(eng, "_stem_patches", ())]
     named += [("raw", br["x"]) for ctx in eng.ctx if ctx and "branches" in ctx for br in ctx["branches"] if br["k"]]
     named += [("param", eng.flat.pflat)]
@@ -461,7 +459,7 @@ KINDS = ("conv", "wgrad", "bn_bwd", "stats", "hgp", "pool_bwd", "im2col")
 
 
 @pytest.mark.parametrize("name", list(MODELS))
-def test_every_backward_launch_matches_float64_autograd(name):
+def test_every_backward_launch_record_matches_float64_autograd(name):
     from yolov6_b200 import _lib
     from yolov6_b200._lib import DT_F32, DT_U8
     eng = _engine(name)
@@ -485,55 +483,52 @@ def test_every_backward_launch_matches_float64_autograd(name):
     wmap = dgrad_weights(eng)
     groups, pools = {}, {}
     for c in eng.bwd_calls:
-        if c[0] == "conv":
-            d, meta = c[1], c[2]
-            key = meta.get("group", ("w", d.w))
-            groups.setdefault(key, (meta, []))[1].append(d)
-        elif c[0] == "pool_bwd":
-            pools.setdefault(c[2]["buf"], []).append(c)
+        if c.kind == "conv":
+            d, wr = c.desc, c.writes[0]
+            key = wr.group or ("w", d.w)
+            groups.setdefault(key, (wr, []))[1].append(d)
+        elif c.kind == "pool_bwd":
+            pools.setdefault(c.writes[0].buf, []).append(c)
     for key, (meta, descs) in groups.items():
         i, wf, stride = wmap[descs[0].w]
         assert all(wmap[d.w][0] == i for d in descs)
-        gbuf = eng.gbufs[meta["buf"]]
+        gbuf = eng.gbufs[meta.buf]
         if not first_time("conv", tuple(signature(d, mem) for d in descs) + (tuple(gbuf.shape),)):
             continue
-        r = check_dgrad(lib, h, sp, mem, descs, wf, stride, gbuf, meta["off"], meta["n"], gen)
+        r = check_dgrad(lib, h, sp, mem, descs, wf, stride, gbuf, meta.off, meta.n, gen)
         assert r <= 1.0, f"{ops[i].name}: dgrad error {r:.2f} x the bar ({len(descs)} launches)"
         worst["conv"] = max(worst["conv"], r)
     for bi, calls in pools.items():
         assert len(calls) == 3
-        if not first_time("pool_bwd", tuple(tuple(x if not torch.is_tensor(x) else None for x in c[1]) for c in calls)):
+        if not first_time("pool_bwd", tuple(tuple(c.args) for c in calls)):
             continue
         r = check_pool_chain(lib, h, sp, eng, calls, gen)
         assert r <= 1.0, f"pool backward of buffer {bi}: error {r:.2f} x the bar"
         worst["pool_bwd"] = max(worst["pool_bwd"], r)
     for c in eng.bwd_calls:
-        kind = c[0]
+        kind, d = c.kind, c.desc
         if kind == "wgrad":
-            d = c[1]
             if first_time(kind, signature(d, mem)):
                 r = check_wgrad(lib, h, sp, mem, d, gen)
                 assert r <= 1.0, f"wgrad {(d.N, d.H, d.W, d.Cin, d.Cout, d.kh, d.stride)}: error {r:.2f} x the bar"
                 worst[kind] = max(worst[kind], r)
         elif kind == "bn_bwd":
-            d = c[1]
             if first_time(kind, signature(d, mem)):
                 out = check_bn_bwd(lib, h, sp, mem, d, gen)
                 for k, r in out.items():
                     bn_worst[k] = max(bn_worst.get(k, 0.0), r)
                     assert r <= 1.0, f"bn_bwd C={d.C} nb={d.nb} act={d.act} res={bool(d.res)}: {k} error {r:.2f} x the bar"
         elif kind == "stats":
-            d = c[1]
             if first_time(kind, signature(d, mem)):
                 r = check_stats_sums(lib, h, sp, mem, d, gen)
                 assert r <= 1.0, f"stats C={d.C} pixels={d.pixels}: error {r:.2f} x the bar"
                 worst[kind] = max(worst[kind], r)
         elif kind == "hgp":
-            if first_time(kind, (bool(c[1][1]),) + tuple(c[1][2:8])):
-                check_hgp(lib, h, sp, mem, c[1], gen)
+            if first_time(kind, (bool(c.args[1]),) + tuple(c.args[2:8])):
+                check_hgp(lib, h, sp, mem, c.args, gen)
         elif kind == "im2col":
-            if first_time(kind, tuple(c[1][1:6])):
-                x_ptr, x_dt, scale, N, H, W, pp, plo = c[1]
+            if first_time(kind, tuple(c.args[1:6])):
+                x_ptr, x_dt, scale, N, H, W, pp, plo = c.args
                 assert x_dt == DT_F32 and x_ptr == eng.x_static.data_ptr()
                 patches, lo = eng._stem_patches
                 assert pp == patches.data_ptr() and plo == lo.data_ptr()
@@ -545,7 +540,7 @@ def test_every_backward_launch_matches_float64_autograd(name):
                 d8 = img8.cuda()
                 check_im2col(lib, h, sp, d8.data_ptr(), img8, DT_U8, scale, N, H, W, patches, lo, gen)
     worst["bn_bwd"] = max(bn_worst.values()) if bn_worst else 0.0
-    kinds_made = {c[0] for c in eng.bwd_calls}
+    kinds_made = {c.kind for c in eng.bwd_calls}
     for k in KINDS:
         if k in kinds_made:
             assert seen[k], f"no {k} launch checked"

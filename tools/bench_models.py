@@ -144,20 +144,20 @@ def train_split(name, size, batch, dev, reps=5):
         for c in calls:
             eng.fwd_calls = [c]
             ms = timed(lambda: eng.run_forward(sp))
-            fwd_ms[c[0]] = fwd_ms.get(c[0], 0.0) + ms
-            if c[0] == "qa":
-                d = c[1]
+            fwd_ms[c.kind] = fwd_ms.get(c.kind, 0.0) + ms
+            if c.kind == "qa":
+                d = c.desc
                 qa["qa_fwd"][0] += ms
                 qa["qa_fwd"][1] += 2 * d.N * d.H * d.W * d.C * (3 + (1 if d.x else 0))
     finally:
         eng.fwd_calls = calls
     for j, c in enumerate(eng.bwd_calls):
-        if c[0] in ("dbg", "bucket"):
+        if c.bucket is not None:
             continue
         ms = timed(lambda: eng.backward(None, None, first=j, last=j + 1))
-        bwd_ms[c[0]] = bwd_ms.get(c[0], 0.0) + ms
-        if c[0] == "qa_bwd":
-            d = c[1]
+        bwd_ms[c.kind] = bwd_ms.get(c.kind, 0.0) + ms
+        if c.kind == "qa_bwd":
+            d = c.desc
             qa["qa_bwd"][0] += ms
             qa["qa_bwd"][1] += 2 * d.N * d.H * d.W * d.C * (2 + d.accumulate)
     out = {"model": name, "mode": "train launch split", "size": size, "batch": batch,

@@ -29,6 +29,7 @@ the BN apply / backward kernels (y = act(z) + alpha * x, alpha read from device 
 """
 import ctypes as C
 import os
+from dataclasses import dataclass
 
 import numpy as np
 import torch
@@ -132,6 +133,72 @@ def _seg(dst, src, n, ds, ss, dst_dtype, src_dtype):
     return s
 
 
+ALL = -1    # Launch.parity of a main-stream launch that waits for every pending weight gradient
+
+
+@dataclass(eq=False)
+class Write:
+    """Channels [off, off + n) of gradient buffer `buf` written by a launch (at every pixel when `full`); `assign(True)` makes
+    the launch overwrite them, `assign(False)` add to them.  The launches of one `group` share one decision."""
+    buf: int
+    off: int
+    n: int
+    full: bool
+    assign: object
+    group: tuple = None
+
+
+@dataclass(eq=False)
+class Launch:
+    """One launch of the training step: library entry point `fn` (a name) called as fn(handle, *args, stream), or a callable
+    fn(stream).  Descriptor launches pass `desc` by reference.  `side`: a weight gradient, run on the side stream next to the
+    main stream; `parity`: the dc scratch pair it reads (side) or refills (main stream, ALL: everything the side stream may
+    read).  `snapshot` = (op index, incoming gradient slice) is copied into engine.dbg before the launch when engine.debug;
+    `bucket` = k marks the unpack of gradient bucket k."""
+    kind: str
+    fn: object
+    args: tuple = ()
+    desc: object = None
+    kernels: int = 1
+    side: bool = False
+    parity: int = None
+    writes: tuple = ()
+    snapshot: tuple = None
+    bucket: int = None
+
+    def run(self, lib, h, sp):
+        if isinstance(self.fn, str):
+            _lib.check(getattr(lib, self.fn)(h, *self.args, sp))
+        else:
+            self.fn(sp)
+
+
+def _desc_launch(kind, fn, d, **kw):
+    return Launch(kind, fn, (C.byref(d),), desc=d, **kw)
+
+
+class _Scratch:
+    """Scratch of one planned shape.  dc: the BN-backward outputs (gradients w.r.t. the raw conv outputs), which live only until
+    their dgrad / wgrad ran, two per op parity: the weight gradients of an op run on a side stream while the next op's BN
+    backward refills the other pair.  Also the max-pool backward scratch, the ConvTranspose quadrant gradients and the head
+    gradients dl; a buffer that grows keeps its smaller predecessors, which earlier launches still use."""
+
+    def __init__(self, dev, dc_elems):
+        self.dev = dev
+        self.dc = [torch.zeros(dc_elems, dtype=torch.bfloat16, device=dev) for _ in range(4)]
+        self.bn_ops = 0
+        self.pool, self.quad, self.dl = [], [], []
+
+    def dc_view(self, par, slot, shape):
+        return self.dc[2 * par + slot][:int(np.prod(shape))].view(shape)
+
+    def grown(self, pools, numel, count, dtype):
+        """The last set of `count` buffers in `pools`, after appending a new set when it holds fewer than numel elements."""
+        if not pools or pools[-1][0].numel() < numel:
+            pools.append([torch.zeros(numel, dtype=dtype, device=self.dev) for _ in range(count)])
+        return pools[-1]
+
+
 class TrainEngine:
     def __init__(self, model, n_buckets=1):
         self.model = model
@@ -214,9 +281,7 @@ class TrainEngine:
         grad_segs, self.bucket_of_op = [], {}
         P = self.params
 
-        def bf16(*shape):
-            return torch.zeros(*shape, dtype=torch.bfloat16, device=dev)
-
+        bf16 = self._bf
         for i, op in enumerate(g.ops):
             if op.kind == "pool":
                 continue
@@ -415,35 +480,36 @@ class TrainEngine:
         q.running_mean, q.running_var, q.stats = fl.ptr(bn + ".running_mean"), fl.ptr(bn + ".running_var"), st[1].data_ptr()
         return q
 
-    def _dgrad_descs(self, dc, ent, k, stride, gsrc, g_off):
-        """g(src)[..., g_off:+Cin] += conv_transpose(dc, w) as one (stride 1) or up to four (stride 2) accumulating convs."""
+    def _dgrad_descs(self, dc, ent, stride, gsrc, g_off):
+        """g(src)[..., g_off:+Cin] += conv_transpose(dc, w) as one (stride 1) or up to four (stride 2) accumulating convs: at
+        stride 2 one conv per input parity (ph, pw), a 1- or 2-tap stride-1 conv each; a 1x1 conv touches parity (0, 0) only."""
         if stride == 1:
             return [self._conv_desc(dc, 0, ent["wt"][0], gsrc, g_off, accumulate=True)]
         n, hs, ws, gct = gsrc.shape
-        ho, wo = dc.shape[1], dc.shape[2]
-        out = []
-        j = 0
-        for ph in range(2):
-            for pw in range(2):
-                if k == 1:
-                    if ph or pw:
-                        continue
-                    wt = ent["wt"][0]
-                else:
-                    wt = ent["wt"][j]
-                    j += 1
-                out.append(self._conv_desc(dc, 0, wt, gsrc, g_off, pad=(0, 0), out_hw=(ho, wo), accumulate=True,
-                                           y_strides=(hs * ws * gct, 2 * ws * gct, 2 * gct), y_elem_off=(ph * ws + pw) * gct))
-        return out
+        return [self._conv_desc(dc, 0, wt, gsrc, g_off, pad=(0, 0), out_hw=tuple(dc.shape[1:3]), accumulate=True,
+                                y_strides=(hs * ws * gct, 2 * ws * gct, 2 * gct), y_elem_off=(ph * ws + pw) * gct)
+                for (ph, pw), wt in zip([(0, 0), (0, 1), (1, 0), (1, 1)], ent["wt"])]
+
+    def _bf(self, *shape):
+        return torch.zeros(*shape, dtype=torch.bfloat16, device=self.dev)
+
+    def _view(self, t):
+        return self.bufs[t.buf], self.gbufs[t.buf]
+
+    def _dgrad_launch(self, d, op, full=True, group=None):
+        """A dgrad conv accumulating into op's input gradient slice g(src)[..., c_off:+cin] (or, as its first writer, assigning)."""
+        def assign(a):
+            if a:           # y = conv(...) instead of y += conv(...): no residual read
+                d.res, d.alpha = 0, 0.0
+        return _desc_launch("conv", "yv6_conv_fwd", d, writes=[Write(op.src.buf, op.src.c_off, op.cin, full, assign, group)])
 
     def _plan(self, N, H, W, in_dtype):
         key = (N, H, W, in_dtype)
         if self._shape == key:
             return
         self._shape = key
-        g, dev, fl, z = self.g, self.dev, self.flat, self._z
-        bf = lambda *s: torch.zeros(*s, dtype=torch.bfloat16, device=dev)   # noqa: E731
-        self.bufs = [bf(N, H >> b.level, W >> b.level, b.c_total) for b in g.bufs]
+        g, dev = self.g, self.dev
+        self.bufs = [self._bf(N, H >> b.level, W >> b.level, b.c_total) for b in g.bufs]
         self.gbufs = [torch.zeros_like(t) for t in self.bufs]
         self.sizes = [(H // s, W // s) for s in g.strides]
         self.offs = [0]
@@ -463,233 +529,248 @@ class TrainEngine:
             self.reg_ab = torch.empty(N, AB_ANCHORS * A, 4, dtype=torch.float32, device=dev)
             self.grad_cls_ab = torch.zeros_like(self.cls_ab)
             self.grad_reg_ab = torch.zeros_like(self.reg_ab)
-            self._ab = {}                     # level -> dict(raw_cls, raw_reg, dl_cls, dl_reg, anchors)
+            self._ab = {}                     # level -> {"cls_ab" / "reg_ab": (fp32 conv output, bf16 gradient)}
         self.x_static = torch.zeros(N, 3, H, W, dtype=in_dtype, device=dev)   # the stem reads this buffer (graph-stable address)
-        view = lambda t: (self.bufs[t.buf], self.gbufs[t.buf])   # noqa: E731
-        # shared scratch: BN-backward outputs (gradients w.r.t. the raw conv outputs) live only until their dgrad / wgrad ran
-        dc_elems = max([N * (H >> g.bufs[op.dst.buf].level) * (W >> g.bufs[op.dst.buf].level) * op.cout
-                        for op in g.ops if op.kind in ("conv", "stem")] + [1])
-        # (two per op parity: the weight gradients of an op run on a side stream while the next op's BN backward refills the other pair)
-        dc_pool = [torch.zeros(dc_elems, dtype=torch.bfloat16, device=dev) for _ in range(4)]
-        bn_ops = 0
-        pool_scr, dq_pool = None, None
-        fwd, bwd_rev = [], []        # bwd_rev[j] = list of calls of op j (assembled in reverse op order afterwards)
-        x_dt = DT_U8 if in_dtype == torch.uint8 else DT_F32
-        for i, op in enumerate(g.ops):
-            calls = []
-            if op.kind == "pool":
-                buf, gbuf = view(op.dst)
-                n, h, w, ct = buf.shape
-                c = op.cin
-                fwd.append(("pool", (buf.data_ptr(), n, h, w, c, ct, 1, 0)))
-                if pool_scr is None or pool_scr.numel() < n * h * w * c:
-                    pool_scr = torch.zeros(n * h * w * c, dtype=torch.float32, device=dev)
-                calls.append(("dbg", (i, gbuf[..., :4 * c])))
-                for j in (3, 2, 1):   # y_j = pool(y_{j-1}); slice j of the concat
-                    calls.append(("pool_bwd", [buf.data_ptr() + (j - 1) * c * 2, ct, gbuf.data_ptr() + j * c * 2, ct, n, h, w, c,
-                                               pool_scr, gbuf.data_ptr() + (j - 1) * c * 2, ct, 1],
-                                  dict(buf=op.dst.buf, off=(j - 1) * c, n=c, full=True)))
-                bwd_rev.append(calls)
-                continue
-            Wt = self.wts[i]
-            if op.kind == "pred" and op.head[0].endswith("_ab"):
-                # fuse_ab pred conv: natural NHWC output [N, hw, na * ch] (fp32, sigmoid fused on the class branch); the pack /
-                # grad kernels (csrc/yv6_fuseab.cu) move between it and the reference's (level, anchor, pixel) row order
-                from .arch import AB_ANCHORS
-                src, gsrc = view(op.src)
-                which, lvl = op.head
-                lh, lw = self.sizes[lvl]
-                ch, chp = op.cout, (op.cout + 15) // 16 * 16
-                st = self._ab.setdefault(lvl, {})
-                raw = torch.empty(N, lh * lw, ch, dtype=torch.float32, device=dev)
-                dl = bf(N, lh, lw, chp)
-                st["raw_" + which[:3]], st["dl_" + which[:3]] = raw, dl
-                fwd.append(("conv", self._conv_desc(src, op.src.c_off, Wt["w"], raw, bias=Wt["bias"], act=op.act,
-                                                    y_strides=(lh * lw * ch, lw * ch, ch))))
-                if which == "reg_ab":          # second of the level's pair in forward order, first in backward order
-                    anc = [v / float(g.strides[lvl]) for v in g.anchors_init[lvl]]          # effidehead_fuseab.py:35
-                    st["anchors"] = (C.c_float * 6)(*anc)
-                    fwd.append(("abp", lvl))
-                    calls.append(("abg", lvl))
-                calls.append(("wgrad", self._wgrad_desc(src, op.src.c_off, op.cin, dl, 0, ch, 1, 1, z(i, "dw"))))
-                calls.append(("stats", self._stats_desc([(dl, 0)], chp, N * lh * lw, z(i, "bsum"), z(i, "bcnt"))))
-                calls.append(("conv", self._conv_desc(dl, 0, Wt["wt"], gsrc, op.src.c_off, accumulate=True),
-                              dict(buf=op.src.buf, off=op.src.c_off, n=op.cin, full=True)))
-                bwd_rev.append(calls)
-                continue
-            if op.kind == "pred":
-                src, gsrc = view(op.src)
-                which, lvl = op.head
-                out, grad = {"cls": (self.cls, self.grad_cls), "reg": (self.reg, self.grad_reg),
-                             "reg_dist": (getattr(self, "reg_dist", None), getattr(self, "grad_reg_dist", None))}[which]
-                ch = out.shape[2]
-                chp = (ch + 15) // 16 * 16
-                lh, lw = self.sizes[lvl]
-                fwd.append(("conv", self._conv_desc(src, op.src.c_off, Wt["w"], out, bias=Wt["bias"], act=op.act,
-                                                    y_strides=(A * ch, lw * ch, ch), y_elem_off=self.offs[lvl] * ch)))
-                dl = bf(N, lh, lw, chp)
-                calls.append(("hgp", (grad.data_ptr(), self.cls.data_ptr() if which == "cls" else 0, N, A, ch, self.offs[lvl], lh * lw, chp,
-                                      dl.data_ptr()), dl))
-                calls.append(("wgrad", self._wgrad_desc(src, op.src.c_off, op.cin, dl, 0, ch, 1, 1, z(i, "dw"))))
-                calls.append(("stats", self._stats_desc([(dl, 0)], chp, N * lh * lw, z(i, "bsum"), z(i, "bcnt"))))
-                calls.append(("conv", self._conv_desc(dl, 0, Wt["wt"], gsrc, op.src.c_off, accumulate=True),
-                              dict(buf=op.src.buf, off=op.src.c_off, n=op.cin, full=True)))
-                bwd_rev.append(calls)
-                continue
-            if op.kind == "convT":
-                src, gsrc = view(op.src)
-                dst, gdst = view(op.dst)
-                _, dh, dw, dct = dst.shape
-                _, sh, sw, _ = src.shape
-                for q in range(4):
-                    dy, dx = q // 2, q % 2
-                    fwd.append(("conv", self._conv_desc(src, op.src.c_off, Wt["w"][q], dst, op.dst.c_off, bias=Wt["bias"],
-                                                        y_strides=(dh * dw * dct, 2 * dw * dct, 2 * dct), y_elem_off=(dy * dw + dx) * dct)))
-                gd = gdst[..., op.dst.c_off:op.dst.c_off + op.cout]
-                calls.append(("dbg", (i, gd)))
-                # bias gradient = column sums of the whole upsampled gradient slice
-                calls.append(("stats", self._stats_desc([(gdst, op.dst.c_off)], op.cout, N * dh * dw, z(i, "bsum"), z(i, "bcnt"))))
-                need = N * sh * sw * op.cout
-                if dq_pool is None or dq_pool[0].numel() < need:
-                    dq_pool = [torch.zeros(need, dtype=torch.bfloat16, device=dev) for _ in range(4)]
-                for q in range(4):
-                    dy, dx = q // 2, q % 2
-                    dq = dq_pool[q][:need].view(N, sh, sw, op.cout)
-                    calls.append(("copy", (dq, gd[:, dy::2, dx::2, :])))               # gradient of quadrant q, dense
-                    calls.append(("wgrad", self._wgrad_desc(src, op.src.c_off, op.cin, dq, 0, op.cout, 1, 1, z(i, "dw") + 4 * q * op.cout * op.cin)))
-                    calls.append(("conv", self._conv_desc(dq, 0, Wt["wt"][q], gsrc, op.src.c_off, accumulate=True),
-                                  dict(buf=op.src.buf, off=op.src.c_off, n=op.cin, full=True)))
-                bwd_rev.append(calls)
-                continue
-            # ---- BN-ed blocks: stem / rep / cba ----
-            dst, gdst = view(op.dst)
-            n, ho, wo, dct = dst.shape
-            count = n * ho * wo
-            br = Wt["br"]
-            nb = len(br)
-            st = self.stat_out[i]
-            xs = []
-            for b, ent in enumerate(br):
-                k = ent["k"]
-                if k == 0:
-                    src, _ = view(op.src)
-                    xs.append((src, op.src.c_off))
-                    self.ctx[i]["branches"][b]["x"] = src
-                    continue
-                raw = bf(n, ho, wo, op.cout)
-                self.ctx[i]["branches"][b]["x"] = raw
-                if op.kind == "stem":
-                    fwd.append(("stem", ops.stem_desc(self.x_static.data_ptr(), N, H, W, in_dtype == torch.uint8, ent["w"].data_ptr(), 0,
-                                                      op.cout, None, raw.data_ptr(), fp32_math=1)))
-                else:
-                    src, _ = view(op.src)
-                    fwd.append(("conv", self._conv_desc(src, op.src.c_off, ent["w"], raw, stride=op.s)))
-                xs.append((raw, 0))
-            qa = op.layout == "qa"
-            if qa:
-                # BN_d statistics of u, then t = BN_d(u) + v [+ x [+ avg3x3 x]] with the post-sum bn's statistics in one launch;
-                # from here on the block is a one-branch BatchNorm over t
-                u, v = xs[0][0], xs[1][0]
-                fwd.append(("stats", self._stats_desc([xs[0]], op.cout, count, z(i, "fsum"), z(i, "fcnt"), [(op.name + ".rbr_dense.bn", st[0])])))
-                tq = bf(n, ho, wo, op.cout)
-                q = self._qa_desc(op, u, v, st, tq, z(i, "qsum"), z(i, "qcnt"))
-                if op.identity:
-                    src, _ = view(op.src)
-                    q.x, q.x_pitch = src.data_ptr() + op.src.c_off * 2, src.shape[3]
-                fwd.append(("qa", q))
-                self.ctx[i].update(u=u, v=v, t=tq, stats_d=st[0], stats_p=st[1])
-                xs, st = [(tq, 0)], st[1:]
-            else:
-                fin = [(ent["prefix"] + (".bn" if ent["k"] else ""), st[b]) for b, ent in enumerate(br)]
-                fwd.append(("stats", self._stats_desc(xs, op.cout, count, z(i, "fsum"), z(i, "fcnt"), fin, op.w_row0)))
-            d = BnDesc()
-            d.nb, d.act, d.C, d.pixels = len(xs), ACT_CODES[op.act], op.cout, count
-            dcs = []
-            for b, (t, off) in enumerate(xs):
-                d.x[b], d.x_pitch[b] = t.data_ptr() + off * 2, t.shape[3]
-                d.mean[b], d.invstd[b] = st[b, 0].data_ptr(), st[b, 1].data_ptr()
-                d.scale[b], d.shift[b] = st[b, 2].data_ptr(), st[b, 3].data_ptr()
-                d.s2[b] = z(i, "s2") + 8 * b * op.cout
-                if br[b]["k"] == 0:      # identity branch: its input gradient goes straight into g(src)
-                    _, gsrc = view(op.src)
-                    d.dx[b], d.dx_pitch[b], d.accumulate[b] = gsrc.data_ptr() + op.src.c_off * 2, gsrc.shape[3], 1
-                    dcs.append(None)
-                else:
-                    dc = dc_pool[2 * (bn_ops & 1) + len([t for t in dcs if t is not None])][:count * op.cout].view(n, ho, wo, op.cout)
-                    d.dx[b], d.dx_pitch[b], d.accumulate[b] = dc.data_ptr(), op.cout, 0
-                    dcs.append(dc)
-            d.y, d.y_pitch = dst.data_ptr() + op.dst.c_off * 2, dct
-            d.dy, d.dy_pitch = gdst.data_ptr() + op.dst.c_off * 2, dct
-            d.s1 = z(i, "s1")
-            d.work, d.counter, d.coef, d.zeroed = z(i, "work"), z(i, "bcnt"), self.coef_out[i].data_ptr(), 1
-            if op.res is not None:
-                rbuf, grbuf = view(op.res)
-                d.res, d.res_pitch, d.res_alpha = rbuf.data_ptr() + op.res.c_off * 2, rbuf.shape[3], 1.0
-                if op.alpha in self.params:
-                    d.res_alpha_dev = fl.ptr(op.alpha)
-                d.dres, d.dres_pitch, d.dalpha = grbuf.data_ptr() + op.res.c_off * 2, grbuf.shape[3], z(i, "dalpha")
-            fwd.append(("apply", d))
-            calls.append(("dbg", (i, gdst[..., op.dst.c_off:op.dst.c_off + op.cout])))
-            wr = []      # gradient slices this launch writes besides the scratch tensors
-            for b in range(nb):
-                if br[b]["k"] == 0:
-                    wr.append(dict(buf=op.src.buf, off=op.src.c_off, n=op.cin, full=True, what=("dx", b)))
-            if op.res is not None:
-                wr.append(dict(buf=op.res.buf, off=op.res.c_off, n=op.cout, full=True, what=("dres", 0)))
-            par = bn_ops & 1
-            bn_ops += 1
-            calls.append(("bn_bwd", d, wr, par))
-            if qa:
-                # dt (d.dx[0]) -> BN_d backward (no activation) -> du; dt also feeds the 1x1 branch and the parameter-free identity /
-                # average-pool branches (yv6_qa_bwd into g(x)); the conv branches below then read dcs = [du, dt]
-                dt = dcs[0]
-                du = dc_pool[2 * par + 1][:count * op.cout].view(n, ho, wo, op.cout)
-                sd_ = self.stat_out[i][0]
-                d2 = BnDesc()
-                d2.nb, d2.act, d2.C, d2.pixels = 1, ACT_CODES[None], op.cout, count
-                d2.x[0], d2.x_pitch[0] = u.data_ptr(), op.cout
-                d2.mean[0], d2.invstd[0], d2.scale[0], d2.shift[0] = (sd_[r].data_ptr() for r in range(4))
-                d2.s2[0], d2.s1 = z(i, "s2d"), z(i, "s1d")
-                d2.dx[0], d2.dx_pitch[0], d2.accumulate[0] = du.data_ptr(), op.cout, 0
-                d2.dy, d2.dy_pitch = dt.data_ptr(), op.cout
-                d2.work, d2.counter, d2.coef, d2.zeroed = z(i, "workd"), z(i, "bcntd"), self.coef_out[i][1].data_ptr(), 1
-                calls.append(("bn_bwd", d2, [], par))
-                if op.identity:
-                    _, gsrc = view(op.src)
-                    qb = self._qa_desc(op, u, v, self.stat_out[i], tq, 0, 0)
-                    qb.dt, qb.dt_pitch = dt.data_ptr(), op.cout
-                    qb.dx, qb.dx_pitch = gsrc.data_ptr() + op.src.c_off * 2, gsrc.shape[3]
-                    calls.append(("qa_bwd", qb, dict(buf=op.src.buf, off=op.src.c_off, n=op.cin, full=True)))
-                dcs = [du, dt]
-            if op.kind == "stem":       # im2col once, then one tensor-core wgrad GEMM per branch
-                patches, patches_lo = bf(n, ho, wo, 32), bf(n, ho, wo, 32)     # image = hi + lo (bf16 planes)
-                self._stem_patches = (patches, patches_lo)
-                calls.append(("im2col", (self.x_static.data_ptr(), x_dt, 1.0 / 255.0, N, H, W, patches.data_ptr(), patches_lo.data_ptr())))
-                for b in range(nb):
-                    for pl in (patches, patches_lo):
-                        calls.append(("wgrad", self._wgrad_desc(pl, 0, 32, dcs[b], 0, op.cout, 1, 1, z(i, "dw", b)), par))
-            else:
-                src, gsrc = view(op.src)
-                for b, ent in enumerate(br):
-                    if ent["k"] == 0:
-                        continue
-                    calls.append(("wgrad", self._wgrad_desc(src, op.src.c_off, op.cin, dcs[b], 0, op.cout, ent["k"], op.s, z(i, "dw", b)), par))
-                    dds = self._dgrad_descs(dcs[b], ent, ent["k"], op.s, gsrc, op.src.c_off)
-                    # a stride-2 3x3 dgrad = four parity convolutions that together cover every pixel; 1x1 stride 2 covers one parity
-                    full = op.s == 1 or ent["k"] == 3
-                    for gi, dd in enumerate(dds):
-                        calls.append(("conv", dd, dict(buf=op.src.buf, off=op.src.c_off, n=op.cin, full=full, group=(i, b), first=gi == 0)))
-            bwd_rev.append(calls)
-        self.fwd_calls = fwd
-        bwd = []
+        self.scratch = _Scratch(dev, max([N * (H >> g.bufs[op.dst.buf].level) * (W >> g.bufs[op.dst.buf].level) * op.cout
+                                          for op in g.ops if op.kind in ("conv", "stem")] + [1]))
+        planners = {"pool": self._plan_pool, "pred": self._plan_pred, "convT": self._plan_convT}
+        self.fwd_calls = []
+        bwd_of_op = [planners.get(op.kind, self._plan_bn_block)(i, op) for i, op in enumerate(g.ops)]
+        self.bwd_calls = []
         for i in range(len(g.ops) - 1, -1, -1):
-            bwd.extend(bwd_rev[i])
+            self.bwd_calls += bwd_of_op[i]
             k = self.bucket_of_op.get(i)
             if k is not None and self.last_op_of_bucket[k] == i:
-                bwd.append(("bucket", k))
-        self.bwd_calls = bwd
-        self._keep = (dc_pool, pool_scr, dq_pool)
+                self.bwd_calls.append(Launch("bucket", None, kernels=0, parity=ALL, bucket=k))
         self._resolve_first_writers()
+
+    # ------------------------------------------------------------------ one planner per op kind: each appends the op's forward
+    # launches to self.fwd_calls and returns its backward launches
+    def _plan_pool(self, i, op):
+        """SPPF: y_j = maxpool5(y_{j-1}) into slice j of the concat, j = 1..3, in one launch; backward: three chained launches."""
+        buf, gbuf = self._view(op.dst)
+        n, h, w, ct = buf.shape
+        c = op.cin
+        self.fwd_calls.append(Launch("pool", "yv6_sppf_pool", (buf.data_ptr(), n, h, w, c, ct, 1, 0)))
+        scr = self.scratch.grown(self.scratch.pool, n * h * w * c, 1, torch.float32)[0]
+        bwd = []
+        for j in (3, 2, 1):
+            args = [buf.data_ptr() + (j - 1) * c * 2, ct, gbuf.data_ptr() + j * c * 2, ct, n, h, w, c, scr.data_ptr(),
+                    gbuf.data_ptr() + (j - 1) * c * 2, ct, 1]
+
+            def assign(a, args=args):       # the last argument: accumulate into g(y_{j-1})
+                args[-1] = 0 if a else 1
+            bwd.append(Launch("pool_bwd", "yv6_maxpool5_bwd", args, kernels=2, writes=[Write(op.dst.buf, (j - 1) * c, c, True, assign)]))
+        bwd[0].snapshot = (i, gbuf[..., :4 * c])
+        return bwd
+
+    def _plan_pred(self, i, op):
+        """Head prediction conv (cls / reg / reg_dist, or a fuse_ab one); backward from the loss gradient of its head tensor."""
+        src, _ = self._view(op.src)
+        Wt, z = self.wts[i], self._z
+        which, lvl = op.head
+        N, A, ch = src.shape[0], self.offs[-1], op.cout
+        lh, lw = self.sizes[lvl]
+        chp = (ch + 15) // 16 * 16
+        dl = self._bf(N, lh, lw, chp)               # bf16 gradient of the conv's output, zero padded to chp channels
+        self.scratch.dl.append(dl)
+        bwd = []
+        if which.endswith("_ab"):
+            # fuse_ab pred conv: natural NHWC output [N, hw, na * ch] (fp32, sigmoid fused on the class branch); the pack /
+            # grad kernels (csrc/yv6_fuseab.cu) move between it and the reference's (level, anchor, pixel) row order
+            raw = torch.empty(N, lh * lw, ch, dtype=torch.float32, device=self.dev)
+            st = self._ab.setdefault(lvl, {})
+            st[which] = (raw, dl)
+            self.fwd_calls.append(_desc_launch("conv", "yv6_conv_fwd", self._conv_desc(src, op.src.c_off, Wt["w"], raw, bias=Wt["bias"],
+                                                                                      act=op.act, y_strides=(lh * lw * ch, lw * ch, ch))))
+            if which == "reg_ab":          # second of the level's pair in forward order, first in backward order
+                from .arch import AB_ANCHORS
+                (raw_c, dl_c), (raw_r, dl_r) = st["cls_ab"], st["reg_ab"]
+                anchors = (C.c_float * 6)(*[v / float(self.g.strides[lvl]) for v in self.g.anchors_init[lvl]])   # effidehead_fuseab.py:35
+                rows = (AB_ANCHORS, self.g.num_classes, anchors, AB_ANCHORS * self.offs[lvl], self.cls_ab.shape[1])
+                self.fwd_calls.append(Launch("abp", "yv6_head_ab_pack", (raw_c.data_ptr(), raw_r.data_ptr(), N, lh * lw, *rows,
+                                                                         self.cls_ab.data_ptr(), self.reg_ab.data_ptr())))
+                bwd.append(Launch("abg", "yv6_head_ab_grad", (self.grad_cls_ab.data_ptr(), self.cls_ab.data_ptr(), self.grad_reg_ab.data_ptr(),
+                                                              raw_r.data_ptr(), N, lh * lw, *rows, dl_c.shape[3], dl_r.shape[3],
+                                                              dl_c.data_ptr(), dl_r.data_ptr())))
+        else:
+            out, grad = {"cls": (self.cls, self.grad_cls), "reg": (self.reg, self.grad_reg),
+                         "reg_dist": (getattr(self, "reg_dist", None), getattr(self, "grad_reg_dist", None))}[which]
+            self.fwd_calls.append(_desc_launch("conv", "yv6_conv_fwd", self._conv_desc(src, op.src.c_off, Wt["w"], out, bias=Wt["bias"],
+                                                                                      act=op.act, y_strides=(A * ch, lw * ch, ch),
+                                                                                      y_elem_off=self.offs[lvl] * ch)))
+            bwd.append(Launch("hgp", "yv6_head_grad_prep", (grad.data_ptr(), self.cls.data_ptr() if which == "cls" else 0, N, A, ch,
+                                                             self.offs[lvl], lh * lw, chp, dl.data_ptr())))
+        bwd.append(_desc_launch("wgrad", "yv6_conv_wgrad", self._wgrad_desc(src, op.src.c_off, op.cin, dl, 0, ch, 1, 1, z(i, "dw")), side=True))
+        bwd.append(_desc_launch("stats", "yv6_bn_stats_finalize", self._stats_desc([(dl, 0)], chp, N * lh * lw, z(i, "bsum"), z(i, "bcnt"))))
+        bwd.append(self._dgrad_launch(self._conv_desc(dl, 0, Wt["wt"], self.gbufs[op.src.buf], op.src.c_off, accumulate=True), op))
+        return bwd
+
+    def _plan_convT(self, i, op):
+        """ConvTranspose2d(k=2, s=2): four 1x1 convs, one per output quadrant (dy, dx), in the forward and the backward."""
+        src, gsrc = self._view(op.src)
+        dst, gdst = self._view(op.dst)
+        Wt, z = self.wts[i], self._z
+        N, dh, dw, dct = dst.shape
+        _, sh, sw, _ = src.shape
+        for q in range(4):
+            dy, dx = q // 2, q % 2
+            self.fwd_calls.append(_desc_launch("conv", "yv6_conv_fwd", self._conv_desc(
+                src, op.src.c_off, Wt["w"][q], dst, op.dst.c_off, bias=Wt["bias"], y_strides=(dh * dw * dct, 2 * dw * dct, 2 * dct),
+                y_elem_off=(dy * dw + dx) * dct)))
+        gd = gdst[..., op.dst.c_off:op.dst.c_off + op.cout]
+        # bias gradient = column sums of the whole upsampled gradient slice
+        bwd = [_desc_launch("stats", "yv6_bn_stats_finalize", self._stats_desc([(gdst, op.dst.c_off)], op.cout, N * dh * dw, z(i, "bsum"),
+                                                                                z(i, "bcnt")), snapshot=(i, gd))]
+        need = N * sh * sw * op.cout
+        pool = self.scratch.grown(self.scratch.quad, need, 4, torch.bfloat16)
+        for q in range(4):
+            dy, dx = q // 2, q % 2
+            dq = pool[q][:need].view(N, sh, sw, op.cout)
+            # the gradient of quadrant q, dense; the quadrant buffers are reused, so the copy waits for every weight gradient
+            bwd.append(Launch("copy", lambda sp, dq=dq, s=gd[:, dy::2, dx::2, :]: dq.copy_(s), parity=ALL))
+            bwd.append(_desc_launch("wgrad", "yv6_conv_wgrad", self._wgrad_desc(src, op.src.c_off, op.cin, dq, 0, op.cout, 1, 1,
+                                                                                z(i, "dw") + 4 * q * op.cout * op.cin), side=True))
+            bwd.append(self._dgrad_launch(self._conv_desc(dq, 0, Wt["wt"][q], gsrc, op.src.c_off, accumulate=True), op))
+        return bwd
+
+    def _plan_bn_block(self, i, op):
+        """BatchNorm-ed block (stem / rep / cba / cm / qa): raw convs of its branches -> batch statistics -> BN apply +
+        activation.  Backward: BN backward into the dc scratch pair of the block's parity, then _plan_branch_grads."""
+        z, sc = self._z, self.scratch
+        dst, gdst = self._view(op.dst)
+        src, gsrc = self._view(op.src) if op.kind != "stem" else (None, None)
+        n, ho, wo, dct = dst.shape
+        count = n * ho * wo
+        br, st = self.wts[i]["br"], self.stat_out[i]
+        xs = []
+        for b, ent in enumerate(br):
+            if ent["k"] == 0:
+                xs.append((src, op.src.c_off))
+            else:
+                raw = self._bf(n, ho, wo, op.cout)
+                if op.kind == "stem":
+                    N, H, W, in_dtype = self._shape
+                    self.fwd_calls.append(_desc_launch("stem", "yv6_stem_fwd", ops.stem_desc(
+                        self.x_static.data_ptr(), N, H, W, in_dtype == torch.uint8, ent["w"].data_ptr(), 0, op.cout, None, raw.data_ptr(),
+                        fp32_math=1)))
+                else:
+                    self.fwd_calls.append(_desc_launch("conv", "yv6_conv_fwd", self._conv_desc(src, op.src.c_off, ent["w"], raw, stride=op.s)))
+                xs.append((raw, 0))
+            self.ctx[i]["branches"][b]["x"] = xs[-1][0]
+        if op.layout == "qa":
+            xs, st = self._plan_qa_fwd(i, op, xs, count), st[1:]
+        else:
+            fin = [(ent["prefix"] + (".bn" if ent["k"] else ""), st[b]) for b, ent in enumerate(br)]
+            self.fwd_calls.append(_desc_launch("stats", "yv6_bn_stats_finalize", self._stats_desc(
+                xs, op.cout, count, z(i, "fsum"), z(i, "fcnt"), fin, op.w_row0)))
+        par, sc.bn_ops = sc.bn_ops & 1, sc.bn_ops + 1
+        d = BnDesc()
+        d.nb, d.act, d.C, d.pixels = len(xs), ACT_CODES[op.act], op.cout, count
+        dcs, writes = [], []     # writes: the gradient slices this launch writes besides the scratch tensors
+        for b, (t, off) in enumerate(xs):
+            d.x[b], d.x_pitch[b] = t.data_ptr() + off * 2, t.shape[3]
+            d.mean[b], d.invstd[b] = st[b, 0].data_ptr(), st[b, 1].data_ptr()
+            d.scale[b], d.shift[b] = st[b, 2].data_ptr(), st[b, 3].data_ptr()
+            d.s2[b] = z(i, "s2") + 8 * b * op.cout
+            if br[b]["k"] == 0:      # identity branch: its input gradient goes straight into g(src)
+                d.dx[b], d.dx_pitch[b], d.accumulate[b] = gsrc.data_ptr() + op.src.c_off * 2, gsrc.shape[3], 1
+
+                def dx_assign(a, b=b):
+                    d.accumulate[b] = 0 if a else 1
+                writes.append(Write(op.src.buf, op.src.c_off, op.cin, True, dx_assign))
+                dcs.append(None)
+            else:
+                dc = sc.dc_view(par, len([t for t in dcs if t is not None]), (n, ho, wo, op.cout))
+                d.dx[b], d.dx_pitch[b], d.accumulate[b] = dc.data_ptr(), op.cout, 0
+                dcs.append(dc)
+        d.y, d.y_pitch = dst.data_ptr() + op.dst.c_off * 2, dct
+        d.dy, d.dy_pitch = gdst.data_ptr() + op.dst.c_off * 2, dct
+        d.s1 = z(i, "s1")
+        d.work, d.counter, d.coef, d.zeroed = z(i, "work"), z(i, "bcnt"), self.coef_out[i].data_ptr(), 1
+        if op.res is not None:
+            rbuf, grbuf = self._view(op.res)
+            d.res, d.res_pitch, d.res_alpha = rbuf.data_ptr() + op.res.c_off * 2, rbuf.shape[3], 1.0
+            if op.alpha in self.params:
+                d.res_alpha_dev = self.flat.ptr(op.alpha)
+            d.dres, d.dres_pitch, d.dalpha = grbuf.data_ptr() + op.res.c_off * 2, grbuf.shape[3], z(i, "dalpha")
+            writes.append(Write(op.res.buf, op.res.c_off, op.cout, True, lambda a: setattr(d, "dres_assign", int(a))))
+        self.fwd_calls.append(_desc_launch("apply", "yv6_bn_apply_fwd", d))
+        bwd = [_desc_launch("bn_bwd", "yv6_bn_bwd", d, kernels=2, parity=par, writes=writes,
+                            snapshot=(i, gdst[..., op.dst.c_off:op.dst.c_off + op.cout]))]
+        if op.layout == "qa":
+            qa_bwd, dcs = self._plan_qa_bwd(i, op, dcs[0], par)
+            bwd += qa_bwd
+        return bwd + self._plan_branch_grads(i, op, dcs, par)
+
+    def _plan_qa_fwd(self, i, op, xs, count):
+        """QA block: BN_d statistics of u, then t = BN_d(u) + v [+ x [+ avg3x3 x]] with the post-sum bn's statistics in one
+        launch.  Returns [(t, 0)]: from here on the block is a one-branch BatchNorm over t."""
+        z, st = self._z, self.stat_out[i]
+        (u, _), (v, _) = xs
+        self.fwd_calls.append(_desc_launch("stats", "yv6_bn_stats_finalize", self._stats_desc(
+            [xs[0]], op.cout, count, z(i, "fsum"), z(i, "fcnt"), [(op.name + ".rbr_dense.bn", st[0])])))
+        tq = self._bf(*u.shape)
+        q = self._qa_desc(op, u, v, st, tq, z(i, "qsum"), z(i, "qcnt"))
+        if op.identity:
+            src = self.bufs[op.src.buf]
+            q.x, q.x_pitch = src.data_ptr() + op.src.c_off * 2, src.shape[3]
+        self.fwd_calls.append(_desc_launch("qa", "yv6_qa_fwd", q))
+        self.ctx[i].update(u=u, v=v, t=tq, stats_d=st[0], stats_p=st[1])
+        return [(tq, 0)]
+
+    def _plan_qa_bwd(self, i, op, dt, par):
+        """QA block after the post-sum bn's backward: dt -> BN_d backward (no activation) -> du; dt also feeds the 1x1 branch and
+        the parameter-free identity / average-pool branches (yv6_qa_bwd into g(x)).  Returns the launches and the gradients of
+        the conv branches' outputs, [du, dt]."""
+        z, ctx = self._z, self.ctx[i]
+        du = self.scratch.dc_view(par, 1, dt.shape)
+        sd = self.stat_out[i][0]
+        d = BnDesc()
+        d.nb, d.act, d.C, d.pixels = 1, ACT_CODES[None], op.cout, dt.numel() // op.cout
+        d.x[0], d.x_pitch[0] = ctx["u"].data_ptr(), op.cout
+        d.mean[0], d.invstd[0], d.scale[0], d.shift[0] = (sd[r].data_ptr() for r in range(4))
+        d.s2[0], d.s1 = z(i, "s2d"), z(i, "s1d")
+        d.dx[0], d.dx_pitch[0], d.accumulate[0] = du.data_ptr(), op.cout, 0
+        d.dy, d.dy_pitch = dt.data_ptr(), op.cout
+        d.work, d.counter, d.coef, d.zeroed = z(i, "workd"), z(i, "bcntd"), self.coef_out[i][1].data_ptr(), 1
+        bwd = [_desc_launch("bn_bwd", "yv6_bn_bwd", d, kernels=2, parity=par)]
+        if op.identity:
+            gsrc = self.gbufs[op.src.buf]
+            qb = self._qa_desc(op, ctx["u"], ctx["v"], self.stat_out[i], ctx["t"], 0, 0)
+            qb.dt, qb.dt_pitch = dt.data_ptr(), op.cout
+            qb.dx, qb.dx_pitch = gsrc.data_ptr() + op.src.c_off * 2, gsrc.shape[3]
+            bwd.append(_desc_launch("qa_bwd", "yv6_qa_bwd", qb, writes=[Write(op.src.buf, op.src.c_off, op.cin, True,
+                                                                               lambda a: setattr(qb, "accumulate", int(not a)))]))
+        return bwd, [du, dt]
+
+    def _plan_branch_grads(self, i, op, dcs, par):
+        """Weight gradients (side stream; they read the dc pair `par`) and input gradients of the conv branches of a BN-ed block,
+        from the gradients dcs[b] of the branches' raw outputs."""
+        z, br = self._z, self.wts[i]["br"]
+        bwd = []
+        if op.kind == "stem":       # im2col once, then one tensor-core wgrad GEMM per branch
+            N, H, W, in_dtype = self._shape
+            patches, patches_lo = self._bf(*dcs[0].shape[:3], 32), self._bf(*dcs[0].shape[:3], 32)     # image = hi + lo (bf16 planes)
+            self._stem_patches = (patches, patches_lo)
+            bwd.append(Launch("im2col", "yv6_stem_im2col", (self.x_static.data_ptr(), DT_U8 if in_dtype == torch.uint8 else DT_F32,
+                                                            1.0 / 255.0, N, H, W, patches.data_ptr(), patches_lo.data_ptr())))
+            for b in range(len(br)):
+                for pl in (patches, patches_lo):
+                    bwd.append(_desc_launch("wgrad", "yv6_conv_wgrad", self._wgrad_desc(pl, 0, 32, dcs[b], 0, op.cout, 1, 1, z(i, "dw", b)),
+                                            side=True, parity=par))
+            return bwd
+        src, gsrc = self._view(op.src)
+        for b, ent in enumerate(br):
+            if ent["k"] == 0:
+                continue
+            bwd.append(_desc_launch("wgrad", "yv6_conv_wgrad", self._wgrad_desc(src, op.src.c_off, op.cin, dcs[b], 0, op.cout, ent["k"], op.s,
+                                                                                z(i, "dw", b)), side=True, parity=par))
+            # a stride-2 3x3 dgrad = four parity convolutions that together cover every pixel; 1x1 stride 2 covers one parity
+            full = op.s == 1 or ent["k"] == 3
+            for d in self._dgrad_descs(dcs[b], ent, op.s, gsrc, op.src.c_off):
+                bwd.append(self._dgrad_launch(d, op, full, group=(i, b)))
+        return bwd
 
     def _resolve_first_writers(self):
         """Gradient buffers are accumulated into by every consumer of a tensor.  Instead of clearing all of them at the start of
@@ -703,41 +784,25 @@ class TrainEngine:
             for t in self.g.feat:
                 cov[t.buf][t.c_off:t.c_off + t.c] = True
 
-        def decide(m):
-            seg = cov[m["buf"]][m["off"]:m["off"] + m["n"]]
-            if m["full"] and not seg.any():
+        def decide(w):
+            seg = cov[w.buf][w.off:w.off + w.n]
+            if w.full and not seg.any():
                 assign = True
             else:
                 assign = False
                 if not seg.all():
-                    need_zero.add(m["buf"])
+                    need_zero.add(w.buf)
             seg[:] = True
             return assign
 
-        for c in self.bwd_calls:
-            kind = c[0]
-            if kind == "conv" and len(c) > 2:
-                m, d = c[2], c[1]
-                if "group" in m:
-                    if m["first"]:
-                        group_decision[m["group"]] = decide(m)
-                    assign = group_decision[m["group"]]
+        for launch in self.bwd_calls:
+            for w in launch.writes:
+                if w.group is None:
+                    w.assign(decide(w))
                 else:
-                    assign = decide(m)
-                if assign:          # y = conv(...) instead of y += conv(...): no residual read
-                    d.res, d.alpha = 0, 0.0
-            elif kind == "bn_bwd":
-                d = c[1]
-                for m in c[2]:
-                    assign = decide(m)
-                    if m["what"][0] == "dx":
-                        d.accumulate[m["what"][1]] = 0 if assign else 1
-                    else:
-                        d.dres_assign = 1 if assign else 0
-            elif kind == "pool_bwd":
-                c[1][11] = 0 if decide(c[2]) else 1
-            elif kind == "qa_bwd":
-                c[1].accumulate = 0 if decide(c[2]) else 1
+                    if w.group not in group_decision:
+                        group_decision[w.group] = decide(w)
+                    w.assign(group_decision[w.group])
         for i, cv in enumerate(cov):        # slices nobody writes are read as zero gradients
             if not cv.all():
                 need_zero.add(i)
@@ -745,18 +810,9 @@ class TrainEngine:
 
     # ================================================================== execution
     def launch_counts(self):
-        """(forward, backward) kernel launches of the current plan, excluding the arena memset and the two repack launches."""
-        f = len(self.fwd_calls)
-        b = 0
-        for c in self.bwd_calls:
-            kind = c[0]
-            if kind == "bn_bwd" or kind == "pool_bwd":
-                b += 2
-            elif kind in ("dbg", "bucket"):
-                continue
-            else:
-                b += 1
-        return f, b + len(self.grad_tables)
+        """(forward, backward) kernel launches of the current plan, excluding the arena memset and the two repack launches; every
+        gradient unpack table counts once."""
+        return sum(c.kernels for c in self.fwd_calls), sum(c.kernels for c in self.bwd_calls) + len(self.grad_tables)
 
     def begin_step(self, sp=None):
         """Clears the per-step accumulators and repacks the master weights into the kernels' layouts."""
@@ -782,38 +838,8 @@ class TrainEngine:
         return self.cls, self.reg
 
     def run_forward(self, sp):
-        lib, h, chk = self.lib, self.h, _lib.check
-        for kind, d in self.fwd_calls:
-            if kind == "conv":
-                chk(lib.yv6_conv_fwd(h, C.byref(d), sp))
-            elif kind == "stats":
-                chk(lib.yv6_bn_stats_finalize(h, C.byref(d), sp))
-            elif kind == "apply":
-                chk(lib.yv6_bn_apply_fwd(h, C.byref(d), sp))
-            elif kind == "stem":
-                chk(lib.yv6_stem_fwd(h, C.byref(d), sp))
-            elif kind == "qa":
-                chk(lib.yv6_qa_fwd(h, C.byref(d), sp))
-            elif kind == "abp":
-                self._ab_call(d, False, sp)
-            else:
-                chk(lib.yv6_sppf_pool(h, C.c_void_p(d[0]), d[1], d[2], d[3], d[4], d[5], d[6], d[7], sp))
-
-    def _ab_call(self, lvl, backward, sp):
-        """fuse_ab level `lvl`: natural-order conv outputs -> (cls_ab, reg_ab) rows, or their gradients -> dense bf16 gradients."""
-        from .arch import AB_ANCHORS
-        st = self._ab[lvl]
-        N = self.cls_ab.shape[0]
-        lh, lw = self.sizes[lvl]
-        nc, A3 = self.g.num_classes, self.cls_ab.shape[1]
-        off3 = AB_ANCHORS * self.offs[lvl]
-        if not backward:
-            _lib.check(self.lib.yv6_head_ab_pack(self.h, _p(st["raw_cls"]), _p(st["raw_reg"]), N, lh * lw, AB_ANCHORS, nc, st["anchors"],
-                                                 off3, A3, _p(self.cls_ab), _p(self.reg_ab), sp))
-        else:
-            _lib.check(self.lib.yv6_head_ab_grad(self.h, _p(self.grad_cls_ab), _p(self.cls_ab), _p(self.grad_reg_ab), _p(st["raw_reg"]), N,
-                                                 lh * lw, AB_ANCHORS, nc, st["anchors"], off3, A3, st["dl_cls"].shape[3], st["dl_reg"].shape[3],
-                                                 _p(st["dl_cls"]), _p(st["dl_reg"]), sp))
+        for c in self.fwd_calls:
+            c.run(self.lib, self.h, sp)
 
     def backward(self, grad_cls, grad_reg, accumulate=False, first=0, last=None, grad_cls_ab=None, grad_reg_ab=None, grad_reg_dist=None):
         """Writes d(loss)/d(parameter) of every trainable parameter into the flat gradient buffer (`accumulate`: adds to it)
@@ -829,7 +855,7 @@ class TrainEngine:
             for buf, gr in ((self.grad_cls_ab, grad_cls_ab), (self.grad_reg_ab, grad_reg_ab)):
                 if gr is not None and gr.data_ptr() != buf.data_ptr():
                     buf.copy_(gr)
-        lib, h, chk = self.lib, self.h, _lib.check
+        lib, h = self.lib, self.h
         sp = _lib.stream_ptr()
         if first == 0:
             for gb in self.zero_gbufs:
@@ -856,65 +882,38 @@ class TrainEngine:
         ssp = _lib.stream_ptr(side) if overlap else sp
         pending = []             # (event recorded on the side stream after a wgrad, scratch parity or None)
 
-        def wait_pending(par=-1):
-            keep = []
+        def wait_pending(par=ALL):
             for ev, q in pending:
-                if par == -1 or q == par:
+                if par == ALL or q == par:
                     main.wait_event(ev)
-                else:
-                    keep.append((ev, q))
-            pending[:] = keep
+            pending[:] = [(ev, q) for ev, q in pending if not (par == ALL or q == par)]
 
         for c in calls[first:]:
-            kind, d = c[0], c[1]
-            if kind == "conv":
-                chk(lib.yv6_conv_fwd(h, C.byref(d), sp))
-            elif kind == "wgrad":
-                if overlap:
-                    ev = torch.cuda.Event()
-                    ev.record(main)
-                    side.wait_event(ev)
-                    chk(lib.yv6_conv_wgrad(h, C.byref(d), ssp))
-                    done = torch.cuda.Event()
-                    done.record(side)
-                    pending.append((done, c[2] if len(c) > 2 else None))
-                else:
-                    chk(lib.yv6_conv_wgrad(h, C.byref(d), sp))
-            elif kind == "bn_bwd":
-                if overlap:
-                    wait_pending(c[3])
-                chk(lib.yv6_bn_bwd(h, C.byref(d), sp))
-            elif kind == "stats":
-                chk(lib.yv6_bn_stats_finalize(h, C.byref(d), sp))
-            elif kind == "qa_bwd":
-                chk(lib.yv6_qa_bwd(h, C.byref(d), sp))
-            elif kind == "copy":
-                if overlap:
-                    wait_pending()
-                d[0].copy_(d[1])
-            elif kind == "abg":
-                self._ab_call(d, True, sp)
-            elif kind == "hgp":
-                chk(lib.yv6_head_grad_prep(h, d[0], d[1], d[2], d[3], d[4], d[5], d[6], d[7], d[8], sp))
-            elif kind == "pool_bwd":
-                chk(lib.yv6_maxpool5_bwd(h, d[0], d[1], d[2], d[3], d[4], d[5], d[6], d[7], d[8].data_ptr(), d[9], d[10], d[11], sp))
-            elif kind == "im2col":
-                chk(lib.yv6_stem_im2col(h, *d, sp))
-            elif kind == "bucket":
-                if overlap:
-                    wait_pending()
-                self.grad_tables[d].launch(lib, h, accumulate, sp)
+            if self.debug and c.snapshot is not None:
+                self.dbg[c.snapshot[0]] = dict(gdst=c.snapshot[1].clone())
+            if overlap and c.side:
+                ev = torch.cuda.Event()
+                ev.record(main)
+                side.wait_event(ev)
+                c.run(lib, h, ssp)
+                done = torch.cuda.Event()
+                done.record(side)
+                pending.append((done, c.parity))
+                continue
+            if overlap and c.parity is not None:
+                wait_pending(c.parity)
+            if c.bucket is not None:
+                self.grad_tables[c.bucket].launch(lib, h, accumulate, sp)
                 if self.bucket_hook is not None:
-                    self.bucket_hook(d)
-            elif kind == "dbg":
-                if self.debug:
-                    self.dbg[d[0]] = dict(gdst=d[1].clone())
+                    self.bucket_hook(c.bucket)
+            else:
+                c.run(lib, h, sp)
         if overlap:
             wait_pending()      # every call (and every captured graph segment) ends joined
 
     def bucket_call_index(self):
         """Indices into the backward call list right after each bucket's unpack (segment boundaries for graph capture)."""
-        return [j + 1 for j, c in enumerate(self.bwd_calls) if c[0] == "bucket"]
+        return [j + 1 for j, c in enumerate(self.bwd_calls) if c.bucket is not None]
 
 
 class _HeadFn(torch.autograd.Function):
