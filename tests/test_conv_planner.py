@@ -1,7 +1,7 @@
 """CPU checks of the conv tile planner (`plan_conv` of yolov6_b200/csrc/yv6_conv_igemm.cu) through the host-only C-ABI entry
 `yv6_conv_plan_host`, with the H100 SXM's device properties stated explicitly (132 SMs, 232448 bytes of opt-in shared memory, 66
 co-resident CTA pairs):
-every conv launch the inference engine makes (engine.conv_launches: fused head siblings, column-pair views) for every supported
+every conv launch the inference engine makes (engine.forward_launches: fused head siblings, column-pair views) for every supported
 model (reference configs/yolov6{n,s,m}.py, yolov6l6.py) at the BASELINE.json configurations gets a plan that fits the SM, and the
 YOLOv6-S plans of the benchmark configuration are pinned.  No compute, no GPU."""
 import ctypes as C
@@ -11,7 +11,7 @@ import pytest
 from yolov6_b200 import _lib, ops
 from yolov6_b200.arch import build_graph
 from yolov6_b200.configs import get_config
-from yolov6_b200.engine import conv_launches, siblings
+from yolov6_b200.engine import forward_launches
 
 H100 = (132, 232448, 66)
 
@@ -26,8 +26,7 @@ def plan(d):
 def layer_descs(name, batch, size):
     """(op name, descriptor) of every conv launch of the bf16 inference engine's forward, at fake 16-byte-aligned addresses."""
     g = build_graph(get_config(name), 80, name)
-    launches = conv_launches(g, batch, size, size, 1, siblings(g), lambda *key: 1 << 20, plan)
-    return [(g.ops[i].name, d) for i, ds in launches.items() for d in ds]
+    return [(r.name, r.desc) for r in forward_launches(g, batch, size, size, 1, lambda *key: 1 << 20, plan) if r.kind == "conv"]
 
 
 @pytest.mark.parametrize("name,batch,size", [("yolov6n", 32, 640), ("yolov6s", 32, 640), ("yolov6s", 1, 64), ("yolov6m", 8, 640),

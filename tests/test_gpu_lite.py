@@ -178,7 +178,7 @@ def test_forward_at_native_size_matches_reference(name, B, H, W, step, precision
 
 
 @pytest.mark.parametrize("precision", ["fp32", "bf16"])
-def test_captured_forward_equals_eager_bit_for_bit(precision):
+def test_captured_graph_replays_the_eager_forward_bit_for_bit(precision):
     m = load("yolov6lite_m", precision)
     eng = m.engine()
     x = fab.synthetic_images(4, 192, 320, seed=1).cuda()
@@ -197,7 +197,7 @@ def test_captured_forward_equals_eager_bit_for_bit(precision):
         graph.replay()
         torch.cuda.synchronize()
     assert torch.equal(out, eager)
-    assert eng.launch_count(4, 192, 320) == len(eng._plan(4, 192, 320, torch.float32)["calls"]) + 1
+    assert eng.launch_count(4, 192, 320) == len(eng.launches(4, 192, 320)) + 1
 
 
 def test_detect_pipeline_matches_eager_model_plus_nms():

@@ -21,7 +21,7 @@ from oracle import fabricate as fab
 from oracle import lite
 from yolov6_b200 import _lib, arch, configs, ops
 from yolov6_b200.checkpoint import _matching_config
-from yolov6_b200.engine import conv_launches, siblings, stem_channels, window_weights
+from yolov6_b200.engine import forward_launches, stem_channels, window_weights
 from yolov6_b200.fold import fold_op, se_weights
 from yolov6_b200.model import build_model
 
@@ -115,14 +115,14 @@ def test_oracle_matches_reference_at_native_size(name, B, H, W, step):
 
 def run_lite_cpu(g, sd, x):
     """Replays the launch list of the Lite graph in float64 on the CPU, on buffers with the engine's channel pitches: the conv
-    launches read the channel window of their descriptor (conv_launches) with the zero-column weights of window_weights, the
+    launches read the channel window of their descriptor (forward_launches) with the zero-column weights of window_weights, the
     stem writes its padded channel count, and the depthwise / SE / shuffle / upsample ops run as their kernels define them.
     Returns (cls, reg) and the buffers."""
     N, _, H, W = x.shape
     bufs = [torch.zeros(N, b.c_total, H >> b.level, W >> b.level, dtype=torch.float64) for b in g.bufs]
     base = lambda b: (b + 1) << 32        # noqa: E731
-    launches = conv_launches(g, N, H, W, 1, siblings(g),
-                             lambda kind, key, q=0: base(key) if kind == "buf" else 1 << 20, lambda d: {"halo": 0})
+    descs = {r.name: r.desc for r in forward_launches(g, N, H, W, 1, lambda kind, key, q=0: base(key) if kind == "buf" else 1 << 20,
+                                                      lambda d: {"halo": 0}) if r.kind == "conv"}
     heads = {"cls": [None] * 4, "reg": [None] * 4}
     act = {"hardswish": F.hardswish, "sigmoid": torch.sigmoid, None: lambda t: t}
 
@@ -149,7 +149,7 @@ def run_lite_cpu(g, sd, x):
             w, b = torch.cat([w, w.new_zeros((cp - op.cout,) + w.shape[1:])]), torch.cat([b, b.new_zeros(cp - op.cout)])
             bufs[op.dst.buf][:] = act[op.act](F.conv2d(x.double(), w.permute(0, 3, 1, 2), b, 2, 1))
         else:
-            (d,) = launches[i]
+            d = descs[op.name]
             off = (d.x - base(op.src.buf)) // 2
             w, b = fold_op(sd, op)
             w = window_weights(g, op, w)
@@ -202,14 +202,14 @@ def _plan(d):
 def test_every_conv_launch_is_aligned_and_gets_a_plan_that_fits_the_sm(name):
     g = arch.build_graph(configs.get_config(name), 80, name)
     for batch, H, W in ((32, 320, 320), (1, 192, 320), (2, 128, 128)):
-        launches = conv_launches(g, batch, H, W, 1, siblings(g), lambda *key: 1 << 20, _plan)
-        assert len(launches) == sum(1 for op in g.ops if op.kind in ("conv", "pred"))
-        for i, ds in launches.items():
-            for d in ds:
-                assert d.Cin % 16 == 0 and d.x % 16 == 0 and d.x_c_total % 16 == 0, (g.ops[i].name, d.Cin, d.x)
-                p = _plan(d)
-                assert 0 < p["smem"] <= H100[1] and p["threads"] == 384, (g.ops[i].name, p)
-                assert 1 <= p["grid"] <= H100[0] and p["stages"] >= 2, (g.ops[i].name, p)
+        convs = [r for r in forward_launches(g, batch, H, W, 1, lambda *key: 1 << 20, _plan) if r.kind == "conv"]
+        assert len(convs) == sum(1 for op in g.ops if op.kind in ("conv", "pred"))
+        for r in convs:
+            d = r.desc
+            assert d.Cin % 16 == 0 and d.x % 16 == 0 and d.x_c_total % 16 == 0, (r.name, d.Cin, d.x)
+            p = _plan(d)
+            assert 0 < p["smem"] <= H100[1] and p["threads"] == 384, (r.name, p)
+            assert 1 <= p["grid"] <= H100[0] and p["stages"] >= 2, (r.name, p)
 
 
 def test_every_lite_layout_is_matched_back_to_its_name():

@@ -22,7 +22,7 @@ from test_graph import _run_graph_cpu
 from test_model_zoo import H100, _Cfg, _plan
 from yolov6_b200 import _lib, arch, configs
 from yolov6_b200.checkpoint import _matching_config
-from yolov6_b200.engine import conv_launches, siblings
+from yolov6_b200.engine import forward_launches, siblings
 from yolov6_b200.model import build_model
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -219,8 +219,7 @@ def test_qa_ops_train_with_both_batchnorms_and_the_bare_1x1():
 
 def _descs(name, N, S):
     g = arch.build_graph(configs.get_config(name), 80, name)
-    launches = conv_launches(g, N, S, S, 1, siblings(g), lambda *key: 1 << 20, _plan)
-    return g, [(g.ops[i].kind, bytes(d)) for i in sorted(launches) for d in launches[i]]
+    return g, [(r.name, bytes(r.desc)) for r in forward_launches(g, N, S, S, 1, lambda *key: 1 << 20, _plan) if r.kind == "conv"]
 
 
 @pytest.mark.parametrize("base", ["yolov6n", "yolov6s", "yolov6m"])
@@ -238,10 +237,9 @@ def test_folded_inference_graph_is_the_float_models_graph(base):
 def test_every_conv_launch_gets_a_plan_that_fits_the_sm(name):
     g = arch.build_graph(configs.get_config(name), 80, name)
     for size, batch in ((640, 32), (SIZE, 2)):
-        launches = conv_launches(g, batch, size, size, 1, siblings(g), lambda *key: 1 << 20, _plan)
-        assert sum(1 for op in g.ops if op.kind in ("conv", "pred", "convT")) <= sum(len(v) for v in launches.values()) + len(siblings(g))
-        for i, ds in launches.items():
-            for d in ds:
-                p = _plan(d)
-                assert 0 < p["smem"] <= H100[1] and p["threads"] == 384, (g.ops[i].name, p)
-                assert 1 <= p["grid"] <= H100[0] and p["stages"] >= 2, (g.ops[i].name, p)
+        convs = [r for r in forward_launches(g, batch, size, size, 1, lambda *key: 1 << 20, _plan) if r.kind == "conv"]
+        assert sum(1 for op in g.ops if op.kind in ("conv", "pred", "convT")) <= len(convs) + len(siblings(g))
+        for r in convs:
+            p = _plan(r.desc)
+            assert 0 < p["smem"] <= H100[1] and p["threads"] == 384, (r.name, p)
+            assert 1 <= p["grid"] <= H100[0] and p["stages"] >= 2, (r.name, p)

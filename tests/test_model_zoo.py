@@ -18,7 +18,7 @@ from oracle import zoo
 from test_graph import _run_graph_cpu
 from yolov6_b200 import _lib, arch, configs, ops
 from yolov6_b200.checkpoint import _matching_config
-from yolov6_b200.engine import conv_launches, siblings
+from yolov6_b200.engine import forward_launches, siblings
 from yolov6_b200.model import Model, build_model
 
 MODELS = {"yolov6l": 64, "yolov6n6": 128, "yolov6s6": 128, "yolov6m6": 128,
@@ -203,10 +203,9 @@ def test_every_conv_launch_gets_a_plan_that_fits_the_sm(name):
     g = arch.build_graph(configs.get_config(name), 80, name)
     native, small = (1280, 8) if len(g.strides) == 4 else (640, 32), (MODELS[name], 2)
     for size, batch in (native, small):
-        launches = conv_launches(g, batch, size, size, 1, siblings(g), lambda *key: 1 << 20, _plan)
-        assert sum(1 for op in g.ops if op.kind in ("conv", "pred", "convT")) <= sum(len(v) for v in launches.values()) + len(siblings(g))
-        for i, ds in launches.items():
-            for d in ds:
-                p = _plan(d)
-                assert 0 < p["smem"] <= H100[1] and p["threads"] == 384, (g.ops[i].name, p)
-                assert 1 <= p["grid"] <= H100[0] and p["stages"] >= 2, (g.ops[i].name, p)
+        convs = [r for r in forward_launches(g, batch, size, size, 1, lambda *key: 1 << 20, _plan) if r.kind == "conv"]
+        assert sum(1 for op in g.ops if op.kind in ("conv", "pred", "convT")) <= len(convs) + len(siblings(g))
+        for r in convs:
+            p = _plan(r.desc)
+            assert 0 < p["smem"] <= H100[1] and p["threads"] == 384, (r.name, p)
+            assert 1 <= p["grid"] <= H100[0] and p["stages"] >= 2, (r.name, p)

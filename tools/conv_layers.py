@@ -59,7 +59,7 @@ def main():
     with torch.no_grad():
         result["default"] = measure(eng, x, args.iters)
         if args.pair:
-            descs = [d for kind, d in eng._plan(BATCH, SIZE, SIZE, torch.float32)["calls"] if kind == "conv"]
+            descs = [r.desc for r in eng.launches(BATCH, SIZE, SIZE) if r.kind == "conv"]
             for d in descs:
                 d.force_pair = 1
             try:

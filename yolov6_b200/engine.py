@@ -12,6 +12,7 @@ equivalent products, used for the 1e-4 parity bar of BASELINE.json).
 import ctypes as C
 import itertools
 import os
+from dataclasses import dataclass
 
 import torch
 
@@ -96,6 +97,35 @@ def stem_channels(g, op):
     return g.bufs[op.dst.buf].c_total
 
 
+@dataclass(eq=False)
+class InferLaunch(ops.Launch):
+    """One launch of the inference forward (ops.Launch) with what the scheduler and the profilers need: the op `name`, the
+    (buffer, first channel, end channel) spans it `reads` and `writes` -- buffers are ("buf", graph buffer index), ("fused",
+    first conv of a sibling pair) or ("head", "cls" | "reg", level) --, `head` "cls" | "reg" for a head conv (its output moves
+    with the head set), and for a conv launch `conv`: its geometry (cin, cout, k, s, input h, w, output ho, wo), algorithmic
+    `flops` (the column-pair view's zero taps do not count) and `y_f32`."""
+    name: str = ""
+    reads: tuple = ()
+    writes: tuple = ()
+    head: str = None
+    conv: dict = None
+
+
+def _viewer(g, N, H, W, sibling, addr):
+    """view(t) -> (buffer key, address, channel offset, (N, h, w, channel pitch)) of graph tensor slice t: buffers are ("buf",
+    graph buffer index) or, for the outputs of a sibling pair, ("fused", first conv of the pair)."""
+    slices = sibling_slices(g, sibling)
+
+    def view(t):
+        b = g.bufs[t.buf]
+        nhw = (N, H >> b.level, W >> b.level)
+        if t.buf in slices:
+            i, c0, pitch = slices[t.buf]
+            return ("fused", i), addr("fused", i), c0 + t.c_off, nhw + (pitch,)
+        return ("buf", t.buf), addr("buf", t.buf), t.c_off, nhw + (b.c_total,)
+    return view
+
+
 def conv_launches(g, N, H, W, nsplit, sibling, addr, plan_fn):
     """Descriptors of the conv launches of one inference forward of graph g over an [N, 3, H, W] input, in launch order:
     {op index: [ConvDesc, ...]} -- four 1x1 quadrant launches for a transposed conv, one otherwise; the first conv of a sibling pair
@@ -109,18 +139,8 @@ def conv_launches(g, N, H, W, nsplit, sibling, addr, plan_fn):
     plan_fn(desc) -> plan dict (ops.PLAN_KEYS) decides where the column-pair view is kept."""
     offs = list(itertools.accumulate(((H // s) * (W // s) for s in g.strides), initial=0))    # first anchor of each level
     A = offs[-1]
-    slices = sibling_slices(g, sibling)
+    view = _viewer(g, N, H, W, sibling, addr)
     second = set(sibling.values())
-
-    def view(t):
-        """(address, channel offset, (N, h, w, channel pitch)) of graph tensor slice t."""
-        b = g.bufs[t.buf]
-        nhw = (N, H >> b.level, W >> b.level)
-        if t.buf in slices:
-            i, c0, pitch = slices[t.buf]
-            return addr("fused", i), c0 + t.c_off, nhw + (pitch,)
-        return addr("buf", t.buf), t.c_off, nhw + (b.c_total,)
-
     out = {}
     for i, op in enumerate(g.ops):
         if op.kind not in ("conv", "pred", "convT") or i in second:
@@ -128,7 +148,7 @@ def conv_launches(g, N, H, W, nsplit, sibling, addr, plan_fn):
         if op.kind == "pred" and op.head[0] not in ("cls", "reg"):
             continue                      # eval forward: anchor-free (cls, reg) branches only (effidehead_fuseab.py:141-199, _distill_ns.py:105-150)
         fused = i in sibling
-        x, x_off, xs = view(op.src)
+        _, x, x_off, xs = view(op.src)
         k, s = (1, 1) if op.kind == "convT" else (op.k, op.s)
         cin = op.cin
         if op.kind != "convT":
@@ -137,7 +157,7 @@ def conv_launches(g, N, H, W, nsplit, sibling, addr, plan_fn):
         ws = (2 * op.cout if fused else op.cout, k, k, cin)
         kw = dict(x_c_off=x_off, bias=addr("bias_fused" if fused else "bias", i), stride=s, act=op.act, nsplit=nsplit)
         if op.res is not None:
-            r, r_off, (_, rh, rw, rct) = view(op.res)
+            _, r, r_off, (_, rh, rw, rct) = view(op.res)
             kw.update(res=r, res_c_off=r_off, res_strides=(rh * rw * rct, rw * rct, rct), alpha=addr("alpha", i))
         if op.kind == "pred":
             which, lvl = op.head
@@ -145,7 +165,7 @@ def conv_launches(g, N, H, W, nsplit, sibling, addr, plan_fn):
             out[i] = [ops.conv_desc(x, xs, addr("w", i), ws, addr("head", which), (A * ch, lw * ch, ch), y_elem_off=offs[lvl] * ch,
                                     y_f32=True, **kw)]
             continue
-        y, y_off, (_, dh, dw, dct) = view(op.dst)
+        _, y, y_off, (_, dh, dw, dct) = view(op.dst)
         if op.kind == "convT":           # scatter quadrant (dy, dx) of the 2x upsample
             out[i] = [ops.conv_desc(x, xs, addr("w", i, q), ws, y, (dh * dw * dct, 2 * dw * dct, 2 * dct), y_c_off=y_off,
                                     y_elem_off=(q // 2 * dw + q % 2) * dct, **kw) for q in range(4)]
@@ -155,6 +175,78 @@ def conv_launches(g, N, H, W, nsplit, sibling, addr, plan_fn):
             d = pair_view(d, addr("w_pair", i), plan_fn)
         out[i] = [d]
     return out
+
+
+def forward_launches(g, N, H, W, nsplit, addr, plan_fn, u8=False):
+    """Every launch of one inference forward of graph g over an [N, 3, H, W] input (uint8 if u8), in launch order, as InferLaunch
+    records: stem, the conv launches of conv_launches (the fused head siblings of siblings(g) included), SPPF pool, depthwise
+    conv, SE, channel shuffle, upsample (the head decode is not included).  Records only: no allocation and no CUDA call, so the
+    launches can be checked without a GPU.  The stem's input address is 0 (set per forward).
+
+    nsplit, addr and plan_fn as for conv_launches; addr also resolves ("w_dev" | "b_dev" | "w1" | "b1" | "w2" | "b2", op index):
+    the stem, depthwise and SE weights and biases."""
+    sibling = siblings(g)
+    convs = conv_launches(g, N, H, W, nsplit, sibling, addr, plan_fn)
+    view = _viewer(g, N, H, W, sibling, addr)
+
+    def span(t):
+        key, _, c0, _ = view(t)
+        return (key, c0, c0 + t.c)
+
+    def at(t):
+        """(address of the slice's first channel, channel pitch, plane stride) of graph tensor slice t."""
+        _, a, c0, (n, h, w, pitch) = view(t)
+        return a + 2 * c0, pitch, n * h * w * pitch if nsplit == 3 else 0
+
+    out = []
+    for i, op in enumerate(g.ops):
+        rec = dict(name=op.name)
+        if op.kind == "stem":
+            _, y, _, (_, h, w, pitch) = view(op.dst)
+            d = ops.stem_desc(0, N, H, W, u8, addr("w_dev", i), addr("b_dev", i), stem_channels(g, op), op.act, y, nsplit,
+                              N * h * w * pitch if nsplit == 3 else 0)
+            out.append(InferLaunch("stem", "yv6_stem_fwd", (C.byref(d),), d, writes=[span(op.dst)], **rec))
+        elif op.kind in ("pool", "dw", "se", "shuffle", "up"):
+            (x, xp, xpl), (_, _, _, (_, h, w, _)) = at(op.src), view(op.src)
+            if op.kind == "pool":      # in place: channels [0, C) -> [C, 4C) of one buffer
+                key, y, _, (_, h, w, ct) = view(op.dst)
+                out.append(InferLaunch("pool", "yv6_sppf_pool", (y, N, h, w, op.cin, ct, nsplit, N * h * w * ct if nsplit == 3 else 0),
+                                       reads=[(key, 0, op.cin)], writes=[(key, op.cin, 4 * op.cin)], **rec))
+            elif op.kind == "dw":
+                y, yp, ypl = at(op.dst)
+                d = ops.dw_desc(x, (N, h, w, xp), xpl, addr("w_dev", i), addr("b_dev", i), op.cin, op.k, op.s, op.act, y, yp, ypl, nsplit)
+                out.append(InferLaunch("dw", "yv6_dwconv_fwd", (C.byref(d),), d, reads=[span(op.src)], writes=[span(op.dst)], **rec))
+            elif op.kind == "se":      # in place
+                d = ops.se_desc(x, N, h * w, op.cin, op.cout, xp, xpl, *(addr(k, i) for k in ("w1", "b1", "w2", "b2")), nsplit=nsplit)
+                out.append(InferLaunch("se", "yv6_se_fwd", (C.byref(d),), d, reads=[span(op.src)], writes=[span(op.src)], **rec))
+            elif op.kind == "shuffle":
+                out.append(InferLaunch("shuffle", "yv6_channel_shuffle", (x, xp, xpl, *at(op.src2), N * h * w, op.cin, *at(op.dst), nsplit),
+                                       reads=[span(op.src), span(op.src2)], writes=[span(op.dst)], **rec))
+            else:
+                out.append(InferLaunch("up", "yv6_upsample2x", (x, xp, xpl, N, h, w, op.cin, *at(op.dst), nsplit),
+                                       reads=[span(op.src)], writes=[span(op.dst)], **rec))
+        elif i in convs:
+            rec["reads"] = [span(op.src)] + ([span(op.res)] if op.res is not None else [])
+            if op.kind == "pred":
+                rec.update(head=op.head[0], writes=[(("head",) + tuple(op.head), 0, 1)])
+            else:
+                rec["writes"] = [(("fused", i), 0, 2 * op.cout) if i in sibling else span(op.dst)]
+            _, _, _, (_, sh, sw, _) = view(op.src)
+            for q, d in enumerate(convs[i]):
+                k, s = d.kh, d.stride      # (of the 3x3 stride-2 conv, also on the column-pair view)
+                oh, ow = (sh + 2 * (k // 2) - k) // s + 1, (sw + 2 * (k // 2) - k) // s + 1
+                geom = dict(name=op.name if op.kind != "convT" else f"{op.name}[{q}]", cin=op.cin, cout=d.Cout, k=k, s=s, ho=oh, wo=ow,
+                            h=sh, w=sw, flops=2.0 * N * oh * ow * d.Cout * op.cin * k * k, y_f32=op.kind == "pred")
+                out.append(InferLaunch("conv", "yv6_conv_fwd", (C.byref(d),), d, conv=geom, **rec))
+    return out
+
+
+class _Plan:
+    """Buffers, launch records and stream schedule of one input shape.  bufs: the graph's activation buffers; fused: first conv
+    of a sibling pair -> the pair's [.., 2 x Cout] output; heads[k]: (cls [N,A,nc], reg [N,A,R]) fp32 of head set k (set 1 is
+    allocated on first use); pred [N,A,5+nc]: the decoded output; launches: forward_launches' records; decode: the head decode
+    launch; lane / waits / tails / events / fork: the stream schedule (InferEngine._schedule); neck_start: index of the first
+    launch after the backbone; image: the input of the last forward (kept alive while its kernels run)."""
 
 
 class InferEngine:
@@ -169,7 +261,6 @@ class InferEngine:
         self.nsplit = 3 if precision == "fp32" else 1
         self.handle = _lib.handle(device.index or 0)
         self.lib = _lib.lib()
-        self.fuse_siblings = True
         self.n_lanes = int(os.environ.get("YV6_LANES", "4"))   # streams the launches of one forward are spread over (1 = serial)
         self._side = None
         self.weights = {}     # op index -> dict(w=..., bias=..., alpha=...)
@@ -187,7 +278,7 @@ class InferEngine:
             w = w.float().to(dev)
             return ops.split3(w).contiguous() if self.nsplit == 3 else w.to(torch.bfloat16).contiguous()
 
-        self.sibling = siblings(self.g) if self.fuse_siblings else {}
+        self.sibling = siblings(self.g)
         for i, op in enumerate(self.g.ops):
             if op.kind in ("pool", "shuffle", "up") or (op.kind == "pred" and op.head[0] not in ("cls", "reg")):   # fuse_ab / distillation preds: training only
                 continue
@@ -235,122 +326,38 @@ class InferEngine:
         maxs = max(g.strides)
         if H % maxs or W % maxs:
             raise RuntimeError(f"input {H}x{W} must be a multiple of the largest stride {maxs}")
-        plan = {"bufs": [], "calls": [], "conv_info": [], "deps": [], "pred_descs": [], "head_set": 0}
-        for b in g.bufs:
-            h, w = H >> b.level, W >> b.level
-            shape = (P, N, h, w, b.c_total) if P == 3 else (N, h, w, b.c_total)
-            plan["bufs"].append(torch.zeros(shape, dtype=torch.bfloat16, device=dev))
+
+        def zeros(level, c):
+            shape = (N, H >> level, W >> level, c)
+            return torch.zeros((P,) + shape if P == 3 else shape, dtype=torch.bfloat16, device=dev)
+
+        plan = _Plan()
+        plan.bufs = [zeros(b.level, b.c_total) for b in g.bufs]
+        plan.fused = {i: zeros(g.bufs[g.ops[i].dst.buf].level, 2 * g.ops[i].cout) for i in self.sibling}
         sizes = [(H // s, W // s) for s in g.strides]
-        A = sum(h * w for h, w in sizes)
-        nc, R = g.num_classes, 4 * (g.reg_max + 1)
-        plan["cls"] = torch.empty(N, A, nc, dtype=torch.float32, device=dev)
-        plan["reg"] = torch.empty(N, A, R, dtype=torch.float32, device=dev)
-        plan["pred"] = torch.empty(N, A, 5 + nc, dtype=torch.float32, device=dev)
-        plan["sizes"], plan["A"] = sizes, A
-        plan["lvl_h"] = (C.c_int32 * len(sizes))(*[h for h, _ in sizes])
-        plan["lvl_w"] = (C.c_int32 * len(sizes))(*[w for _, w in sizes])
-        plan["lvl_s"] = (C.c_float * len(sizes))(*[float(s) for s in g.strides])
-        plan["image"] = None
-
-        slices = sibling_slices(g, self.sibling)
-        fused = {}          # first conv of a sibling pair -> the pair's [.., 2 x Cout] output
-        for i in self.sibling:
-            lvl = g.bufs[g.ops[i].dst.buf].level
-            shape = (N, H >> lvl, W >> lvl, 2 * g.ops[i].cout)
-            fused[i] = torch.zeros((P,) + shape if P == 3 else shape, dtype=torch.bfloat16, device=dev)
-        plan["fused_bufs"] = list(fused.values())
-
-        def view(t):
-            """(tensor, first channel) of a graph tensor slice."""
-            if t.buf in slices:
-                i, c0, _ = slices[t.buf]
-                return fused[i], c0 + t.c_off
-            return plan["bufs"][t.buf], t.c_off
-
-        def span(t):
-            """(tensor identity, first channel, end channel) of a graph tensor slice: the unit of the dependency analysis."""
-            buf, c0 = view(t)
-            return (id(buf), c0, c0 + t.c)
+        A, nc, R = sum(h * w for h, w in sizes), g.num_classes, 4 * (g.reg_max + 1)
+        plan.heads = [(torch.empty(N, A, nc, dtype=torch.float32, device=dev), torch.empty(N, A, R, dtype=torch.float32, device=dev))]
+        plan.pred = torch.empty(N, A, 5 + nc, dtype=torch.float32, device=dev)
+        plan.sizes, plan.head_set, plan.image = sizes, 0, None
 
         def addr(kind, key, q=0):
-            """Device addresses of this plan's tensors and the packed weights (see conv_launches)."""
-            if kind == "buf":
-                return plan["bufs"][key].data_ptr()
-            if kind == "fused":
-                return fused[key].data_ptr()
+            """Device addresses of this plan's tensors and the packed weights (see forward_launches)."""
+            if kind in ("buf", "fused"):
+                return (plan.bufs if kind == "buf" else plan.fused)[key].data_ptr()
             if kind == "head":
-                return plan[key].data_ptr()
+                return plan.heads[0][("cls", "reg").index(key)].data_ptr()
             if kind == "alpha":
                 return self.weights[key]["alpha"]
             t = self.weights[key][kind]
             return (t[q] if kind == "w" else t).data_ptr()
 
-        launches = conv_launches(g, N, H, W, P, self.sibling, addr, lambda d: ops.plan_of(d, dev.index or 0))
-
-        def slice_args(t):
-            """(address of the slice's first channel, channel pitch, plane stride) of a graph tensor slice."""
-            buf, c0 = view(t)
-            return buf.data_ptr() + 2 * c0, buf.shape[-1], buf.stride(0) if P == 3 else 0
-
-        plan["call_names"] = []
-        for i, op in enumerate(g.ops):
-            lvl = g.bufs[op.src.buf].level if op.src is not None else 0
-            if op.kind == "stem":
-                buf, _ = view(op.dst)
-                ent = self.weights[i]
-                d = ops.stem_desc(0, N, H, W, in_dtype == torch.uint8, ent["w_dev"].data_ptr(), ent["b_dev"].data_ptr(), stem_channels(g, op),
-                                  op.act, buf.data_ptr(), P, buf.stride(0) if P == 3 else 0)
-                plan["stem"] = d
-                plan["calls"].append(("stem", d))
-                plan["deps"].append(dict(reads=[], writes=[span(op.dst)]))
-            elif op.kind == "pool":
-                buf, _ = view(op.dst)
-                h, w, ct = buf.shape[-3:]
-                plan["calls"].append(("pool", (buf.data_ptr(), N, h, w, op.cin, ct, P, buf.stride(0) if P == 3 else 0)))
-                plan["deps"].append(dict(reads=[(id(buf), 0, op.cin)], writes=[(id(buf), op.cin, 4 * op.cin)]))
-            elif op.kind == "dw":
-                ent = self.weights[i]
-                (x, xp, xpl), (y, yp, ypl) = slice_args(op.src), slice_args(op.dst)
-                d = ops.dw_desc(x, (N, H >> lvl, W >> lvl, xp), xpl, ent["w_dev"].data_ptr(), ent["b_dev"].data_ptr(), op.cin, op.k, op.s,
-                                op.act, y, yp, ypl, P)
-                plan["calls"].append(("dw", d))
-                plan["deps"].append(dict(reads=[span(op.src)], writes=[span(op.dst)]))
-            elif op.kind == "se":
-                ent = self.weights[i]
-                x, xp, xpl = slice_args(op.src)
-                d = ops.se_desc(x, N, (H >> lvl) * (W >> lvl), op.cin, op.cout, xp, xpl, *(ent[k].data_ptr() for k in ("w1", "b1", "w2", "b2")),
-                                nsplit=P)
-                plan["calls"].append(("se", d))
-                plan["deps"].append(dict(reads=[span(op.src)], writes=[span(op.src)]))
-            elif op.kind == "shuffle":
-                (a, ap, apl), (b, bp, bpl), (y, yp, ypl) = slice_args(op.src), slice_args(op.src2), slice_args(op.dst)
-                plan["calls"].append(("shuffle", (a, ap, apl, b, bp, bpl, N * (H >> lvl) * (W >> lvl), op.cin, y, yp, ypl, P)))
-                plan["deps"].append(dict(reads=[span(op.src), span(op.src2)], writes=[span(op.dst)]))
-            elif op.kind == "up":
-                (x, xp, xpl), (y, yp, ypl) = slice_args(op.src), slice_args(op.dst)
-                plan["calls"].append(("up", (x, xp, xpl, N, H >> lvl, W >> lvl, op.cin, y, yp, ypl, P)))
-                plan["deps"].append(dict(reads=[span(op.src)], writes=[span(op.dst)]))
-            plan["call_names"] += [op.name] * (len(plan["calls"]) - len(plan["call_names"]))
-            for q, d in enumerate(launches.get(i, ())):
-                lvl = g.bufs[op.src.buf].level
-                sh, sw, k, s = H >> lvl, W >> lvl, d.kh, d.stride      # (of the 3x3 stride-2 conv, also on the column-pair view)
-                oh, ow = (sh + 2 * (k // 2) - k) // s + 1, (sw + 2 * (k // 2) - k) // s + 1
-                plan["conv_info"].append(dict(name=op.name if op.kind != "convT" else f"{op.name}[{q}]", cin=op.cin, cout=d.Cout,
-                                              k=k, s=s, ho=oh, wo=ow, h=sh, w=sw, flops=2.0 * N * oh * ow * d.Cout * op.cin * k * k,
-                                              y_f32=op.kind == "pred"))
-                reads = [span(op.src)] + ([span(op.res)] if op.res is not None else [])
-                if op.kind == "pred":
-                    plan["pred_descs"].append((d, op.head[0], d.y - plan[op.head[0]].data_ptr()))
-                    writes = [(("head",) + tuple(op.head), 0, 1)]
-                elif i in fused:
-                    writes = [(id(fused[i]), 0, 2 * op.cout)]
-                else:
-                    writes = [span(op.dst)]
-                if "neck_start" not in plan and op.name.startswith("neck."):
-                    plan["neck_start"] = len(plan["calls"])     # first launch after the backbone (pipeline.DetectStream forks here)
-                plan["calls"].append(("conv", d))
-                plan["deps"].append(dict(reads=reads, writes=writes))
-                plan["call_names"].append(op.name)
+        plan.launches = forward_launches(g, N, H, W, P, addr, lambda d: ops.plan_of(d, dev.index or 0), in_dtype == torch.uint8)
+        plan.stem = next(r.desc for r in plan.launches if r.kind == "stem")
+        plan.neck_start = next((j for j, r in enumerate(plan.launches) if r.kind == "conv" and r.name.startswith("neck.")), 0)
+        lvl = [(C.c_int32 * len(sizes))(*[h for h, _ in sizes]), (C.c_int32 * len(sizes))(*[w for _, w in sizes]),
+               (C.c_float * len(sizes))(*[float(s) for s in g.strides])]
+        plan.decode = ops.Launch("decode", "yv6_head_decode", (*(t.data_ptr() for t in plan.heads[0] + (plan.pred,)), N, nc, R,
+                                                               len(sizes), *lvl))
         self._schedule(plan)
         self._plans[key] = plan
         return plan
@@ -363,14 +370,13 @@ class InferEngine:
         their launch-to-first-MMA latency and drain overlap instead of adding up.  Inside a captured CUDA graph the events
         become plain graph edges."""
         K = self.n_lanes
-        deps = plan["deps"]
-        n = len(deps)
+        n = len(plan.launches)
         writers = {}
         lane, waits = [0] * n, [[] for _ in range(n)]
         last_on = [-1] * K
-        for i, dp in enumerate(deps):
+        for i, r in enumerate(plan.launches):
             prod = set()
-            for key, lo, hi in dp["reads"]:
+            for key, lo, hi in r.reads:
                 for wlo, whi, j in writers.get(key, ()):
                     if wlo < hi and lo < whi:
                         prod.add(j)
@@ -384,36 +390,51 @@ class InferEngine:
             lane[i] = s
             waits[i] = sorted(j for j in prod if lane[j] != s)
             last_on[s] = i
-            for key, lo, hi in dp["writes"]:
+            for key, lo, hi in r.writes:
                 writers.setdefault(key, []).append((lo, hi, i))
         need = set(j for w in waits for j in w)
         tails = [last_on[t] for t in range(1, K) if last_on[t] >= 0]
         need.update(tails)
-        plan["lane"], plan["waits"], plan["tails"] = lane, waits, tails
-        plan["events"] = {j: torch.cuda.Event() for j in need}
-        plan["fork"] = torch.cuda.Event()
+        plan.lane, plan.waits, plan.tails = lane, waits, tails
+        plan.events = {j: torch.cuda.Event() for j in need}
+        plan.fork = torch.cuda.Event()
 
     def pin(self, N, H, W, in_dtype=torch.float32):
         """Keep the buffers of this shape for the engine's lifetime (they are referenced by a captured CUDA graph)."""
         self._plan(N, H, W, in_dtype)
         self._pinned.add((N, H, W, in_dtype))
 
+    def launches(self, N, H, W, in_dtype=torch.float32):
+        """The launch records (InferLaunch) of one forward of this shape, in launch order; the head decode is not among them."""
+        return self._plan(N, H, W, in_dtype).launches
+
+    def neck_start(self, N, H, W, in_dtype=torch.float32):
+        """Index of the first launch after the backbone (the serving pipeline forks its NMS branch there)."""
+        return self._plan(N, H, W, in_dtype).neck_start
+
     # ------------------------------------------------------------------ execution
     def launch_count(self, N, H, W, in_dtype=torch.float32):
         """Kernels launched per forward for this shape (convs + stem + pools + decode)."""
-        return len(self._plan(N, H, W, in_dtype)["calls"]) + 1
+        return len(self.launches(N, H, W, in_dtype)) + 1
+
+    def _heads(self, plan, k):
+        """(cls, reg) of head set k of a plan, allocating set 1 on first use."""
+        if k == 1 and len(plan.heads) == 1:
+            plan.heads.append(tuple(torch.empty_like(t) for t in plan.heads[0]))
+        return plan.heads[k]
 
     def _select_head_set(self, plan, k):
         """Point the pred convs at head-output set k (0 = the default tensors; 1 = a second pair, allocated on first use).
         The software-pipelined serving loop (pipeline.DetectStream) alternates between the two so that the NMS of batch
         i - 1 can read one set while the network of batch i writes the other."""
-        if k == plan["head_set"]:
+        if k == plan.head_set:
             return
-        if k == 1 and "cls_alt" not in plan:
-            plan["cls_alt"], plan["reg_alt"] = torch.empty_like(plan["cls"]), torch.empty_like(plan["reg"])
-        for d, which, off in plan["pred_descs"]:
-            d.y = plan[which + ("_alt" if k == 1 else "")].data_ptr() + off
-        plan["head_set"] = k
+        old, new = self._heads(plan, plan.head_set), self._heads(plan, k)
+        for r in plan.launches:
+            if r.head is not None:
+                j = ("cls", "reg").index(r.head)
+                r.desc.y += new[j].data_ptr() - old[j].data_ptr()
+        plan.head_set = k
 
     def forward(self, x, stream=None, decode=True, head_set=0, hook=None):
         """x: [N,3,H,W] CUDA tensor, fp32 in [0,1] or uint8.  Returns pred [N,A,5+nc] fp32 (a buffer owned
@@ -429,168 +450,124 @@ class InferEngine:
         N, Cin, H, W = x.shape
         assert Cin == 3
         plan = self._plan(N, H, W, x.dtype)
-        plan["image"] = x  # keep alive while kernels are in flight
+        plan.image = x  # keep alive while kernels are in flight
         assert head_set == 0 or not decode, "the alternate head set is for decode=False callers"
         self._select_head_set(plan, head_set)
         main = stream if stream is not None else torch.cuda.current_stream(self.device)
         sp = _lib.stream_ptr(main)
-        lib, h, chk = self.lib, self.handle, _lib.check
-        plan["stem"].x = x.data_ptr()
-        lane, waits, events = plan["lane"], plan["waits"], plan["events"]
+        lib, h = self.lib, self.handle
+        plan.stem.x = x.data_ptr()
+        lane, waits, events = plan.lane, plan.waits, plan.events
         multi = self.n_lanes > 1 and max(lane) > 0
         if multi:
             if self._side is None:
                 self._side = [torch.cuda.Stream(device=self.device) for _ in range(self.n_lanes - 1)]
             streams = [main] + self._side
             sps = [_lib.stream_ptr(t) for t in streams]
-            plan["fork"].record(main)
+            plan.fork.record(main)
             forked = set()
-        for i, (kind, d) in enumerate(plan["calls"]):
+        for i, r in enumerate(plan.launches):
             if hook is not None and i == hook[0]:
                 hook[1]()
             if multi:
                 t = lane[i]
                 if t and t not in forked:        # a side stream starts after everything the caller queued before this forward
-                    streams[t].wait_event(plan["fork"])
+                    streams[t].wait_event(plan.fork)
                     forked.add(t)
                 for j in waits[i]:
                     streams[t].wait_event(events[j])
                 sp = sps[t]
-            self._launch(kind, d, sp)
+            r.run(lib, h, sp)
             if multi and i in events:
                 events[i].record(streams[lane[i]])
         if multi:                                  # join: the caller's stream continues after every lane
-            for j in plan["tails"]:
+            for j in plan.tails:
                 main.wait_event(events[j])
             sp = sps[0]
-        g = self.g
         if not decode:
-            if head_set == 1:
-                return plan["cls_alt"], plan["reg_alt"], plan["sizes"]
-            return plan["cls"], plan["reg"], plan["sizes"]
-        chk(lib.yv6_head_decode(h, C.c_void_p(plan["cls"].data_ptr()), C.c_void_p(plan["reg"].data_ptr()),
-                                C.c_void_p(plan["pred"].data_ptr()), N, g.num_classes, 4 * (g.reg_max + 1),
-                                len(g.strides), plan["lvl_h"], plan["lvl_w"], plan["lvl_s"], sp))
-        return plan["pred"]
+            return (*plan.heads[head_set], plan.sizes)
+        plan.decode.run(lib, h, sp)
+        return plan.pred
 
-    def _launch(self, kind, d, sp):
-        lib, h, chk = self.lib, self.handle, _lib.check
-        if kind == "conv":
-            chk(lib.yv6_conv_fwd(h, C.byref(d), sp))
-        elif kind == "stem":
-            chk(lib.yv6_stem_fwd(h, C.byref(d), sp))
-        elif kind == "pool":
-            chk(lib.yv6_sppf_pool(h, C.c_void_p(d[0]), d[1], d[2], d[3], d[4], d[5], d[6], d[7], sp))
-        elif kind == "dw":
-            chk(lib.yv6_dwconv_fwd(h, C.byref(d), sp))
-        elif kind == "se":
-            chk(lib.yv6_se_fwd(h, C.byref(d), sp))
-        elif kind == "shuffle":
-            chk(lib.yv6_channel_shuffle(h, *d, sp))
-        elif kind == "up":
-            chk(lib.yv6_upsample2x(h, *d, sp))
-        else:
-            raise RuntimeError(f"no kernel for launch kind {kind!r}")
-
-    def profile_calls(self, x, steps=20, stream=None):
-        """Device time of every launch of one forward, each launched alone between CUDA events (serial, one stream):
-        [(kind, op name, ms)], the median over `steps` runs."""
-        x = x.contiguous()
-        N, _, H, W = x.shape
-        plan = self._plan(N, H, W, x.dtype if x.dtype == torch.uint8 else torch.float32)
-        self.forward(x, stream)
-        torch.cuda.synchronize()
-        sp = _lib.stream_ptr(stream)
-        rows = []
-        for (kind, d), name in zip(plan["calls"], plan["call_names"]):
-            ts = []
-            for _ in range(steps):
-                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                e0.record()
-                self._launch(kind, d, sp)
-                e1.record()
-                torch.cuda.synchronize()
-                ts.append(e0.elapsed_time(e1))
-            rows.append((kind, name, sorted(ts)[len(ts) // 2]))
-        return rows
-
-    def head_outputs(self, N, H, W, in_dtype=torch.float32):
-        """(cls [N,A,nc] post-sigmoid, reg [N,A,R] raw) of the last forward with this shape."""
-        plan = self._plan(N, H, W, in_dtype)
-        return plan["cls"], plan["reg"]
+    def head_outputs(self, N, H, W, in_dtype=torch.float32, head_set=0):
+        """(cls [N,A,nc] post-sigmoid, reg [N,A,R] raw) of head set `head_set` (see forward) of the last forward with this shape."""
+        return self._heads(self._plan(N, H, W, in_dtype), head_set)
 
     def feature_maps(self, N, H, W, in_dtype=torch.float32):
         """Neck outputs as NCHW views (reference `featmaps`, yolo.py:37-39); bf16 (hi plane in fp32 mode)."""
         plan = self._plan(N, H, W, in_dtype)
         out = []
         for t in self.g.feat:
-            buf = plan["bufs"][t.buf]
+            buf = plan.bufs[t.buf]
             buf = buf[0] if self.nsplit == 3 else buf
             out.append(buf[..., t.c_off:t.c_off + t.c].permute(0, 3, 1, 2))
         return out
 
+    # ------------------------------------------------------------------ profiling
+    def _profiled(self, x, stream):
+        """(launch records, stream pointer) of x's shape after one forward of x, synchronized."""
+        x = x.contiguous()
+        N, _, H, W = x.shape
+        launches = self.launches(N, H, W, x.dtype if x.dtype == torch.uint8 else torch.float32)
+        self.forward(x, stream)
+        torch.cuda.synchronize()
+        return launches, _lib.stream_ptr(stream)
+
+    def _timed(self, launches, sp, steps, before=None):
+        """Device times (ms) of `steps` runs of the launches back to back between one pair of CUDA events, each run
+        synchronized; before() runs ahead of each."""
+        ts = []
+        for _ in range(steps):
+            if before is not None:
+                before()
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            for r in launches:
+                r.run(self.lib, self.handle, sp)
+            e1.record()
+            torch.cuda.synchronize()
+            ts.append(e0.elapsed_time(e1))
+        return ts
+
+    def profile_calls(self, x, steps=20, stream=None):
+        """Device time of every launch of one forward, each launched alone between CUDA events (serial, one stream):
+        [(kind, op name, ms)], the median over `steps` runs."""
+        launches, sp = self._profiled(x, stream)
+        return [(r.kind, r.name, sorted(self._timed([r], sp, steps))[steps // 2]) for r in launches]
+
     def profile_convs(self, x, steps=5, stream=None):
         """Roofline instrumentation for bench.py: CUDA events around every conv_igemm launch.
         Returns (conv-kernel ms per forward, algorithmic conv FLOPs per forward, launches per forward)."""
-        x = x.contiguous()
-        N, _, H, W = x.shape
-        plan = self._plan(N, H, W, x.dtype if x.dtype == torch.uint8 else torch.float32)
-        self.forward(x, stream)
-        torch.cuda.synchronize()
-        sp = _lib.stream_ptr(stream)
-        convs = [d for kind, d in plan["calls"] if kind == "conv"]
-        flops = sum(ci["flops"] for ci in plan["conv_info"])     # algorithmic (the column-pair view's zero taps do not count)
+        launches, sp = self._profiled(x, stream)
+        convs = [r for r in launches if r.kind == "conv"]
         # one event pair around the back-to-back conv launches of a forward (launch gaps between the
         # kernels are part of the step, so they stay in the denominator)
-        total_ms = 0.0
-        for _ in range(steps):
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
-            for d in convs:
-                _lib.check(self.lib.yv6_conv_fwd(self.handle, C.byref(d), sp))
-            e1.record()
-            torch.cuda.synchronize()
-            total_ms += e0.elapsed_time(e1)
-        return total_ms / steps, flops, len(convs)
+        return sum(self._timed(convs, sp, steps)) / steps, sum(r.conv["flops"] for r in convs), len(convs)
 
     def conv_bytes_per_launch(self, N, H, W):
         """Algorithmic HBM bytes of an average conv launch: each conv reads its input slice and writes its output
         slice once (bf16), weights once."""
-        plan = self._plan(N, H, W, torch.float32)
         tot, n = 0.0, 0
-        for ci in plan["conv_info"]:
-            ysz = 4 if ci["y_f32"] else 2
-            tot += N * (ci["h"] * ci["w"] * ci["cin"] * 2 + ci["ho"] * ci["wo"] * ci["cout"] * ysz) + ci["cout"] * ci["k"] ** 2 * ci["cin"] * 2
-            n += 1
+        for r in self.launches(N, H, W):
+            if r.kind == "conv":
+                ci = r.conv
+                ysz = 4 if ci["y_f32"] else 2
+                tot += N * (ci["h"] * ci["w"] * ci["cin"] * 2 + ci["ho"] * ci["wo"] * ci["cout"] * ysz) + ci["cout"] * ci["k"] ** 2 * ci["cin"] * 2
+                n += 1
         return tot / max(n, 1)
 
     def profile_layers(self, x, iters=10, stream=None):
         """Per-launch timing table (name, shape, ms, TFLOP/s) with an L2 flush before every launch."""
-        x = x.contiguous()
-        N, _, H, W = x.shape
-        plan = self._plan(N, H, W, x.dtype if x.dtype == torch.uint8 else torch.float32)
-        self.forward(x, stream)
-        torch.cuda.synchronize()
-        sp = _lib.stream_ptr(stream)
+        launches, sp = self._profiled(x, stream)
         flush = torch.empty(256 << 20, dtype=torch.uint8, device=self.device)
         rows = []
-        convs = [d for kind, d in plan["calls"] if kind == "conv"]
-        for ci, d in zip(plan["conv_info"], convs):
-            name = ci["name"]
-            ts = []
-            for _ in range(iters):
-                flush.zero_()
-                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                e0.record()
-                _lib.check(self.lib.yv6_conv_fwd(self.handle, C.byref(d), sp))
-                e1.record()
-                torch.cuda.synchronize()
-                ts.append(e0.elapsed_time(e1))
-            ts.sort()
-            ms = ts[len(ts) // 2]
+        for r in launches:
+            if r.kind != "conv":
+                continue
+            ci, d = r.conv, r.desc
+            ms = sorted(self._timed([r], sp, iters, flush.zero_))[iters // 2]
             ho, wo = ci["ho"], ci["wo"]
-            fl = ci["flops"]
             by = 2.0 * d.N * (ci["h"] * ci["w"] * ci["cin"] + ho * wo * ci["cout"])
-            rows.append(dict(name=name, cin=ci["cin"], cout=ci["cout"], k=ci["k"], s=ci["s"], hw=f"{ho}x{wo}", ms=ms,
-                             tflops=fl / ms / 1e9, gbs=by / ms / 1e6, plan=ops.plan_of(d, self.device.index or 0)))
+            rows.append(dict(name=ci["name"], cin=ci["cin"], cout=ci["cout"], k=ci["k"], s=ci["s"], hw=f"{ho}x{wo}", ms=ms,
+                             tflops=ci["flops"] / ms / 1e9, gbs=by / ms / 1e6, plan=ops.plan_of(d, self.device.index or 0)))
         return rows

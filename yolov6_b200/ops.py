@@ -3,6 +3,7 @@ GPU needed), and launch functions over torch CUDA tensors used purely as device 
 channel slices, bf16x3 planes) are made by the caller (`yolov6_b200.engine`).
 """
 import ctypes as C
+from dataclasses import dataclass
 
 import torch
 
@@ -11,6 +12,22 @@ from ._lib import ACT_CODES, DT_BF16, DT_F32, DT_U8, ConvDesc, DwDesc, SeDesc, S
 
 # Names of the yv6_conv_plan (10) / yv6_conv_plan_host (12) output words.  a_res = A stages * 100 + CTA pair * 10 + B resident.
 PLAN_KEYS = ("BW", "BH", "BI", "BN", "KB", "stages", "grid", "tiles", "halo", "a_res", "smem", "threads")
+
+
+@dataclass(eq=False)
+class Launch:
+    """One kernel launch of an engine: library entry point `fn` (a name) called as fn(handle, *args, stream), or a callable
+    fn(stream).  Descriptor launches pass `desc` by reference."""
+    kind: str
+    fn: object
+    args: tuple = ()
+    desc: object = None
+
+    def run(self, lib, h, sp):
+        if isinstance(self.fn, str):
+            _lib.check(getattr(lib, self.fn)(h, *self.args, sp))
+        else:
+            self.fn(sp)
 
 
 def _ptr(t):

@@ -228,7 +228,9 @@ class DetectStream:
         self._drained = False
         self.eng = engine if engine is not None else model.engine()
         self.eng.pin(batch, height, width, dt)
-        A = sum((height // int(s)) * (width // int(s)) for s in model.graph.strides)
+        self.shape = (batch, height, width, dt)
+        self.sizes = [(height // int(s), width // int(s)) for s in model.graph.strides]
+        A = sum(h * w for h, w in self.sizes)
         self.nms_ws = torch.empty(workspace_bytes(batch, A, model.graph.num_classes, multi_label), dtype=torch.uint8, device=self.dev)
         self.side = torch.cuda.Stream(device=self.dev)
         self.copy_stream = torch.cuda.Stream(device=self.dev)
@@ -243,10 +245,8 @@ class DetectStream:
 
     def _nms(self, k, store):
         """NMS over head set k -> result slot k (pinned host when host_input; the device tensors go to `store[k]`)."""
-        plan = self.eng._plan(self.B, self.x_dev[0].shape[2], self.x_dev[0].shape[3], self.x_dev[0].dtype)
-        cls = plan["cls_alt"] if k == 1 else plan["cls"]
-        reg = plan["reg_alt"] if k == 1 else plan["reg"]
-        out, count, src, overflow = nms_batched_head(cls, reg, plan["sizes"], self.model.graph.strides, workspace=self.nms_ws, **self.kw)
+        cls, reg = self.eng.head_outputs(*self.shape, head_set=k)
+        out, count, src, overflow = nms_batched_head(cls, reg, self.sizes, self.model.graph.strides, workspace=self.nms_ws, **self.kw)
         if self.raw:
             # res_geo[k] is the geometry of the batch whose network wrote head set k: the copy stream may already be refilling
             # geo_dev[k] with the batch after next
@@ -270,8 +270,7 @@ class DetectStream:
         # The branch starts where the backbone ends: the neck / head launches are single waves of <= 128 CTAs that leave SMs
         # idle, whereas next to the backbone's persistent one-CTA-per-SM kernels the one-CTA-per-image NMS kernels just take SMs away
         # (forking at the start of the step gains 2 %, measured).
-        plan = self.eng._plan(self.B, self.x_dev[0].shape[2], self.x_dev[0].shape[3], self.x_dev[0].dtype)
-        at = plan.get("neck_start", 0) if self.fork_at_neck else 0
+        at = self.eng.neck_start(*self.shape) if self.fork_at_neck else 0
         self._letterbox(k)
         self.eng.forward(self.x_dev[k], decode=False, head_set=k, hook=(at, fork))
         cur.wait_event(self.ev_join)

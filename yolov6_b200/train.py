@@ -149,28 +149,17 @@ class Write:
 
 
 @dataclass(eq=False)
-class Launch:
-    """One launch of the training step: library entry point `fn` (a name) called as fn(handle, *args, stream), or a callable
-    fn(stream).  Descriptor launches pass `desc` by reference.  `side`: a weight gradient, run on the side stream next to the
-    main stream; `parity`: the dc scratch pair it reads (side) or refills (main stream, ALL: everything the side stream may
-    read).  `snapshot` = (op index, incoming gradient slice) is copied into engine.dbg before the launch when engine.debug;
+class Launch(ops.Launch):
+    """One launch of the training step (ops.Launch).  `side`: a weight gradient, run on the side stream next to the main
+    stream; `parity`: the dc scratch pair it reads (side) or refills (main stream, ALL: everything the side stream may read).
+    `snapshot` = (op index, incoming gradient slice) is copied into engine.dbg before the launch when engine.debug;
     `bucket` = k marks the unpack of gradient bucket k."""
-    kind: str
-    fn: object
-    args: tuple = ()
-    desc: object = None
     kernels: int = 1
     side: bool = False
     parity: int = None
     writes: tuple = ()
     snapshot: tuple = None
     bucket: int = None
-
-    def run(self, lib, h, sp):
-        if isinstance(self.fn, str):
-            _lib.check(getattr(lib, self.fn)(h, *self.args, sp))
-        else:
-            self.fn(sp)
 
 
 def _desc_launch(kind, fn, d, **kw):
