@@ -945,12 +945,16 @@ static int plan_conv(const yv6_handle* h, const yv6_conv_desc* d, ConvPlan* plan
   k.bias = d->bias;
 
   // Output through a tensor map (C, W, H, N) with boxes of (box_bytes / element size) channels x the BW x BH x BI tile:
-  // needs one output plane, no residual, a 16-byte aligned base and strides, and in fp32 (where one staging half holds 64
-  // rows) a 128-row tile split into two 64-row boxes along H.
+  // needs one output plane, no residual, a 16-byte aligned base and strides, a pixel's Cout outputs ending on a 16-byte
+  // boundary, and in fp32 (where one staging half holds 64 rows) a 128-row tile split into two 64-row boxes along H.
+  // Measured on an H100 SXM, tests/test_gpu_forward_launches.py: with the map's dims[0] = Cout = 12, the bf16 1x1 conv
+  // backbone.lite_effiblock_2.0.conv_pw_2 of YOLOv6Lite-S (2 x 128 x 128, output [2, 32, 32, 16], slice [0, 12)) also
+  // stored channels 12..15 (zeros) of all 8192 of its pixels x 4, and the same conv of YOLOv6Lite-L at 192 x 320 all
+  // 122880: the store did not clip at the end of the 24-byte channel row.  Those outputs take the chunk epilogue.
   {
     const int esz = d->y_dtype == YV6_DT_F32 ? 4 : 2;
     const int64_t strides[3] = {d->y_w_stride * esz, d->y_h_stride * esz, d->y_img_stride * esz};
-    bool ok = k.out_planes == 1 && d->res == nullptr && (reinterpret_cast<uintptr_t>(d->y) & 15) == 0;
+    bool ok = k.out_planes == 1 && d->res == nullptr && (reinterpret_cast<uintptr_t>(d->y) & 15) == 0 && (d->Cout * esz) % 16 == 0;
     for (int64_t s : strides) ok = ok && s > 0 && s % 16 == 0 && s < (1ll << 40);
     if (esz == 4) ok = ok && k.BI == 1 && k.BH % 2 == 0 && k.BW * k.BH == kTileRows;
     k.tma_store = ok ? 1 : 0;

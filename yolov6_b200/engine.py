@@ -103,7 +103,12 @@ class InferLaunch(ops.Launch):
     (buffer, first channel, end channel) spans it `reads` and `writes` -- buffers are ("buf", graph buffer index), ("fused",
     first conv of a sibling pair) or ("head", "cls" | "reg", level) --, `head` "cls" | "reg" for a head conv (its output moves
     with the head set), and for a conv launch `conv`: its geometry (cin, cout, k, s, input h, w, output ho, wo), algorithmic
-    `flops` (the column-pair view's zero taps do not count) and `y_f32`."""
+    `flops` (the column-pair view's zero taps do not count) and `y_f32`.
+
+    `writes` covers every element the launch stores.  `reads` covers every element whose value reaches the output; a conv of
+    a Lite graph also loads the rest of its 16-aligned channel window (conv_window), through weights that are zero in every
+    plane, and those channels are not declared: any finite value there contributes exactly 0, so the schedule need not order
+    the launch after their writers."""
     name: str = ""
     reads: tuple = ()
     writes: tuple = ()
@@ -201,11 +206,12 @@ def forward_launches(g, N, H, W, nsplit, addr, plan_fn, u8=False):
     out = []
     for i, op in enumerate(g.ops):
         rec = dict(name=op.name)
-        if op.kind == "stem":
-            _, y, _, (_, h, w, pitch) = view(op.dst)
+        if op.kind == "stem":         # writes its buffer's whole pitch (the Lite stem's zero pad channels included)
+            key, y, c0, (_, h, w, pitch) = view(op.dst)
+            assert c0 == 0
             d = ops.stem_desc(0, N, H, W, u8, addr("w_dev", i), addr("b_dev", i), stem_channels(g, op), op.act, y, nsplit,
                               N * h * w * pitch if nsplit == 3 else 0)
-            out.append(InferLaunch("stem", "yv6_stem_fwd", (C.byref(d),), d, writes=[span(op.dst)], **rec))
+            out.append(InferLaunch("stem", "yv6_stem_fwd", (C.byref(d),), d, writes=[(key, 0, stem_channels(g, op))], **rec))
         elif op.kind in ("pool", "dw", "se", "shuffle", "up"):
             (x, xp, xpl), (_, _, _, (_, h, w, _)) = at(op.src), view(op.src)
             if op.kind == "pool":      # in place: channels [0, C) -> [C, 4C) of one buffer
