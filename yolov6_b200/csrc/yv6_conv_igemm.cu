@@ -29,6 +29,7 @@
 //     pairs, giving fp32-equivalent products with fp32 accumulation.
 //   * halo variants (MODE 1 / 2: 3x3 stride 1; MODE 3 / 4: 3x3 stride 2 on the column-pair view of the input): ONE input box
 //     per channel block feeds every tap through shifted wgmma descriptors; weights streamed through their own ring or resident.
+//     At BN = 64 the tile is computed transposed, 64 channels x 128 pixels (mma_kblock_t): one m64n128k16 per k16 step.
 //   * CTA-pair variants (CP = true): clusters of two CTAs on adjacent M tiles; each loads half of the weight tile with a TMA
 //     multicast into both CTAs.
 #include <algorithm>
@@ -344,6 +345,64 @@ __device__ __forceinline__ void stage_out_tile(const ConvKParams& p, float (&acc
   }
 }
 
+// stmatrix .trans: the four 8 x 8 b16 blocks whose mma fragments are r0..r3, each stored transposed -- lane 8 k + i gives the
+// address of row i of block k, which receives column i of the fragment block (16 bytes)
+__device__ __forceinline__ void stmatrix_x4_trans(uint32_t addr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.trans.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r0), "r"(r1), "r"(r2),
+               "r"(r3)
+               : "memory");
+}
+
+// TMA-store epilogue of a transposed BN = 64 halo tile (see mma_kblock_t): bias + activation on one accumulator half, which
+// holds channels r0 + 8 i and pixels 8 j + c0, + 1 (j < 8) of a 64-pixel half, rounded to the output dtype and written
+// pixel-major into the same boxes as stage_out_tile, from pixel row px0 of the staging half on.  bf16: the four 8 x 8
+// (channel x pixel) blocks of j = 2 jj, 2 jj + 1 go out in one stmatrix .trans, each as eight 16-byte units (one pixel's 8
+// channels, one swizzled unit per 128-byte row): conflict-free, where 2-byte stores would hit one bank for every pixel.
+template <bool F32>
+__device__ __forceinline__ void stage_out_tile_t(const ConvKParams& p, float (&acc)[32], const float* sbias, uint8_t* stage, int px0,
+                                                 int r0, int c0, int lane) {
+  float b[2] = {0.f, 0.f};
+  if (p.bias != nullptr) {
+    b[0] = sbias[r0];
+    b[1] = sbias[r0 + 8];
+  }
+  if constexpr (F32) {
+    constexpr int kBox = y_box_bytes(64, 4), kCols = kBox / 4, kGroupBytes = 64 * kBox;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      float v[4] = {acc[4 * j], acc[4 * j + 1], acc[4 * j + 2], acc[4 * j + 3]};   // (channel r0 + 8 (m / 2), pixel + m % 2)
+      if (p.bias != nullptr) {
+#pragma unroll
+        for (int m = 0; m < 4; ++m) v[m] += b[m / 2];
+      }
+      activate(p, v);
+#pragma unroll
+      for (int m = 0; m < 4; ++m) {
+        const int q = px0 + 8 * j + c0 + (m & 1), n = r0 + 8 * (m >> 1);
+        *reinterpret_cast<float*>(stage + (n / kCols) * kGroupBytes + q * kBox + (((n % kCols) * 4) ^ ((q & 7) << 4))) = v[m];
+      }
+    }
+  } else {
+    // lane 8 k + i: row i (pixel 8 j + i) of block k = (j = 2 jj + k / 2, channels 8 (2 w + k % 2) ..., w = r0 / 16); the box
+    // rows are 128 bytes and 8-row aligned, so the swizzle XORs the 16-byte unit with i
+    const int k = lane >> 3, i = lane & 7;
+    const uint32_t dst = smem_u32(stage) + (uint32_t)(px0 + 8 * (k >> 1) + i) * 128u + ((uint32_t)((2 * (r0 >> 4) + (k & 1)) ^ i) << 4);
+#pragma unroll
+    for (int jj = 0; jj < 4; ++jj) {
+      float v[8];                                    // v[m] = channel r0 + 8 ((m / 2) % 2), pixel 8 (2 jj + m / 4) + c0 + m % 2
+#pragma unroll
+      for (int m = 0; m < 8; ++m) v[m] = acc[8 * jj + m];
+      if (p.bias != nullptr) {
+#pragma unroll
+        for (int m = 0; m < 8; ++m) v[m] += b[(m >> 1) & 1];
+      }
+      activate(p, v);
+      stmatrix_x4_trans(dst + (uint32_t)jj * 16u * 128u, pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3]), pack_bf16x2(v[4], v[5]),
+                        pack_bf16x2(v[6], v[7]));
+    }
+  }
+}
+
 // One K block of a 128-row tile: 2 x KSTEPS k16 MMAs (rows 0-63 from descriptor ad, rows 64-127 from ad + a_hi, the same
 // B operand), issued back to back as ONE commit group.  KSTEPS must be known at compile time: an MMA under a runtime
 // condition makes ptxas split the group and inject warpgroup.arrive around it (warning C7519).
@@ -356,6 +415,19 @@ __device__ __forceinline__ void mma_kblock(float (&acc)[2][BN / 2], uint64_t ad,
     Wgmma<BN, 0, 0>::mma(acc[0], ad + (uint64_t)(2 * k), bd + (uint64_t)(2 * k), sd);
     Wgmma<BN, 0, 0>::mma(acc[1], ad + (uint64_t)(a_hi + 2 * k), bd + (uint64_t)(2 * k), sd);
   }
+  wgmma_commit();
+}
+
+// The same K block of a BN = 64 halo tile computed transposed, D[64 channels x 128 pixels]: the 64-row weight tile (wd) is the
+// A operand and the input box's 128 pixel rows (xd, sixteen 8-row groups) the B operand -- one m64n128k16 per k16 step, half
+// the instructions of mma_kblock<64> for the same FLOPs.  acc[h] holds pixels 64 h .. 64 h + 63 (wgmma fragment columns
+// 8 j + ..., j = 8 h + j' -> acc[h][4 j' + ...]).
+template <int KSTEPS>
+__device__ __forceinline__ void mma_kblock_t(float (&acc)[2][32], uint64_t wd, uint64_t xd, uint32_t scale_d) {
+  float(&d)[64] = reinterpret_cast<float(&)[64]>(acc);
+  wgmma_fence();
+#pragma unroll
+  for (int k = 0; k < KSTEPS; ++k) Wgmma<128, 0, 0>::mma(d, wd + (uint64_t)(2 * k), xd + (uint64_t)(2 * k), k == 0 ? scale_d : 1u);
   wgmma_commit();
 }
 
@@ -386,6 +458,7 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   const int lane = threadIdx.x & 31;
   constexpr bool HALO = (MODE != 0);
   constexpr bool BRES = (MODE == 2 || MODE == 4);
+  constexpr bool SWAP = (HALO && BN == 64);         // the tile is computed transposed (mma_kblock_t)
   using HG = HaloGeom<(MODE >= 3)>;
   // schedule: the CTA (or CTA pair) takes units unit0, unit0 + ustep, ...; in pair mode this CTA computes M tile `rank` of a unit
   const int rank = CP ? (int)cluster_ctarank() : 0;
@@ -550,7 +623,8 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       }
       if constexpr (HALO) {
         // A descriptors walk the halo tile: 8-row groups are the 8 pixels of one output row, SH halo rows apart;
-        // tap (r,s) shifts the start address by (W r + s) pixels, rows 64-127 start 8 output rows further.
+        // tap (r,s) shifts the start address by (W r + s) pixels, rows 64-127 start 8 output rows further.  At BN = 64 the same
+        // descriptor is the B operand and spans all 16 groups.
         const uint32_t row_bytes = (uint32_t)(HG::W * 128 * HG::SH);
         const uint64_t desc_a = wgmma_desc(16u, row_bytes, 1u);
         const uint64_t desc_b = wgmma_desc(16u, 1024u, 1u);
@@ -575,7 +649,8 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             if (!BRES || first) mbar_wait(&b_full[bs], BRES ? 0u : phb);
             const uint64_t ad = desc_a | (uint64_t)(a0 + (uint32_t)((tap / HG::KW) * HG::W + (tap % HG::KW)) * 8u);
             const uint64_t bd = desc_b | (uint64_t)(b_base + (uint32_t)bs * b_step);
-            mma_kblock<BN, 4>(acc, ad, a_hi, bd, started);
+            if constexpr (SWAP) mma_kblock_t<4>(acc, bd, ad, started);
+            else mma_kblock<BN, 4>(acc, ad, a_hi, bd, started);
             started = 1u;
             if (!BRES || prev_sa >= 0) {
               wgmma_wait<1>();
@@ -645,7 +720,14 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           if (h == 1 && !f32) break;
           if (ct == 0) bulk_wait_read();               // the last store has read the staging half
           warpgroup_bar_sync(wg);
-          if (f32) {
+          if constexpr (SWAP) {
+            if (f32) {
+              stage_out_tile_t<true>(p, acc[h], sbias, stage, 0, r0, c0, lane);
+            } else {
+              stage_out_tile_t<false>(p, acc[0], sbias, stage, 0, r0, c0, lane);
+              stage_out_tile_t<false>(p, acc[1], sbias, stage, 64, r0, c0, lane);
+            }
+          } else if (f32) {
             stage_out_tile<BN, true>(p, acc[h], sbias, stage, r0, c0);
           } else {
             stage_out_tile<BN, false>(p, acc[0], sbias, stage, r0, c0);
@@ -672,12 +754,21 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         const int rows = min(64, p.rows - 64 * h);
         if (rows <= 0) break;
         warpgroup_bar_sync(wg);                  // the previous pass's chunks have all been read from the staging half
+        if constexpr (SWAP) {                    // transposed: channels r0 + 8 i of pixels 8 j + c0 + c
 #pragma unroll
-        for (int j = 0; j < BN / 8; ++j) {
+          for (int j = 0; j < 8; ++j) {
 #pragma unroll
-          for (int i = 0; i < 2; ++i) {
-            *reinterpret_cast<float2*>(sCw + (r0 + 8 * i) * stage_pitch(BN) + 8 * j + c0) =
-                make_float2(acc[h][4 * j + 2 * i], acc[h][4 * j + 2 * i + 1]);
+            for (int m = 0; m < 4; ++m)
+              sCw[(8 * j + c0 + (m & 1)) * stage_pitch(BN) + r0 + 8 * (m >> 1)] = acc[h][4 * j + m];
+          }
+        } else {
+#pragma unroll
+          for (int j = 0; j < BN / 8; ++j) {
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+              *reinterpret_cast<float2*>(sCw + (r0 + 8 * i) * stage_pitch(BN) + 8 * j + c0) =
+                  make_float2(acc[h][4 * j + 2 * i], acc[h][4 * j + 2 * i + 1]);
+            }
           }
         }
         warpgroup_bar_sync(wg);
