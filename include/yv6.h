@@ -455,6 +455,11 @@ typedef struct yv6_wgrad_desc {
   int32_t force_taps;                                   /* ABI 2: 0 = auto (3x3: one CTA accumulates a filter row), 1 = one tap per CTA */
 } yv6_wgrad_desc;
 int yv6_conv_wgrad(yv6_handle* h, const yv6_wgrad_desc* d, void* stream);
+/* Host-only: the plan yv6_conv_wgrad makes for a device with the stated properties, no CUDA call.  out[0..9] = NT (Cin tile),
+ * T (taps per CTA), PT (pixels per stage), BW, BH (pixel box), pixel tiles, ksplit (CTAs that add partial sums of the same dW
+ * elements with fp32 atomics), pixels per split (PT * pixel tiles of the largest split, zero-filled rows included), CTAs,
+ * dynamic shared memory in bytes. */
+int yv6_wgrad_plan_host(int num_sms, int max_smem_optin, const yv6_wgrad_desc* d, int32_t* out10);
 
 /* Per-channel sum and sum of squares (float64) of an NHWC bf16 tensor slice with channel pitch `pitch`. */
 int yv6_bn_stats(yv6_handle* h, const void* x, int64_t pixels, int32_t C, int64_t pitch, double* sum, double* sumsq,

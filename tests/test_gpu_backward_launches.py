@@ -1,25 +1,53 @@
-"""Every backward launch of the training engine, run alone on fresh seeded data and checked against float64 autograd on the CPU.
+"""Every backward launch of the training engine, run alone on fresh seeded data and checked against float64.
 
 `test_train_step_matches_reference_op_by_op` checks whole buffers at 1e-2 relative L2, which a wrong edge column or a wrong tap
-in the border pixels of one dgrad parity does not move.  Here the engine (YOLOv6-N / M / L6) plans a step, and every launch of
-its backward call list -- dgrad convs (grouped per op and branch: four parity launches for a 3x3 stride-2 conv, one for 1x1
-stride 2), weight gradients, BatchNorm backward (with the BottleRep shortcut), the sums-only statistics of the pred and
-ConvTranspose bias gradients, the head-gradient repack, the SPPF max-pool backward chain and the stem im2col -- runs on its own
-descriptor: every raw pointer is resolved to the engine tensor it lies in, so offsets and pitches are exactly the engine's.
-Launches with the same descriptor signature (fields, and pointer offsets inside their tensors) run once.
+in the border pixels of one dgrad parity does not move.  Here the engine plans a step -- YOLOv6-N / M / L6 at 96-128 px, N-QA
+(the QA block's qa_bwd and its second bn_bwd on BN_d), N with the fuse_ab head (head_ab_grad), and the shapes the benchmark
+trains: YOLOv6-S at 640, batch 32, uint8 input, and YOLOv6-M at 640, batch 8 -- and every launch of its backward call list --
+dgrad convs (grouped per op and branch: four parity launches for a 3x3 stride-2 conv, one for 1x1 stride 2), weight
+gradients, BatchNorm backward (with the BottleRep shortcut), qa_bwd, the sums-only statistics of the pred and ConvTranspose
+bias gradients, the head-gradient repacks, the SPPF max-pool backward chain and the stem im2col -- runs on its own descriptor:
+every raw pointer is resolved to the engine tensor it lies in, so offsets and pitches are exactly the engine's.  Launches
+with the same descriptor signature (fields, and pointer offsets inside their tensors) run once.
 
-Bars are per element and scale with R = the same operation on absolute values (the sum of absolute terms):
-  fp32 accumulation (wgrad, BatchNorm sums, dalpha): |got - ref| <= 1e-5 R.  K <= 2^13 products or pixel partials are summed in
-    fp32 (per-thread runs of <= ~16 pixels, then float64 or split-K fp32 atomics), which costs a few 2^-24 sqrt(K) R at most;
-  bf16 outputs (dgrad, dx, dres): 2^-8 |ref| (one round-to-nearest-even to bf16, 8 significant bits) on top of the fp32 bar;
-  exact: the head-gradient repack (g * (s * (1 - s)) in fp32, rounded once) and im2col (fp32 image -> bf16 hi + bf16 lo);
+Engine memory.  Every tensor of the engine (activations, gradient buffers, dc / quadrant / pool scratch, head tensors and
+gradients, statistics and coefficients, patches, fuse_ab and QA tensors) holds 2^100 before each launch, except the zero
+arena, which holds zero as begin_step leaves it.  A check seeds the launch's inputs and the priors of its accumulating
+outputs; an assigning output keeps the sentinel, so a pixel it fails to write is left at 2^100.  After the launch the inputs
+must be unchanged, and once the inputs and outputs are put back every tensor must be at rest again, bit for bit.  The
+gradient-buffer outputs of a launch are its Write records (train.Write: buffer, channel slice, every pixel when `full`), so
+what a launch changes in the gradient buffers is held to what the first-writer resolution (train._resolve_first_writers)
+was told.
+
+Exact passes.  The flat master weights are integers in [-2, 2], repacked by begin_step into the forward and dgrad layouts
+(the real-valued passes run on the fabricated weights).  dgrad, wgrad and the statistic sums also run on integer operands
+in [-2, 2] (dgrad onto an integer prior when it
+accumulates): every fp32 partial sum is then an integer below 2^24 (asserted per launch: K * max|a| * max|b| < 2^24), so
+whatever the split-K, tiling or parity, wgrad must equal float64 plus the prior in fp32, dgrad float64 rounded once to bf16,
+and the sums the float64 sums -- a lost or doubled split, tile or parity launch cannot hide in a rounding bar.
+
+Real-valued passes, bars per element, R = the same operation on absolute values (the sum of absolute terms), u = 2^-24:
+  dgrad, wgrad: 1e-5 R (fp32 accumulation of random terms), plus 2^-8 |ref| for a bf16 output;
+  statistic sums: (L + 2) u R, L = the pixels one thread sums in fp32 before the float64 column sums (chan_run restates
+    chan_grid of yv6_train.cu); the terms (bf16 values and their squares) are exact in fp32, so this bound is rigorous;
+  bn_bwd: 1e-5 R for the pointwise fp32 work (activation backward, products, the apply pass) plus (L + 2) u R for the
+    per-thread run of the reduce pass; dalpha sums 8 channels per pixel and a warp tree, a run of 8 L + 5; the premise
+    L u < 2^-10 (first-order bound) is asserted per launch;
+  qa_bwd: the 3x3 window sum of 9 terms, the product by 1/9 and two additions in fp32, 16 u of the absolute terms, plus one
+    bf16 rounding;
+  exact: head-gradient repack (g * (s * (1 - s)) in fp32, rounded once), head_ab_grad's class columns and box offsets,
+    im2col (image -> bf16 hi + bf16 lo); head_ab_grad's w / h columns (sigmoid through expf): 2^-20 of |g * 8 anchor| s^2 plus
+    one bf16 rounding;
   max-pool backward: sums of <= 25 quantised bf16 values are exact in fp32, so each launch's output is one bf16 rounding of
     the exact sum; the reference rounds each link of the chain the same way and the bar allows one bf16 rounding.
-A wrong tap, a lost pixel tile or a doubled half-warp changes elements by O(|ref|), far above these bars.  The printed numbers
-are the worst error / bar ratio per launch kind."""
+The float64 references run on the GPU (torch's float64 convolutions and autograd, no code shared with this library); the
+first launch of each kind with a float64 reference is cross-checked once against the same computation on the CPU (image 0
+where the operation is per image).  The printed numbers are the distinct and total launches per kind, the worst error / bar
+ratio per kind, and the time taken."""
 import ctypes as C
 import functools
 import math
+import time
 
 import pytest
 import torch
@@ -30,11 +58,21 @@ from oracle import fabricate as fab
 
 pytestmark = pytest.mark.gpu
 
-MODELS = {"yolov6n": (128, 2), "yolov6m": (96, 2), "yolov6l6": (128, 2)}     # name: (image size, batch)
+# name -> model config, image size, batch, fuse_ab head, uint8 input.  S and M at 640 are the shapes bench.py trains.
+MODELS = {
+    "yolov6n": dict(cfg="yolov6n", size=128, batch=2), "yolov6m": dict(cfg="yolov6m", size=96, batch=2),
+    "yolov6l6": dict(cfg="yolov6l6", size=128, batch=2), "yolov6n_qa": dict(cfg="yolov6n_qa", size=96, batch=2),
+    "yolov6n_fuse_ab": dict(cfg="yolov6n", size=128, batch=2, fuse_ab=True),
+    "yolov6s_640_b32_u8": dict(cfg="yolov6s", size=640, batch=32, u8=True), "yolov6m_640_b8": dict(cfg="yolov6m", size=640, batch=8),
+}
+GOLDEN_KEYS = ("yolov6n", "yolov6s", "yolov6m", "yolov6l6")
 BN_EPS = 1e-3
 F32_SUM = 1e-5           # fp32 accumulation, relative to the sum of absolute terms
 BF16_ULP = 2.0 ** -8     # one round-to-nearest-even to bf16 (8 significant bits) moves a value by at most 2^-8 of it
+U = 2.0 ** -24           # fp32 unit roundoff
+SENTINEL = 2.0 ** 100
 BF16, F32, F64 = torch.bfloat16, torch.float32, torch.float64
+REST_EXEMPT = ("param", "img")   # master weights and the input image: not outputs of any backward launch
 
 
 # ---------------------------------------------------------------------------------------------------------------- helpers
@@ -73,6 +111,93 @@ class Mem:
         return self.find(ptr)[1]
 
 
+class IO:
+    """What one check did to engine memory: inputs it seeded (with a copy, they must come out unchanged) and outputs."""
+
+    def __init__(self):
+        self.seeded, self.ins, self.outs = [], [], []
+
+    def seed(self, v):
+        self.seeded.append(v)
+        return v
+
+    def freeze(self):
+        """Right before the launch: copies of the seeded inputs."""
+        self.ins = [(v, v.clone()) for v in self.seeded]
+
+    def out(self, v):
+        self.outs.append(v)
+        return v
+
+
+def int_view(t):
+    return t.view({1: torch.uint8, 2: torch.int16, 4: torch.int32, 8: torch.int64}[t.element_size()])
+
+
+def at_rest(tag, t):
+    if tag == "arena":
+        return not bool(t.any())
+    return bool((int_view(t) == int_view(torch.tensor([SENTINEL], dtype=t.dtype)).item()).all())
+
+
+def poison(mem):
+    """Every engine tensor to its rest state: the zero arena zero (as begin_step leaves it), everything else 2^100."""
+    for _, _, tag, t in mem.ts:
+        if tag == "arena":
+            t.zero_()
+        elif tag not in REST_EXEMPT:
+            t.fill_(SENTINEL)
+
+
+def settle(mem, ins, outs, what):
+    """After a checked launch: its inputs still hold what was seeded; then inputs and outputs go back to rest, and every engine
+    tensor must be at rest everywhere -- an element the launch wrote outside its declared outputs is left over."""
+    for v, before in ins:
+        assert torch.equal(int_view(v), int_view(before)), f"{what}: changed one of its inputs"
+    for v in [v for v, _ in ins] + list(outs):
+        if mem.find(v.data_ptr())[0] == "arena":
+            v.zero_()
+        else:
+            v.fill_(SENTINEL)
+    bad = [f"{tag} {tuple(t.shape)}" for _, _, tag, t in mem.ts if tag not in REST_EXEMPT and not at_rest(tag, t)]
+    assert not bad, f"{what}: wrote outside the outputs it declares: " + "; ".join(bad)
+
+
+def assert_full_write(v, what):
+    """An assigning write started from the sentinel: every element must have been written."""
+    left = v.float().abs() >= SENTINEL
+    assert not bool(left.any()), f"{what}: not every pixel of a full write was written ({int(left.sum())} elements left)"
+
+
+def assert_exact(got, exp, what):
+    diff = got.double() != exp.double()
+    assert not bool(diff.any()), (f"{what}: not exact: {int(diff.sum())} elements differ, worst by "
+                                  f"{float((got.double() - exp.double()).abs().max()):.3g}")
+
+
+def exact_k_bound(k, amax, bmax, prior=2):
+    """Every fp32 partial sum of k products of integers |a| <= amax, |b| <= bmax onto an integer prior is exact."""
+    return k * amax * bmax + prior < 2 ** 24
+
+
+def num_sms():
+    return torch.cuda.get_device_properties(0).multi_processor_count
+
+
+def chan_run(pixels, c, per_sm, min_iters):
+    """Pixels one thread of the channel-reduction kernels sums in fp32: chan_grid (yv6_train.cu) restated.  Threads per block
+    cover C / 8 channel groups x prows pixel rows; the grid is capped at per_sm blocks per SM."""
+    prows = max(1, 256 // (c // 8))
+    grid = max(1, min(-(-pixels // (prows * min_iters)), num_sms() * per_sm))
+    return -(-pixels // (grid * prows))
+
+
+def run_bar(run):
+    """fp32 sum of `run` terms, then converted into a float64 sum: (run + 2) u of the sum of absolute terms (first order)."""
+    assert run * U < 2.0 ** -10, f"a run of {run} fp32 additions is outside the first-order bound"
+    return (run + 2) * U
+
+
 def signature(d, mem):
     """Descriptor fields, with each pointer replaced by (tensor kind, offset inside it); per-op accumulator slots in the zero
     arena and parameters compare equal whatever their offset."""
@@ -91,7 +216,11 @@ def signature(d, mem):
 
 
 def rnd(gen, *shape, dtype=BF16, scale=1.0, shift=0.0):
-    return (torch.randn(*shape, generator=gen, dtype=F64) * scale + shift).to(dtype)
+    return (torch.randn(*shape, generator=gen, dtype=F64, device=gen.device) * scale + shift).to(dtype)
+
+
+def ints(gen, *shape, dtype=BF16):
+    return torch.randint(-2, 3, shape, generator=gen, device=gen.device).to(dtype)
 
 
 def ratio(got, exp, bound):
@@ -114,130 +243,208 @@ def nchw(t):
     return t.double().permute(0, 3, 1, 2)
 
 
+def nhwc_strides(H, W, pitch):
+    return (H * W * pitch, W * pitch, pitch, 1)
+
+
 def check(lib_rc, lib):
     assert lib_rc == 0, lib.yv6_last_error().decode()
 
 
+XCHECKED = set()     # kinds whose GPU float64 reference was cross-checked on the CPU
+
+
+def cross_check(kind, ref, R, fn):
+    """Once per kind: the GPU float64 reference `ref` (R: its absolute-value sum) against fn() = the same on the CPU."""
+    if kind in XCHECKED:
+        return
+    XCHECKED.add(kind)
+    rc = fn()
+    err = float(((ref.cpu() - rc).abs() / (R.cpu() + 1e-300)).max())
+    assert err < 1e-12, f"{kind}: GPU float64 reference differs from the CPU by {err:.2e} of R"
+
+
 # ---------------------------------------------------------------------------------------------------------------- per-kind checks
-def check_dgrad(lib, h, sp, mem, descs, wf, stride, gbuf, off, cin, gen):
+def check_dgrad(lib, h, sp, mem, descs, wf, stride, gbuf, meta, gen, io, exact):
     """One op's input gradient: g(src)[..., off:off + cin] (+)= conv2d_input(dc, W) over the launches of `descs` (all read the same
-    dc).  Elements outside the slice, and pixels no launch writes, keep the prior bit for bit."""
+    dc).  An assigning group starts from the sentinel, an accumulating one from a prior; pixels no launch writes keep it."""
     d0 = descs[0]
+    off, cin = meta.off, meta.n
     N, Hd, Wd, Cd, xct = d0.N, d0.H, d0.W, d0.Cin, d0.x_c_total
     assert all(d.x == d0.x for d in descs)
     acc = {bool(d.res) for d in descs}
     assert len(acc) == 1, "launches of one dgrad disagree on accumulate"
     acc = acc.pop()
-    dc = rnd(gen, N, Hd, Wd, Cd)
-    mem.at(d0.x, BF16, (N, Hd, Wd, Cd), (Hd * Wd * xct, Wd * xct, xct, 1)).copy_(dc)
-    prior = rnd(gen, *gbuf.shape)
-    gbuf.copy_(prior)
+    co, k, _, ci = wf.shape
+    assert ci == cin
+    if exact:
+        assert exact_k_bound(co * k * k, 2, 2), "dgrad sum too long for exact integer operands"
+    dcv = mem.at(d0.x, BF16, (N, Hd, Wd, Cd), (Hd * Wd * xct, Wd * xct, xct, 1))
+    dcv.copy_(ints(gen, N, Hd, Wd, Cd) if exact else rnd(gen, N, Hd, Wd, Cd))
+    io.seed(dcv)
+    sl = io.out(gbuf[..., off:off + cin])
+    if acc:
+        sl.copy_(ints(gen, *sl.shape) if exact else rnd(gen, *sl.shape))
+    before = sl.clone()
+    io.freeze()
     for d in descs:
         check(lib.yv6_conv_fwd(h, C.byref(d), sp), lib)
     torch.cuda.synchronize()
-    got = gbuf.cpu()
     # which pixels the launches write: element (n, i, j) of launch d sits at d.y + n*s0 + i*s1 + j*s2 (elements)
     n_, hs, ws, gct = gbuf.shape
-    written = torch.zeros(n_ * hs * ws, dtype=torch.bool)
+    dev = gbuf.device
+    written = torch.zeros(n_ * hs * ws, dtype=torch.bool, device=dev)
     base = gbuf.data_ptr()
     for d in descs:
         oh = d.out_h or (d.H + 2 * d.pad - d.kh) // d.stride + 1
         ow = d.out_w or (d.W + 2 * d.pad - d.kw) // d.stride + 1
         e0 = (d.y - base) // 2 - off
-        idx = (e0 + torch.arange(d.N).view(-1, 1, 1) * d.y_img_stride + torch.arange(oh).view(1, -1, 1) * d.y_h_stride
-               + torch.arange(ow).view(1, 1, -1) * d.y_w_stride)
+        idx = (e0 + torch.arange(d.N, device=dev).view(-1, 1, 1) * d.y_img_stride + torch.arange(oh, device=dev).view(1, -1, 1) * d.y_h_stride
+               + torch.arange(ow, device=dev).view(1, 1, -1) * d.y_w_stride)
         assert bool((idx % gct == 0).all())
         written[(idx // gct).reshape(-1)] = True
-    written = written.view(n_, hs, ws, 1)
-    co, k, _, ci = wf.shape
-    assert ci == cin
-    w64 = nchw(wf.cpu()).contiguous()
-    dcn = nchw(dc[..., :co])
+    written = written.view(n_, hs, ws)
+    assert not meta.full or bool(written.all()), "a full Write whose launches leave pixels out"
+    w64 = nchw(wf).contiguous()
+    dcn = nchw(dcv[..., :co])
     gin = torch.nn.grad.conv2d_input((n_, ci, hs, ws), w64, dcn, stride=stride, padding=k // 2).permute(0, 2, 3, 1)
+    assert not bool(((gin != 0) & ~written[..., None]).any()), "the launches do not cover every pixel of the input gradient"
+    got = sl.clone()
+    assert torch.equal(int_view(got[~written]), int_view(before[~written])), "dgrad wrote pixels outside its launches"
+    if not acc:
+        assert_full_write(got[written], "dgrad")
+    p = before[written].double() if acc else 0.0
+    exp = p + gin[written]
+    if exact:
+        assert_exact(got[written], exp.to(BF16), "dgrad")
+        return 0.0
     R = torch.nn.grad.conv2d_input((n_, ci, hs, ws), w64.abs(), dcn.abs(), stride=stride, padding=k // 2).permute(0, 2, 3, 1)
-    assert not bool(((gin != 0) & ~written).any()), "the launches do not cover every pixel of the input gradient"
-    p = prior[..., off:off + cin].double()
-    exp = torch.where(written, p * acc + gin, p)
-    bound = torch.where(written, BF16_ULP * exp.abs() + F32_SUM * (R + acc * p.abs()), torch.zeros_like(p))
-    r = ratio(got[..., off:off + cin], exp, bound)
-    outside = torch.ones(gct, dtype=torch.bool)
-    outside[off:off + cin] = False
-    assert bits_equal(got[..., outside], prior[..., outside]), "dgrad wrote outside its channel slice"
-    return r
+    cross_check("dgrad", gin[:1], R[:1], lambda: torch.nn.grad.conv2d_input((1, ci, hs, ws), w64.cpu(), dcn[:1].cpu(), stride=stride,
+                                                                            padding=k // 2).permute(0, 2, 3, 1))
+    pa = p.abs() if acc else 0.0
+    return ratio(got[written], exp, BF16_ULP * exp.abs() + F32_SUM * (R[written] + pa))
 
 
-def wgrad_ref(x, dy, cout, k, stride, pad):
+def wgrad_ref(x, dy, cout, k, stride, pad, absolute=True):
     """dW [Cout][k][k][Cin] of conv2d(x, W) against dy, and the same on absolute values (x, dy: NHWC)."""
     xs, ds = nchw(x), nchw(dy)
     shape = (cout, x.shape[3], k, k)
     ref = torch.nn.grad.conv2d_weight(xs, shape, ds, stride=stride, padding=pad).permute(0, 2, 3, 1)
+    if not absolute:
+        return ref, None
     R = torch.nn.grad.conv2d_weight(xs.abs(), shape, ds.abs(), stride=stride, padding=pad).permute(0, 2, 3, 1)
     return ref, R
 
 
-def check_wgrad(lib, h, sp, mem, d, gen):
-    """dW += wgrad(x, dY) on the descriptor's slices, onto a random prior and onto zeros."""
+def check_wgrad(lib, h, sp, mem, d, gen, io, exact):
+    """dW += wgrad(x, dY) on the descriptor's slices, onto a prior and onto zeros."""
     N, H, W, Cin, xct, Cout, dct, k = d.N, d.H, d.W, d.Cin, d.x_c_total, d.Cout, d.dy_c_total, d.kh
     Ho, Wo = (H + 2 * d.pad - k) // d.stride + 1, (W + 2 * d.pad - d.kw) // d.stride + 1
+    if exact:
+        assert exact_k_bound(N * Ho * Wo, 2, 2), "wgrad sum too long for exact integer operands"
     for ptr in (d.x, d.dy):     # whole tensors: channels outside the slices hold data too
         t = mem.base(ptr)
-        t.copy_(rnd(gen, *t.shape))
-    x = mem.at(d.x, BF16, (N, H, W, Cin), (H * W * xct, W * xct, xct, 1)).cpu()
-    dy = mem.at(d.dy, BF16, (N, Ho, Wo, Cout), (Ho * Wo * dct, Wo * dct, dct, 1)).cpu()
-    dw = mem.at(d.dw, F32, (Cout, k, k, Cin))
-    ref, R = wgrad_ref(x, dy, Cout, k, d.stride, d.pad)
-    prior = rnd(gen, Cout, k, k, Cin, dtype=F32)
+        t.copy_(ints(gen, *t.shape, dtype=t.dtype) if exact else rnd(gen, *t.shape, dtype=t.dtype))
+        io.seed(t)
+    x = mem.at(d.x, BF16, (N, H, W, Cin), (H * W * xct, W * xct, xct, 1))
+    dy = mem.at(d.dy, BF16, (N, Ho, Wo, Cout), (Ho * Wo * dct, Wo * dct, dct, 1))
+    dw = io.out(mem.at(d.dw, F32, (Cout, k, k, Cin)))
+    ref, R = wgrad_ref(x, dy, Cout, k, d.stride, d.pad, absolute=not exact)
+    if not exact:
+        cross_check("wgrad", wgrad_ref(x[:1], dy[:1], Cout, k, d.stride, d.pad, absolute=False)[0],
+                    wgrad_ref(x[:1], dy[:1], Cout, k, d.stride, d.pad)[1],
+                    lambda: wgrad_ref(x[:1].cpu(), dy[:1].cpu(), Cout, k, d.stride, d.pad, absolute=False)[0])
+    prior = ints(gen, Cout, k, k, Cin, dtype=F32) if exact else rnd(gen, Cout, k, k, Cin, dtype=F32)
     worst = 0.0
     for pr in (prior, torch.zeros_like(prior)):
         dw.copy_(pr)
+        io.freeze()
         check(lib.yv6_conv_wgrad(h, C.byref(d), sp), lib)
         torch.cuda.synchronize()
         p = pr.double()
-        worst = max(worst, ratio(dw.cpu(), p + ref, F32_SUM * (R + p.abs())))
+        if exact:
+            assert_exact(dw, (p + ref).float(), "wgrad")
+        else:
+            worst = max(worst, ratio(dw, p + ref, F32_SUM * (R + p.abs())))
     return worst
 
 
-def check_stats_sums(lib, h, sp, mem, d, gen):
+def check_stats_sums(lib, h, sp, mem, d, gen, io, exact):
     """Sums only (no finalize): per-channel sum and sum of squares of an NHWC slice into a zeroed arena slot."""
     assert d.nb == 1 and not d.stats[0]
     P, Cc, pitch = d.pixels, d.C, d.x_pitch[0]
     t = mem.base(d.x[0])
-    t.copy_(rnd(gen, *t.shape))
-    x = mem.at(d.x[0], BF16, (P, Cc), (pitch, 1)).cpu().double()
-    sums = mem.at(d.sums, F64, (2, Cc))
-    cnt = mem.at(d.counter, torch.int32, (1,))
-    assert d.zeroed
-    sums.zero_()
-    cnt.zero_()
+    t.copy_(ints(gen, *t.shape, dtype=t.dtype) if exact else rnd(gen, *t.shape, dtype=t.dtype))
+    io.seed(t)
+    x = mem.at(d.x[0], BF16, (P, Cc), (pitch, 1)).double()
+    sums = io.out(mem.at(d.sums, F64, (2, Cc)))
+    io.out(mem.at(d.counter, torch.int32, (1,)))
+    assert d.zeroed      # the arena slots are zero, as begin_step leaves them
+    io.freeze()
     check(lib.yv6_bn_stats_finalize(h, C.byref(d), sp), lib)
     torch.cuda.synchronize()
-    got = sums.cpu()
     q = x * x
-    return max(ratio(got[0], x.sum(0), F32_SUM * x.abs().sum(0)), ratio(got[1], q.sum(0), F32_SUM * q.sum(0)))
+    if exact:
+        assert exact_k_bound(P, 2, 2), "statistic sums too long for exact integer operands"
+        assert_exact(sums[0], x.sum(0), "stats sum")
+        assert_exact(sums[1], q.sum(0), "stats sum of squares")
+        return 0.0
+    cross_check("stats", x.sum(0), x.abs().sum(0), lambda: x.cpu().sum(0))
+    bar = run_bar(chan_run(P, Cc, 4, 16))
+    return max(ratio(sums[0], x.sum(0), bar * x.abs().sum(0)), ratio(sums[1], q.sum(0), bar * q.sum(0)))
 
 
-def check_bn_bwd(lib, h, sp, mem, d, gen, positive=False):
-    """yv6_bn_bwd on fresh branch inputs with their true batch statistics in the stat slots, against autograd through
-    act(sum_b BN_b(x_b)) (+ alpha * res) with batch-statistics BatchNorm.  Returns {output: worst ratio}."""
+def bn_bwd_ref(xs, st, dy, act, res=None, alpha=0.0):
+    """Autograd through act(sum_b BN_b(x_b)) (+ alpha * res) with batch-statistics BatchNorm, float64.  Returns (dz, dbeta,
+    [dgamma_b], [dx_b], dres, dalpha)."""
+    xr = [x.clone().requires_grad_(True) for x in xs]
+    gr = [s["gam"].clone().requires_grad_(True) for s in st]
+    br = [s["bet"].clone().requires_grad_(True) for s in st]
+    z = 0
+    for b in range(len(xs)):
+        mu, var = xr[b].mean(0), xr[b].var(0, unbiased=False)
+        z = z + (xr[b] - mu) / torch.sqrt(var + BN_EPS) * gr[b] + br[b]
+    z.retain_grad()
+    y = torch.relu(z) if act == 1 else (z * torch.sigmoid(z) if act == 2 else z)
+    rr = al = None
+    if res is not None:
+        rr = res.double().requires_grad_(True)
+        al = torch.tensor(alpha, dtype=F64, device=res.device, requires_grad=True)
+        y = y + al * rr
+    (y * dy.double()).sum().backward()
+    return (z.grad, br[0].grad, [g.grad for g in gr], [x.grad for x in xr], None if rr is None else rr.grad,
+            None if al is None else al.grad.view(1))
+
+
+def check_bn_bwd(lib, h, sp, mem, d, gen, positive=False, io=None):
+    """yv6_bn_bwd on fresh branch inputs with their true batch statistics in the stat slots, against float64 autograd through
+    act(sum_b BN_b(x_b)) (+ alpha * res) with batch-statistics BatchNorm.  Returns {output: worst ratio}.  With `io` (engine
+    memory) an assigning output starts from the sentinel and must be written everywhere."""
     nb, Cc, P, act = d.nb, d.C, d.pixels, d.act
+    dev = gen.device
+    host = lambda t: t.to(dev)     # noqa: E731
     view = lambda ptr, pitch: mem.at(ptr, BF16, (P, Cc), (pitch, 1))     # noqa: E731
+    engine = io is not None
+    io = io or IO()
+    L = chan_run(P, Cc, 4, 16)           # the reduce pass's grid (yv6_bn_bwd: grid_r)
+    rb = F32_SUM + run_bar(L)
     xs, st = [], []
     for b in range(nb):
         x = rnd(gen, P, Cc, scale=1 + b, shift=0.3 * b)
-        view(d.x[b], d.x_pitch[b]).copy_(x)
+        io.seed(view(d.x[b], d.x_pitch[b])).copy_(x)
         xs.append(x.double())
     for b in range(nb):
         x = xs[b]
-        gam = torch.rand(Cc, generator=gen, dtype=F64) + 0.5
-        bet = torch.randn(Cc, generator=gen, dtype=F64) * 0.1
+        gam = torch.rand(Cc, generator=gen, dtype=F64, device=dev) + 0.5
+        bet = torch.randn(Cc, generator=gen, dtype=F64, device=dev) * 0.1
         mean, var = x.mean(0), x.var(0, unbiased=False)
         inv = 1.0 / torch.sqrt(var + BN_EPS)
         vals = [mean, inv, gam * inv, bet - mean * gam * inv]
         for ptr, v in zip((d.mean[b], d.invstd[b], d.scale[b], d.shift[b]), vals):
-            mem.at(ptr, F32, (Cc,)).copy_(v.float())
+            io.seed(mem.at(ptr, F32, (Cc,))).copy_(v.float())
         st.append(dict(gam=gam, bet=bet, mean=mean.float().double(), inv=inv.float().double(), sc=(gam * inv).float().double(),
                        sh=(bet - mean * gam * inv).float().double()))
-    dy = torch.randn(P, Cc, generator=gen, dtype=F64)
+    dy = torch.randn(P, Cc, generator=gen, dtype=F64, device=dev)
     if positive:
         dy = dy.abs() + 0.1
     if act == 1:       # relu: where z is within fp32 rounding of 0 the kernel and float64 may disagree on the mask -- no gradient there
@@ -245,31 +452,37 @@ def check_bn_bwd(lib, h, sp, mem, d, gen, positive=False):
         tau = 1e-5 * (sum(st[b]["sh"].abs() for b in range(nb)) + sum((xs[b] * st[b]["sc"]).abs() for b in range(nb)))
         dy[z32.abs() < tau] = 0
     dy = dy.to(BF16)
-    view(d.dy, d.dy_pitch).copy_(dy)
+    io.seed(view(d.dy, d.dy_pitch)).copy_(dy)
     has_res = bool(d.res)
+    sentinel_assign = engine
     if has_res:
         res = rnd(gen, P, Cc)
         if positive:
             res = res.abs()
-        view(d.res, d.res_pitch).copy_(res)
+        io.seed(view(d.res, d.res_pitch)).copy_(res)
         alpha = float(mem.at(d.res_alpha_dev, F32, (1,)).item()) if d.res_alpha_dev else float(d.res_alpha)
         dres_prior = rnd(gen, P, Cc)
-        view(d.dres, d.dres_pitch).copy_(dres_prior)
+        dres_v = io.out(view(d.dres, d.dres_pitch))
+        if not (sentinel_assign and d.dres_assign):
+            dres_v.copy_(dres_prior)
     dx_prior = []
     for b in range(nb):
         pr = rnd(gen, P, Cc)
-        view(d.dx[b], d.dx_pitch[b]).copy_(pr)
+        v = io.out(view(d.dx[b], d.dx_pitch[b]))
+        if not (sentinel_assign and not d.accumulate[b]):
+            v.copy_(pr)
         dx_prior.append(pr)
     # accumulators: a caller arena with zeroed = 1 is cleared by the caller; otherwise the launch clears them (garbage here)
     caller = bool(d.work)
-    garbage = lambda t: t.copy_(torch.randn(t.shape, generator=gen, dtype=F64).to(t.dtype))   # noqa: E731
-    s1 = mem.at(d.s1, F64, (Cc,))
-    s2 = [mem.at(d.s2[b], F64, (Cc,)) for b in range(nb)]
+    garbage = lambda t: t.copy_(torch.randn(t.shape, generator=gen, dtype=F64, device=dev).to(t.dtype))   # noqa: E731
+    s1 = io.out(mem.at(d.s1, F64, (Cc,)))
+    s2 = [io.out(mem.at(d.s2[b], F64, (Cc,))) for b in range(nb)]
     for t in s2:
         garbage(t)
-    da = mem.at(d.dalpha, F64, (1,)) if has_res else None
+    da = io.out(mem.at(d.dalpha, F64, (1,))) if has_res else None
     if caller:
-        work, cnt, coef = mem.at(d.work, F64, (nb, Cc)), mem.at(d.counter, torch.int32, (1,)), mem.at(d.coef, F32, (nb, 2, Cc))
+        work, cnt = io.out(mem.at(d.work, F64, (nb, Cc))), io.out(mem.at(d.counter, torch.int32, (1,)))
+        coef = io.out(mem.at(d.coef, F32, (nb, 2, Cc)))
         garbage(coef)
     if caller and d.zeroed:
         for t in [s1, work, cnt] + ([da] if has_res else []):
@@ -277,119 +490,186 @@ def check_bn_bwd(lib, h, sp, mem, d, gen, positive=False):
     else:
         for t in [s1] + ([da] if has_res else []) + ([work] if caller else []):
             garbage(t)
+    io.freeze()
     check(lib.yv6_bn_bwd(h, C.byref(d), sp), lib)
     torch.cuda.synchronize()
 
     # ---- float64 reference
-    xr = [x.clone().requires_grad_(True) for x in xs]
-    gr = [s["gam"].clone().requires_grad_(True) for s in st]
-    br = [s["bet"].clone().requires_grad_(True) for s in st]
-    z = 0
-    for b in range(nb):
-        mu, var = xr[b].mean(0), xr[b].var(0, unbiased=False)
-        z = z + (xr[b] - mu) / torch.sqrt(var + BN_EPS) * gr[b] + br[b]
-    z.retain_grad()
-    y = torch.relu(z) if act == 1 else (z * torch.sigmoid(z) if act == 2 else z)
-    if has_res:
-        rr = res.double().requires_grad_(True)
-        al = torch.tensor(alpha, dtype=F64, requires_grad=True)
-        y = y + al * rr
-    (y * dy.double()).sum().backward()
-    dz = z.grad
+    dz, S1, S2s, dxs, dres_g, dal = bn_bwd_ref(xs, st, dy, act, res if has_res else None, alpha if has_res else 0.0)
+    if "bn_bwd" not in XCHECKED and P * Cc <= 1 << 22:
+        cpu = lambda t: None if t is None else t.cpu()     # noqa: E731
+        ref_c = bn_bwd_ref([cpu(x) for x in xs], [{k: cpu(v) for k, v in s.items()} for s in st], cpu(dy), act,
+                           cpu(res) if has_res else None, alpha if has_res else 0.0)
+        cross_check("bn_bwd", dxs[0], torch.full_like(dxs[0], float(dxs[0].abs().max())), lambda: ref_c[3][0])
     out = {}
     R1 = dz.abs().sum(0)
-    S1 = br[0].grad
-    out["s1"] = ratio(s1.cpu(), S1, F32_SUM * R1)
+    out["s1"] = ratio(host(s1), S1, rb * R1)
     worst_dx, worst_s2 = 0.0, 0.0
     for b in range(nb):
         s = st[b]
         R2 = s["inv"] * ((dz.abs() * xs[b].abs()).sum(0) + s["mean"].abs() * R1)
-        S2 = gr[b].grad
-        worst_s2 = max(worst_s2, ratio(s2[b].cpu(), S2, F32_SUM * R2))
-        Bc = -s["sc"] * s["inv"] * S2 / P
+        worst_s2 = max(worst_s2, ratio(host(s2[b]), S2s[b], rb * R2))
+        Bc = -s["sc"] * s["inv"] * S2s[b] / P
         Cb = -s["sc"] * S1 / P - Bc * s["mean"]
         xhat = (xs[b] - s["mean"]) * s["inv"]
         acc = bool(d.accumulate[b])
         p = dx_prior[b].double() * acc
         Rdx = ((s["sc"] * dz).abs() + Bc.abs() * xs[b].abs() + Cb.abs() + s["sc"].abs() * (R1 + xhat.abs() * R2) / P + p.abs())
-        exp = p + xr[b].grad
-        worst_dx = max(worst_dx, ratio(view(d.dx[b], d.dx_pitch[b]).cpu(), exp, BF16_ULP * exp.abs() + F32_SUM * Rdx))
+        exp = p + dxs[b]
+        got = host(view(d.dx[b], d.dx_pitch[b]))
+        if sentinel_assign and not acc:
+            assert_full_write(got, "bn_bwd dx")
+        worst_dx = max(worst_dx, ratio(got, exp, BF16_ULP * exp.abs() + rb * Rdx))
         if caller:      # coefficients of the apply pass: the closed form of the kernel's comment on its own sums
-            S1k, S2k = s1.cpu(), s2[b].cpu()
+            S1k, S2k = host(s1), host(s2[b])
             Bk = -s["sc"] * s["inv"] * S2k / P
             Ck = -s["sc"] * S1k / P - Bk * s["mean"]
-            cf = coef.cpu().double()
+            cf = host(coef).double()
             out["coef"] = max(out.get("coef", 0.0), ratio(cf[b, 0], Bk, 2.0 ** -22 * Bk.abs()),
                               ratio(cf[b, 1], Ck, 2.0 ** -22 * ((s["sc"] * S1k / P).abs() + (Bk * s["mean"]).abs())))
     out["s2"], out["dx"] = worst_s2, worst_dx
     if has_res:
         keep = 0.0 if d.dres_assign else 1.0
         p = dres_prior.double() * keep
-        exp = p + rr.grad
-        out["dres"] = ratio(view(d.dres, d.dres_pitch).cpu(), exp, BF16_ULP * exp.abs() + F32_SUM * ((alpha * dy.double()).abs() + p.abs()))
-        out["dalpha"] = ratio(da.cpu(), al.grad.view(1), F32_SUM * (dy.double() * res.double()).abs().sum().view(1))
+        exp = p + dres_g
+        got = host(view(d.dres, d.dres_pitch))
+        if sentinel_assign and d.dres_assign:
+            assert_full_write(got, "bn_bwd dres")
+        out["dres"] = ratio(got, exp, BF16_ULP * exp.abs() + F32_SUM * ((alpha * dy.double()).abs() + p.abs()))
+        out["dalpha"] = ratio(host(da), dal, (F32_SUM + run_bar(8 * L + 5)) * (dy.double() * res.double()).abs().sum().view(1))
     return out
 
 
-def check_hgp(lib, h, sp, mem, args, gen):
+def check_qa_bwd(lib, h, sp, mem, q, gen, io):
+    """yv6_qa_bwd: dx (+)= dt + avg3x3^T(dt) (the adjoint of AvgPool2d(3, 1, 1) with count_include_pad is the same box filter)."""
+    N, H, W, Cc = q.N, q.H, q.W, q.C
+    dt = io.seed(mem.at(q.dt, BF16, (N, H, W, Cc), nhwc_strides(H, W, q.dt_pitch)))
+    dt.copy_(rnd(gen, N, H, W, Cc))
+    dx = io.out(mem.at(q.dx, BF16, (N, H, W, Cc), nhwc_strides(H, W, q.dx_pitch)))
+    acc = bool(q.accumulate)
+    if acc:
+        dx.copy_(rnd(gen, N, H, W, Cc))
+    p = dx.double() if acc else 0.0
+    io.freeze()
+    check(lib.yv6_qa_bwd(h, C.byref(q), sp), lib)
+    torch.cuda.synchronize()
+    d64 = dt.double()
+    avg3 = lambda t: F.avg_pool2d(t.permute(0, 3, 1, 2), 3, 1, 1, count_include_pad=True).permute(0, 2, 3, 1)  # noqa: E731
+    ref = p + d64 + (avg3(d64) if q.avg else 0.0)
+    R = d64.abs() + (avg3(d64.abs()) if q.avg else 0.0) + (p.abs() if acc else 0.0)
+    if q.avg:
+        cross_check("qa_bwd", (d64 + avg3(d64))[:1], R[:1], lambda: d64[:1].cpu() + avg3(d64[:1].cpu()))
+    if not acc:
+        assert_full_write(dx, "qa_bwd dx")
+    return ratio(dx, ref, 16 * U * R + BF16_ULP * ref.abs())     # window of 9 terms, x 1/9, two additions
+
+
+def check_hgp(lib, h, sp, mem, args, gen, io):
     """dlogit = bf16(g * (s * (1 - s))) (or bf16(g)), repacked to NHWC with zero padded channels: bit for bit."""
     gp, sp_, B, A, ch, off, hw, chp, outp = args
-    g = mem.at(gp, F32, (B, A, ch))
-    g.copy_(torch.randn(B, A, ch, generator=gen))
+    g = io.seed(mem.at(gp, F32, (B, A, ch)))
+    g.copy_(torch.randn(B, A, ch, generator=gen, device=gen.device))
     if sp_:
-        s = mem.at(sp_, F32, (B, A, ch))
-        s.copy_(torch.rand(B, A, ch, generator=gen))
-    out = mem.at(outp, BF16, (B, hw, chp))
-    out.copy_(rnd(gen, B, hw, chp))
+        s = io.seed(mem.at(sp_, F32, (B, A, ch)))
+        s.copy_(torch.rand(B, A, ch, generator=gen, device=gen.device))
+    out = io.out(mem.at(outp, BF16, (B, hw, chp)))
+    io.freeze()
     check(lib.yv6_head_grad_prep(h, gp, sp_, B, A, ch, off, hw, chp, outp, sp), lib)
     torch.cuda.synchronize()
-    v = g.cpu()[:, off:off + hw]
+    v = g[:, off:off + hw]
     if sp_:
-        sv = s.cpu()[:, off:off + hw]
+        sv = s[:, off:off + hw]
         v = v * (sv * (1 - sv))
-    exp = torch.zeros(B, hw, chp, dtype=F32)
+    exp = torch.zeros(B, hw, chp, dtype=F32, device=g.device)
     exp[..., :ch] = v
-    assert bits_equal(out.cpu(), exp.to(BF16)), "head_grad_prep differs from bf16(g * s * (1 - s))"
+    assert bits_equal(out, exp.to(BF16)), "head_grad_prep differs from bf16(g * s * (1 - s))"
     return 0.0
 
 
-def check_pool_chain(lib, h, sp, eng, calls, gen):
+def check_abg(lib, h, sp, mem, args, gen, io):
+    """yv6_head_ab_grad: rows (level, anchor, pixel) of the fuse_ab gradients -> NHWC bf16 gradients of the raw pred outputs.
+    Class columns bf16((g * s) * (1 - s)) and box offsets bf16(g) bit for bit; w / h: g * 8 anchor s^2 (1 - s), s = sigmoid of
+    the raw output; padded channels zero."""
+    gca, ca, gra, rawr, B, hw, na, nc, anchors, row_off, rows, cpad, rpad, dlc, dlr = args
+    dev = gen.device
+    gc, sc = io.seed(mem.at(gca, F32, (B, rows, nc))), io.seed(mem.at(ca, F32, (B, rows, nc)))
+    gr, raw = io.seed(mem.at(gra, F32, (B, rows, 4))), io.seed(mem.at(rawr, F32, (B, hw, na * 4)))
+    gc.copy_(torch.randn(gc.shape, generator=gen, device=dev))
+    sc.copy_(torch.rand(sc.shape, generator=gen, device=dev))
+    gr.copy_(torch.randn(gr.shape, generator=gen, device=dev))
+    raw.copy_(torch.randn(raw.shape, generator=gen, device=dev) * 2)
+    oc, orr = io.out(mem.at(dlc, BF16, (B, hw, cpad))), io.out(mem.at(dlr, BF16, (B, hw, rpad)))
+    io.freeze()
+    check(lib.yv6_head_ab_grad(h, *args, sp), lib)
+    torch.cuda.synchronize()
+    rows_of = lambda t, c: t[:, row_off:row_off + na * hw].reshape(B, na, hw, c).permute(0, 2, 1, 3)   # noqa: E731  [B, hw, na, c]
+    g, s = rows_of(gc, nc), rows_of(sc, nc)
+    exp_c = torch.zeros(B, hw, cpad, dtype=F32, device=dev)
+    exp_c[..., :na * nc] = ((g * s) * (1 - s)).reshape(B, hw, na * nc)
+    assert bits_equal(oc, exp_c.to(BF16)), "head_ab_grad: class columns"
+    g4 = rows_of(gr, 4).double()                                   # [B, hw, na, 4]
+    r4 = raw.view(B, hw, na, 4).double()
+    anc = torch.tensor(list(anchors), dtype=F64, device=dev).view(1, 1, na, 2)
+    sg = torch.sigmoid(r4[..., 2:])
+    wh = g4[..., 2:] * anc * 8 * sg * sg * (1 - sg)
+    got = orr[..., :na * 4].reshape(B, hw, na, 4)
+    assert bits_equal(got[..., :2], g4[..., :2].float().to(BF16)), "head_ab_grad: box offsets"
+    assert not bool(orr[..., na * 4:].any()), "head_ab_grad: padded channels"
+    return ratio(got[..., 2:], wh, BF16_ULP * wh.abs() + 2.0 ** -20 * (g4[..., 2:] * anc * 8).abs() * sg * sg)
+
+
+def check_pool_chain(lib, h, sp, eng, mem, calls, gen, io):
     """The three chained MaxPool2d(5, 1, 2) backward launches of one SPPF against torch's max-pool backward in float64 (scatter to
-    the first maximum in row-major window order), on operands quantised to a few levels so that ties are everywhere."""
+    the first maximum in row-major window order), on operands quantised to a few levels so that ties are everywhere.  Each
+    launch changes exactly the slice of its Write record; an assigning launch starts from the sentinel."""
     n, hh, ww, c = calls[0].args[4:8]
     bi = calls[0].writes[0].buf
     buf, gbuf = eng.bufs[bi], eng.gbufs[bi]
-    ys = [torch.randint(0, 4, (n, c, hh, ww), generator=gen).double()]
+    cg = torch.Generator().manual_seed(int(torch.randint(0, 1 << 30, (1,), generator=gen, device=gen.device)))
+    ys = [torch.randint(0, 4, (n, c, hh, ww), generator=cg).double()]
     for _ in range(3):
         ys.append(F.max_pool2d(ys[-1], 5, 1, 2))
     for j in range(4):
         buf[..., j * c:(j + 1) * c] = ys[j].permute(0, 2, 3, 1).to(BF16).to(buf.device)
-    prior = torch.randint(-3, 4, tuple(gbuf.shape), generator=gen).to(BF16)
-    gbuf.copy_(prior)
+    io.seed(buf)
+    prior = torch.randint(-3, 4, (n, hh, ww, 4 * c), generator=cg).to(BF16)
+    io.seed(gbuf[..., 3 * c:4 * c]).copy_(prior[..., 3 * c:])           # the incoming gradient of the last pooled slice
+    for call in calls:
+        w = call.writes[0]
+        assert w.full and w.n == c
+        if call.args[11]:            # accumulates: starts from a prior; an assigning launch starts from the sentinel
+            gbuf[..., w.off:w.off + c] = prior[..., w.off:w.off + c].to(gbuf.device)
+        io.out(mem.base(call.args[8]))
+    io.out(gbuf[..., :3 * c])
+    io.freeze()
     G = [nchw(prior[..., j * c:(j + 1) * c]) for j in range(4)]
     for call in calls:
-        d = call.args
-        j = call.writes[0].off // c + 1
+        d, w = call.args, call.writes[0]
+        j = w.off // c + 1
         assert d[0] == buf.data_ptr() + (j - 1) * c * 2 and d[2] == gbuf.data_ptr() + j * c * 2
+        before = gbuf.clone()
         check(lib.yv6_maxpool5_bwd(h, *d, sp), lib)
+        torch.cuda.synchronize()
+        keep = torch.ones(gbuf.shape[-1], dtype=torch.bool, device=gbuf.device)
+        keep[w.off:w.off + w.n] = False
+        assert torch.equal(int_view(gbuf[..., keep]), int_view(before[..., keep])), "pool_bwd wrote outside its Write record"
+        if not d[11]:
+            assert_full_write(gbuf[..., w.off:w.off + c], "pool_bwd")
         y = ys[j - 1].clone().requires_grad_(True)
         F.max_pool2d(y, 5, 1, 2).backward(G[j])
         G[j - 1] = (G[j - 1] * d[11] + y.grad).to(BF16).double()
-    torch.cuda.synchronize()
-    got = gbuf.cpu()
+    got = gbuf[..., :4 * c].cpu()
     exp = torch.cat([g.permute(0, 2, 3, 1) for g in G], -1)
-    r = ratio(got[..., :4 * c], exp, BF16_ULP * exp.abs())
-    assert bits_equal(got[..., 4 * c:], prior[..., 4 * c:])
-    return r
+    return ratio(got, exp, BF16_ULP * exp.abs())
 
 
 def im2col_ref(img, scale):
     """patches [N, Ho, Wo, 32] fp32: column (r*3+s)*3+c = x[n, c, 2ho+r-1, 2wo+s-1] (zero outside), columns 27..31 zero."""
-    x = img.float() * torch.tensor(scale, dtype=F32) if img.dtype == torch.uint8 else img.float()
+    x = img.float() * torch.tensor(scale, dtype=F32, device=img.device) if img.dtype == torch.uint8 else img.float()
     N, _, H, W = x.shape
     Ho, Wo = (H - 1) // 2 + 1, (W - 1) // 2 + 1
     xp = F.pad(x, (1, 1, 1, 1))
-    v = torch.zeros(N, Ho, Wo, 32, dtype=F32)
+    v = torch.zeros(N, Ho, Wo, 32, dtype=F32, device=img.device)
     for r in range(3):
         for s in range(3):
             for c in range(3):
@@ -398,31 +678,60 @@ def im2col_ref(img, scale):
     return hi, (v - hi.float()).to(BF16)
 
 
-def check_im2col(lib, h, sp, img_ptr, img_cpu, x_dt, scale, N, H, W, patches, patches_lo, gen):
-    patches.copy_(rnd(gen, *patches.shape))
-    patches_lo.copy_(rnd(gen, *patches_lo.shape))
+def check_im2col(lib, h, sp, img_ptr, img, x_dt, scale, N, H, W, patches, patches_lo, gen, io=None):
+    """Bit for bit.  With `io` (engine memory) the patches start from the sentinel, so every element must be written."""
+    if io is None:
+        patches.copy_(rnd(gen, *patches.shape).to(patches.device))
+        patches_lo.copy_(rnd(gen, *patches_lo.shape).to(patches.device))
+    else:
+        io.out(patches), io.out(patches_lo)
     check(lib.yv6_stem_im2col(h, img_ptr, x_dt, C.c_float(scale), N, H, W, patches.data_ptr(), patches_lo.data_ptr(), sp), lib)
     torch.cuda.synchronize()
-    hi, lo = im2col_ref(img_cpu, C.c_float(scale).value)
-    assert bits_equal(patches.cpu(), hi), "im2col: bf16 patches"
-    assert bits_equal(patches_lo.cpu(), lo), "im2col: bf16 residual plane"
+    hi, lo = im2col_ref(img, C.c_float(scale).value)
+    assert bits_equal(patches.to(hi.device), hi), "im2col: bf16 patches"
+    assert bits_equal(patches_lo.to(hi.device), lo), "im2col: bf16 residual plane"
     return 0.0
 
 
 # ---------------------------------------------------------------------------------------------------------------- the engine's launches
 @functools.lru_cache(maxsize=1)
 def _engine(name):
+    """The model's training engine, planned at the configuration's shape, and its master weights: the fabricated ones and
+    integers in [-2, 2] (use_weights repacks one set or the other)."""
     from yolov6_b200.model import build_model
-    size, batch = MODELS[name]
+    from yolov6_b200.synth import randomize_
+    c = MODELS[name]
+    size, batch, cfg, fuse_ab = c["size"], c["batch"], c["cfg"], c.get("fuse_ab", False)
     dev = torch.device("cuda:0")
-    m = build_model(name, 80, dev)
-    m.load_state_dict(fab.fabricate_state_dict(golden_keys(name), seed=0))
+    m = build_model(cfg, 80, dev, fuse_ab=fuse_ab)
+    if cfg in GOLDEN_KEYS:
+        m.load_state_dict(fab.fabricate_state_dict(golden_keys(cfg + ("_fuseab" if fuse_ab else "")), seed=0))
+    else:
+        randomize_(m, seed=0)
     m.train()
     eng = m.train_engine()
+    x = fab.synthetic_images(batch, size, size, seed=11)
+    if c.get("u8"):
+        x = (x * 255).round().to(torch.uint8)
     with torch.no_grad():
-        eng.forward(fab.synthetic_images(batch, size, size, seed=11).to(dev))     # plans the step, packs the weights
+        eng.forward(x.to(dev))                   # plans the step
+    gen = torch.Generator(device=dev).manual_seed(3)
+    fl = eng.flat.pflat
+    eng.weight_sets = {False: fl.clone(), True: torch.randint(-2, 3, fl.shape, generator=gen, device=dev).to(fl.dtype)}
+    eng.weights_now = False
     torch.cuda.synchronize()
-    return eng
+    return m, eng
+
+
+def use_weights(eng, integer):
+    """Master weights for the next checks: integers (exact passes) or the fabricated ones (real-valued passes, and the
+    BottleRep shortcut weight that bn_bwd reads from the parameter buffer); begin_step repacks them into the forward and
+    dgrad layouts and clears the zero arena, which is its rest state."""
+    if eng.weights_now is not integer:
+        eng.flat.pflat.copy_(eng.weight_sets[integer])
+        eng.begin_step()
+        torch.cuda.synchronize()
+        eng.weights_now = integer
 
 
 def engine_mem(eng):
@@ -434,7 +743,11 @@ def engine_mem(eng):
     named += [("dl", t) for t in sc.dl]
     named += [("patch", t) for t in getattr(eng, "_stem_patches", ())]
     named += [("raw", br["x"]) for ctx in eng.ctx if ctx and "branches" in ctx for br in ctx["branches"] if br["k"]]
-    named += [("param", eng.flat.pflat)]
+    named += [("qa_t", ctx["t"]) for ctx in eng.ctx if ctx and "t" in ctx]
+    if getattr(eng.g, "fuse_ab", False):
+        named += [("ab", t) for t in (eng.cls_ab, eng.reg_ab, eng.grad_cls_ab, eng.grad_reg_ab)]
+        named += [("ab_raw", raw) for st in eng._ab.values() for raw, _ in st.values()]
+    named += [("gflat", eng.flat.gflat), ("param", eng.flat.pflat)]
     return Mem(named)
 
 
@@ -455,22 +768,32 @@ def dgrad_weights(eng):
     return out
 
 
-KINDS = ("conv", "wgrad", "bn_bwd", "stats", "hgp", "pool_bwd", "im2col")
+def assert_write_view(eng, w, ptr, pitch, c, pixels, what):
+    """A launch's output view (ptr, channel pitch, C channels, pixels) is exactly the slice its Write record declares."""
+    g = eng.gbufs[w.buf]
+    assert ptr == g.data_ptr() + 2 * w.off and pitch == g.shape[3] and c == w.n, f"{what}: output view is not its Write record"
+    assert w.full and pixels == g.numel() // g.shape[3], f"{what}: a full Write over part of the pixels"
+
+
+KINDS = ("conv", "wgrad", "bn_bwd", "stats", "hgp", "pool_bwd", "im2col", "qa_bwd", "abg")
 
 
 @pytest.mark.parametrize("name", list(MODELS))
 def test_every_backward_launch_record_matches_float64_autograd(name):
     from yolov6_b200 import _lib
     from yolov6_b200._lib import DT_F32, DT_U8
-    eng = _engine(name)
+    t0 = time.time()
+    m, eng = _engine(name)
     lib, h, sp = eng.lib, eng.h, _lib.stream_ptr()
     mem = engine_mem(eng)
+    poison(mem)
     ops = eng.g.ops
-    gen = torch.Generator().manual_seed(20261015)
+    gen = torch.Generator(device="cuda").manual_seed(20261015)
     worst = {k: 0.0 for k in KINDS}
     bn_worst = {}
     seen = {k: set() for k in KINDS}
     total = {k: 0 for k in KINDS}
+    exact = {k: 0 for k in ("conv", "wgrad", "stats")}
 
     def first_time(kind, sig):
         total[kind] += 1
@@ -478,6 +801,12 @@ def test_every_backward_launch_record_matches_float64_autograd(name):
             return False
         seen[kind].add(sig)
         return True
+
+    def run(kind, what, fn):
+        io = IO()
+        r = fn(io)
+        settle(mem, io.ins, io.outs, f"{name}: {kind} {what}")
+        return r
 
     # dgrads: one group per (op, branch) or per dgrad weight; the four parity launches of a stride-2 3x3 conv together
     wmap = dgrad_weights(eng)
@@ -495,60 +824,98 @@ def test_every_backward_launch_record_matches_float64_autograd(name):
         gbuf = eng.gbufs[meta.buf]
         if not first_time("conv", tuple(signature(d, mem) for d in descs) + (tuple(gbuf.shape),)):
             continue
-        r = check_dgrad(lib, h, sp, mem, descs, wf, stride, gbuf, meta.off, meta.n, gen)
-        assert r <= 1.0, f"{ops[i].name}: dgrad error {r:.2f} x the bar ({len(descs)} launches)"
-        worst["conv"] = max(worst["conv"], r)
+        for ex in (False, True):
+            use_weights(eng, ex)
+            r = run("dgrad", ops[i].name, lambda io: check_dgrad(lib, h, sp, mem, descs, wf, stride, gbuf, meta, gen, io, ex))
+            assert r <= 1.0, f"{ops[i].name}: dgrad error {r:.2f} x the bar ({len(descs)} launches)"
+            worst["conv"] = max(worst["conv"], r)
+        exact["conv"] += 1
     for bi, calls in pools.items():
         assert len(calls) == 3
         if not first_time("pool_bwd", tuple(tuple(c.args) for c in calls)):
             continue
-        r = check_pool_chain(lib, h, sp, eng, calls, gen)
+        r = run("pool_bwd", bi, lambda io: check_pool_chain(lib, h, sp, eng, mem, calls, gen, io))
         assert r <= 1.0, f"pool backward of buffer {bi}: error {r:.2f} x the bar"
         worst["pool_bwd"] = max(worst["pool_bwd"], r)
     for c in eng.bwd_calls:
         kind, d = c.kind, c.desc
         if kind == "wgrad":
             if first_time(kind, signature(d, mem)):
-                r = check_wgrad(lib, h, sp, mem, d, gen)
-                assert r <= 1.0, f"wgrad {(d.N, d.H, d.W, d.Cin, d.Cout, d.kh, d.stride)}: error {r:.2f} x the bar"
-                worst[kind] = max(worst[kind], r)
+                for ex in (False, True):
+                    r = run(kind, (d.N, d.H, d.W, d.Cin, d.Cout, d.kh), lambda io: check_wgrad(lib, h, sp, mem, d, gen, io, ex))
+                    assert r <= 1.0, f"wgrad {(d.N, d.H, d.W, d.Cin, d.Cout, d.kh, d.stride)}: error {r:.2f} x the bar"
+                    worst[kind] = max(worst[kind], r)
+                exact[kind] += 1
         elif kind == "bn_bwd":
             if first_time(kind, signature(d, mem)):
-                out = check_bn_bwd(lib, h, sp, mem, d, gen)
+                for w in c.writes:          # identity-branch dx and the shortcut's dres: exactly their Write records
+                    dx_ptrs = [(d.dx[b], d.dx_pitch[b]) for b in range(d.nb) if d.dx[b] == eng.gbufs[w.buf].data_ptr() + 2 * w.off]
+                    ptr, pitch = dx_ptrs[0] if dx_ptrs else (d.dres, d.dres_pitch)
+                    assert_write_view(eng, w, ptr, pitch, d.C, d.pixels, f"bn_bwd launch {total[kind]}")
+                use_weights(eng, False)
+                out = run(kind, f"launch {total[kind]} (C={d.C}, nb={d.nb})", lambda io: check_bn_bwd(lib, h, sp, mem, d, gen, io=io))
                 for k, r in out.items():
                     bn_worst[k] = max(bn_worst.get(k, 0.0), r)
                     assert r <= 1.0, f"bn_bwd C={d.C} nb={d.nb} act={d.act} res={bool(d.res)}: {k} error {r:.2f} x the bar"
+        elif kind == "qa_bwd":
+            if first_time(kind, signature(d, mem)):
+                w, = c.writes
+                assert_write_view(eng, w, d.dx, d.dx_pitch, d.C, d.N * d.H * d.W, f"qa_bwd launch {total[kind]}")
+                r = run(kind, f"launch {total[kind]} (C={d.C})", lambda io: check_qa_bwd(lib, h, sp, mem, d, gen, io))
+                assert r <= 1.0, f"qa_bwd C={d.C}: error {r:.2f} x the bar"
+                worst[kind] = max(worst[kind], r)
         elif kind == "stats":
             if first_time(kind, signature(d, mem)):
-                r = check_stats_sums(lib, h, sp, mem, d, gen)
-                assert r <= 1.0, f"stats C={d.C} pixels={d.pixels}: error {r:.2f} x the bar"
-                worst[kind] = max(worst[kind], r)
+                for ex in (False, True):
+                    r = run(kind, (d.C, d.pixels), lambda io: check_stats_sums(lib, h, sp, mem, d, gen, io, ex))
+                    assert r <= 1.0, f"stats C={d.C} pixels={d.pixels}: error {r:.2f} x the bar"
+                    worst[kind] = max(worst[kind], r)
+                exact[kind] += 1
         elif kind == "hgp":
             if first_time(kind, (bool(c.args[1]),) + tuple(c.args[2:8])):
-                check_hgp(lib, h, sp, mem, c.args, gen)
+                run(kind, c.args[2:8], lambda io: check_hgp(lib, h, sp, mem, c.args, gen, io))
+        elif kind == "abg":
+            if first_time(kind, tuple(c.args[4:8]) + tuple(c.args[9:13])):
+                r = run(kind, c.args[4:8], lambda io: check_abg(lib, h, sp, mem, c.args, gen, io))
+                assert r <= 1.0, f"head_ab_grad: error {r:.2f} x the bar"
+                worst[kind] = max(worst[kind], r)
         elif kind == "im2col":
             if first_time(kind, tuple(c.args[1:6])):
                 x_ptr, x_dt, scale, N, H, W, pp, plo = c.args
-                assert x_dt == DT_F32 and x_ptr == eng.x_static.data_ptr()
+                img = eng.x_static
+                assert x_ptr == img.data_ptr() and x_dt == (DT_U8 if img.dtype == torch.uint8 else DT_F32)
                 patches, lo = eng._stem_patches
                 assert pp == patches.data_ptr() and plo == lo.data_ptr()
-                img = torch.rand(N, 3, H, W, generator=gen)
-                img[0, :, 0, :] = 1.0 / 3.0                          # values with a non-zero bf16 residual
-                eng.x_static.copy_(img)
-                check_im2col(lib, h, sp, x_ptr, img, x_dt, scale, N, H, W, patches, lo, gen)
-                img8 = torch.randint(0, 256, (N, 3, H, W), generator=gen, dtype=torch.uint8)
-                d8 = img8.cuda()
-                check_im2col(lib, h, sp, d8.data_ptr(), img8, DT_U8, scale, N, H, W, patches, lo, gen)
+
+                def im2col(io):
+                    if img.dtype == torch.uint8:
+                        img.copy_(torch.randint(0, 256, img.shape, generator=gen, device=img.device, dtype=torch.uint8))
+                        other = torch.rand(img.shape, generator=gen, device=img.device)
+                        other[0, :, 0, :] = 1.0 / 3.0                  # values with a non-zero bf16 residual
+                    else:
+                        img.copy_(torch.rand(img.shape, generator=gen, device=img.device))
+                        img[0, :, 0, :] = 1.0 / 3.0
+                        other = torch.randint(0, 256, img.shape, generator=gen, device=img.device, dtype=torch.uint8)
+                    check_im2col(lib, h, sp, x_ptr, img, x_dt, scale, N, H, W, patches, lo, gen, io)
+                    check_im2col(lib, h, sp, other.data_ptr(), other, DT_F32 if other.dtype == F32 else DT_U8, scale, N, H, W,
+                                 patches, lo, gen, io)
+                    return 0.0
+                run(kind, (N, H, W), im2col)
     worst["bn_bwd"] = max(bn_worst.values()) if bn_worst else 0.0
     kinds_made = {c.kind for c in eng.bwd_calls}
     for k in KINDS:
         if k in kinds_made:
             assert seen[k], f"no {k} launch checked"
-    print(f"\n{name}: distinct launches checked (of all in the plan): "
-          + ", ".join(f"{k} {len(seen[k])}/{total[k]}" for k in KINDS))
-    print(f"{name}: worst error / bar: " + ", ".join(f"{k} {worst[k]:.3f}" for k in KINDS if k not in ("hgp", "im2col"))
-          + " (hgp, im2col: bit-exact); bn_bwd by output: " + ", ".join(f"{k} {v:.3f}" for k, v in sorted(bn_worst.items())))
-
+    made = [k for k in KINDS if total[k]]
+    print(f"\n{name}: distinct launches checked (of all in the plan): " + ", ".join(f"{k} {len(seen[k])}/{total[k]}" for k in made))
+    print(f"{name}: exact integer passes (error 0): " + ", ".join(f"{k} {v}" for k, v in exact.items())
+          + "; worst error / bar of the real-valued passes: "
+          + ", ".join(f"{k} {worst[k]:.3f}" for k in made if k not in ("hgp", "im2col"))
+          + " (hgp, im2col: bit-exact); bn_bwd by output: " + ", ".join(f"{k} {v:.3f}" for k, v in sorted(bn_worst.items()))
+          + f"; {time.time() - t0:.1f} s")
+    del mem, eng, m
+    _engine.cache_clear()
+    torch.cuda.empty_cache()
 
 # ---------------------------------------------------------------------------------------------------------------- edges outside the engine's shapes
 @pytest.mark.parametrize("nb,ch,pixels,pitch_extra,zeroed", [

@@ -34,16 +34,21 @@ CASES = {
 def dry_engine(case):
     """A TrainEngine over a CPU model whose library, handle and streams are the recorder's stand-ins."""
     c = CASES[case]
-    cfg = configs.get_config(c["cfg"])
-    if c.get("distill_ns"):       # the N / S distillation student needs the DFL head
+    return dry_engine_of(c["cfg"], N_BUCKETS, fuse_ab=c.get("fuse_ab", False), distill_ns=c.get("distill_ns", False),
+                         external_feat_grads=bool(c.get("external_feat_grads")))
+
+
+def dry_engine_of(cfg_name, n_buckets, fuse_ab=False, distill_ns=False, external_feat_grads=False):
+    cfg = configs.get_config(cfg_name)
+    if distill_ns:                # the N / S distillation student needs the DFL head
         cfg["head"]["use_dfl"], cfg["head"]["reg_max"] = True, 16
-    m = build_model(cfg, 80, torch.device("cpu"), fuse_ab=c.get("fuse_ab", False), distill_ns=c.get("distill_ns", False)).train()
+    m = build_model(cfg, 80, torch.device("cpu"), fuse_ab=fuse_ab, distill_ns=distill_ns).train()
     eng = TrainEngine.__new__(TrainEngine)
     eng.model, eng.g, eng.dev = m, m.graph, torch.device("cpu")
-    eng.n_buckets = N_BUCKETS
+    eng.n_buckets = n_buckets
     eng.debug, eng.dbg, eng._shape, eng.bucket_hook = False, {}, None, None
     eng.overlap_wgrad, eng._wg_stream = True, None
-    eng.external_feat_grads, eng._feat_grads = bool(c.get("external_feat_grads")), None
+    eng.external_feat_grads, eng._feat_grads = external_feat_grads, None
     eng._build_state()
     rec = Recorder(eng)
     eng.lib, eng.h = FakeLib(rec), rec.handle

@@ -201,6 +201,7 @@ _SIGNATURES = {
     "yv6_det_loss_workspace_bytes": (C.c_int64, [C.c_int32, C.c_int32]),
     "yv6_det_loss": (C.c_int, [C.c_void_p, C.POINTER(LossDesc), C.c_void_p]),
     "yv6_conv_wgrad": (C.c_int, [C.c_void_p, C.POINTER(WgradDesc), C.c_void_p]),
+    "yv6_wgrad_plan_host": (C.c_int, [C.c_int, C.c_int, C.POINTER(WgradDesc), C.POINTER(C.c_int32)]),
     "yv6_bn_stats": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]),
     "yv6_bn_finalize": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_double, C.c_void_p, C.c_void_p, C.c_float, C.c_float,
                                   C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]),

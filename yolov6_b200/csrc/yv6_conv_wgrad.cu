@@ -23,6 +23,7 @@ namespace yv6 {
 
 constexpr int kWgThreads = 384;
 constexpr int kWgMaxStages = 8;
+constexpr int kWgFixedSmem = 1024 /* alignment */ + 512 /* barriers */;
 
 struct WgParams {
   int32_t BW, BH, PT;                 // pixel box, BW*BH == PT (128 or 64): the K extent of one pipeline stage
@@ -182,15 +183,13 @@ static const WgradKernelFn kWgradKernels[4][2] = {{conv_wgrad_kernel<16, 1>, con
                                                   {conv_wgrad_kernel<64, 1>, conv_wgrad_kernel<64, 3>},
                                                   {conv_wgrad_kernel<128, 1>, nullptr}};
 
-extern "C" int yv6_conv_wgrad(yv6_handle* h, const yv6_wgrad_desc* d, void* stream) {
-  yv6_device_guard _dev(h);
-  YV6_REQUIRE(h && d && d->x && d->dy && d->dw, "wgrad: null argument");
-  YV6_REQUIRE(h->encode_tiled != nullptr, "wgrad: cuTensorMapEncodeTiled unavailable");
+// The launch plan of one weight gradient on a device with `num_sms` SMs and `max_smem_optin` bytes of opt-in shared memory:
+// tile shapes, pipeline depth and the split-K over pixel ranges.  Shared by yv6_conv_wgrad and yv6_wgrad_plan_host.
+static int plan_wgrad(int num_sms, int max_smem_optin, const yv6_wgrad_desc* d, WgParams& p) {
   YV6_REQUIRE(d->Cin > 0 && d->Cin % 16 == 0 && d->x_c_total % 8 == 0 && d->dy_c_total % 8 == 0, "wgrad: channel counts");
   YV6_REQUIRE(d->kh == d->kw && (d->kh == 1 || d->kh == 3), "wgrad: kernel %dx%d unsupported", d->kh, d->kw);
   YV6_REQUIRE(d->stride == 1 || d->stride == 2, "wgrad: stride %d", d->stride);
   const int Ho = (d->H + 2 * d->pad - d->kh) / d->stride + 1, Wo = (d->W + 2 * d->pad - d->kw) / d->stride + 1;
-  WgParams p;
   memset(&p, 0, sizeof(p));
   p.Cout = d->Cout; p.Cin = d->Cin; p.stride = d->stride; p.pad = d->pad;
   p.taps = d->kh * d->kw; p.kw = d->kw;
@@ -223,8 +222,7 @@ extern "C" int yv6_conv_wgrad(yv6_handle* h, const yv6_wgrad_desc* d, void* stre
   p.a_stage_bytes = p.a_loaded * p.PT * 128;
   p.b_tap_bytes = ((p.b_blocks * p.PT * p.b_blk_bytes + 1023) / 1024) * 1024;
   p.b_stage_bytes = p.T * p.b_tap_bytes;
-  const int fixed = 1024 /* alignment */ + 512 /* barriers */;
-  const int budget = h->max_smem_optin - fixed;
+  const int budget = max_smem_optin - kWgFixedSmem;
   p.stages = std::min(kWgMaxStages, budget / (p.a_stage_bytes + p.b_stage_bytes));
   YV6_REQUIRE(p.stages >= 2, "wgrad: not enough shared memory");
   const int base_units = p.co_tiles * p.ci_tiles * p.tap_groups;
@@ -233,9 +231,39 @@ extern "C" int yv6_conv_wgrad(yv6_handle* h, const yv6_wgrad_desc* d, void* stre
   // a multiple of the SM count costs a whole extra wave -- with at least ~8 stages of work each (every extra split adds a
   // pass of fp32 reductions over the weight tensor)
   const int min_tiles = 8 * 128 / p.PT;
-  p.ksplit = std::max(1, std::min((p.ptiles + min_tiles - 1) / min_tiles, std::max(1, 2 * h->num_sms / base_units)));
+  p.ksplit = std::max(1, std::min((p.ptiles + min_tiles - 1) / min_tiles, std::max(1, 2 * num_sms / base_units)));
   if (d->force_ksplit > 0) p.ksplit = std::min(p.ptiles, d->force_ksplit);
-  const int units = base_units * p.ksplit;
+  return YV6_OK;
+}
+
+extern "C" int yv6_wgrad_plan_host(int num_sms, int max_smem_optin, const yv6_wgrad_desc* d, int32_t* out10) {
+  YV6_REQUIRE(d != nullptr && out10 != nullptr, "wgrad_plan_host: null argument");
+  YV6_REQUIRE(num_sms > 0 && max_smem_optin > 0, "wgrad_plan_host: bad device properties");
+  WgParams p;
+  const int rc = plan_wgrad(num_sms, max_smem_optin, d, p);
+  if (rc != YV6_OK) return rc;
+  const int per = (p.ptiles + p.ksplit - 1) / p.ksplit;
+  out10[0] = p.NT;
+  out10[1] = p.T;
+  out10[2] = p.PT;
+  out10[3] = p.BW;
+  out10[4] = p.BH;
+  out10[5] = p.ptiles;
+  out10[6] = p.ksplit;
+  out10[7] = per * p.PT;
+  out10[8] = p.co_tiles * p.ci_tiles * p.tap_groups * p.ksplit;
+  out10[9] = p.stages * (p.a_stage_bytes + p.b_stage_bytes) + kWgFixedSmem;
+  return YV6_OK;
+}
+
+extern "C" int yv6_conv_wgrad(yv6_handle* h, const yv6_wgrad_desc* d, void* stream) {
+  yv6_device_guard _dev(h);
+  YV6_REQUIRE(h && d && d->x && d->dy && d->dw, "wgrad: null argument");
+  YV6_REQUIRE(h->encode_tiled != nullptr, "wgrad: cuTensorMapEncodeTiled unavailable");
+  WgParams p;
+  { const int rc = plan_wgrad(h->num_sms, h->max_smem_optin, d, p); if (rc != YV6_OK) return rc; }
+  const int Ho = (d->H + 2 * d->pad - d->kh) / d->stride + 1, Wo = (d->W + 2 * d->pad - d->kw) / d->stride + 1;
+  const int units = p.co_tiles * p.ci_tiles * p.tap_groups * p.ksplit;
 
   CUtensorMap tmDY, tmX;
   {
@@ -269,7 +297,7 @@ extern "C" int yv6_conv_wgrad(yv6_handle* h, const yv6_wgrad_desc* d, void* stre
           YV6_CHECK_CUDA(cudaFuncSetAttribute(kWgradKernels[i][j], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->max_smem_optin));
     h->configured |= YV6_CFG_WGRAD;
   }
-  const size_t smem = (size_t)p.stages * (p.a_stage_bytes + p.b_stage_bytes) + fixed;
+  const size_t smem = (size_t)p.stages * (p.a_stage_bytes + p.b_stage_bytes) + kWgFixedSmem;
   const int nt_idx = p.NT == 16 ? 0 : p.NT == 32 ? 1 : p.NT == 64 ? 2 : 3;
   kWgradKernels[nt_idx][p.T == 3 ? 1 : 0]<<<units, kWgThreads, smem, (cudaStream_t)stream>>>(tmDY, tmX, p);
   YV6_CHECK_CUDA(cudaGetLastError());
