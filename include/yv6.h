@@ -287,13 +287,31 @@ int yv6_pr_metric(yv6_handle* h, const yv6_pr_state* st, int32_t n_images, const
  *   (core/inferer.py:161-171) -> dst uint8 NCHW [B,3,H,W] (the stem's YV6_DT_U8 input; the 1/255 stays in the stem).
  *   Canvas outside [top, top+nh) x [left, left+nw) = 114; inside, cv2.resize INTER_LINEAR of the uint8 source, bit-exact,
  *   or a plain copy when (nh, nw) == (h0, w0).  A slot with nh = 0 is all border.  W % 16 == 0, dst 16-byte aligned.
+ * yv6_letterbox_frames: the same canvases, but image b is read through srcs[b] (device [B] yv6_lb_src) instead of
+ *   src + src_off, so each image may lie anywhere in device memory (a decoder's output, a crop view of a larger frame, a
+ *   staging buffer) in either layout below; geo supplies everything else and its src_off is ignored.  The layout is data,
+ *   so one captured graph serves any mix of layouts and frame locations.  Pitches are in bytes:
+ *     YV6_LB_BGR_HWC  pixel (y, x) channel c (B, G, R) at base + y * row_pitch + x * 3 + c; plane_pitch unused (cv2 imread);
+ *     YV6_LB_RGB_CHW  pixel (y, x) channel c (R, G, B) at base + c * plane_pitch + y * row_pitch + x (torchvision decoders).
+ *   Canvas plane c reads source channel 2 - c of BGR HWC and source plane c of RGB CHW, so both give the canvas yv6_letterbox
+ *   gives for the equivalent BGR HWC image.  A slot with nh = 0 reads nothing (its record may hold a null base).
  * yv6_rescale_boxes: Inferer.rescale((H, W), det[:, :4], (h0, w0)) followed by .round() (inferer.py:103, 173-188) on the
  *   NMS output det [B,max_det,6] / count [B] -> out [B,max_det,6] (x1, y1, x2, y2 in source pixels, conf, cls), rows
  *   beyond count[b] zeroed.  Reads h0, w0 of geo.  Ratio and padding are the reference's doubles, box math its fp32.
  * ---------------------------------------------------------------------------------------------- */
 #define YV6_LB_GEO 8
+enum { YV6_LB_BGR_HWC = 0, YV6_LB_RGB_CHW = 1 };
+typedef struct {
+  const uint8_t* base;         /* pixel (0, 0) of the image's first channel                                   */
+  int64_t row_pitch;           /* bytes from one image row to the next                                        */
+  int64_t plane_pitch;         /* bytes from one channel plane to the next (YV6_LB_RGB_CHW)                   */
+  int32_t layout;              /* YV6_LB_BGR_HWC or YV6_LB_RGB_CHW                                            */
+  int32_t reserved0;
+} yv6_lb_src;
 int yv6_letterbox(yv6_handle* h, const uint8_t* src, const int32_t* geo, int32_t B, int32_t H, int32_t W, uint8_t* dst,
                   void* stream);
+int yv6_letterbox_frames(yv6_handle* h, const yv6_lb_src* srcs, const int32_t* geo, int32_t B, int32_t H, int32_t W, uint8_t* dst,
+                         void* stream);
 int yv6_rescale_boxes(yv6_handle* h, const float* det, const int32_t* count, const int32_t* geo, int32_t B, int32_t max_det,
                       int32_t H, int32_t W, float* out, void* stream);
 

@@ -154,6 +154,14 @@ class QaDesc(C.Structure):
     ]
 
 
+class LbSrc(C.Structure):
+    """Mirror of `yv6_lb_src` (include/yv6.h): where one image of yv6_letterbox_frames lies and in which layout."""
+    _fields_ = [
+        ("base", C.c_void_p), ("row_pitch", C.c_int64), ("plane_pitch", C.c_int64), ("layout", C.c_int32), ("reserved0", C.c_int32),
+    ]
+
+
+LB_BGR_HWC, LB_RGB_CHW = 0, 1
 XF_F32, XF_F64, XF_BF16 = 0, 1, 2
 XFORM_CHUNK = 4096
 
@@ -219,6 +227,7 @@ _SIGNATURES = {
                                        C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
     "yv6_eval_boxes": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
     "yv6_letterbox": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
+    "yv6_letterbox_frames": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
     "yv6_rescale_boxes": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                     C.c_void_p, C.c_void_p]),
     "yv6_aug_resize": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int64, C.c_void_p]),

@@ -1,6 +1,8 @@
 // yv6_letterbox.cu -- the image side of the reference's Inferer around the model, for a whole batch per launch:
 //   yv6_letterbox:      letterbox (yolov6/data/data_augment.py:29-58, auto=False) + HWC->CHW + BGR->RGB of
 //                       Inferer.process_image (core/inferer.py:161-171); the 1/255 stays in the stem kernel.
+//   yv6_letterbox_frames: the same canvases from images anywhere in device memory, each addressed by a yv6_lb_src record
+//                       (BGR HWC with padded rows, or RGB CHW as torchvision's decoders return it).
 //   yv6_rescale_boxes:  Inferer.rescale (core/inferer.py:173-188) followed by the `.round()` of inferer.py:103.
 //
 // Resampling is OpenCV's uint8 INTER_LINEAR path of cv2.resize, reproduced bit for bit:
@@ -24,37 +26,52 @@ namespace yv6 {
 constexpr int kLbPix = 16;     // output pixels per thread: one 16-byte store into each channel plane
 
 // geo [B][YV6_LB_GEO] = (src_off, h0, w0, nh, nw, top, left, 0); thread = 16 consecutive pixels of one canvas row.
-__global__ void __launch_bounds__(256) letterbox_kernel(const uint8_t* __restrict__ src, const int32_t* __restrict__ geo, int H, int W,
-                                                        uint8_t* __restrict__ dst) {
+// Image b is read through srcs[b] (yv6_letterbox_frames) or, when srcs is null, as packed BGR HWC at packed + src_off
+// (yv6_letterbox): one sampling routine for both entry points, only the address of a tap depends on the record.
+__global__ void __launch_bounds__(256) letterbox_kernel(const yv6_lb_src* __restrict__ srcs, const uint8_t* __restrict__ packed,
+                                                        const int32_t* __restrict__ geo, int H, int W, uint8_t* __restrict__ dst) {
   const int b = blockIdx.y;
   const int per_row = W / kLbPix;
   const int q = blockIdx.x * blockDim.x + threadIdx.x;
   if (q >= H * per_row) return;
   const int y = q / per_row, x0 = (q - y * per_row) * kLbPix;
   const int32_t* g = geo + b * YV6_LB_GEO;
-  const int off = __ldg(g + 0), h0 = __ldg(g + 1), w0 = __ldg(g + 2), nh = __ldg(g + 3), nw = __ldg(g + 4), top = __ldg(g + 5),
-            left = __ldg(g + 6);
-  const uint8_t* im = src + off;
+  const int h0 = __ldg(g + 1), w0 = __ldg(g + 2), nh = __ldg(g + 3), nw = __ldg(g + 4), top = __ldg(g + 5), left = __ldg(g + 6);
+  const uint8_t* im;
+  int64_t row_pitch, plane_pitch;
+  int layout;
+  if (srcs) {
+    const yv6_lb_src s = srcs[b];
+    im = s.base, row_pitch = s.row_pitch, plane_pitch = s.plane_pitch, layout = s.layout;
+  } else {
+    im = packed + __ldg(g + 0), row_pitch = (int64_t)w0 * 3, plane_pitch = 0, layout = YV6_LB_BGR_HWC;
+  }
+  // canvas channel c (R, G, B) of pixel x lies at row + x * px + ch[c]: BGR HWC reads channel 2 - c, RGB CHW plane c
+  const bool chw = layout == YV6_LB_RGB_CHW;
+  const int px = chw ? 1 : 3;
+  int64_t ch[3];
+#pragma unroll
+  for (int c = 0; c < 3; ++c) ch[c] = chw ? c * plane_pitch : 2 - c;
   alignas(16) uint8_t o[3][kLbPix];
   const int ys = y - top;
   if (ys < 0 || ys >= nh) {
 #pragma unroll
     for (int i = 0; i < kLbPix; ++i) o[0][i] = o[1][i] = o[2][i] = 114;
   } else if (nh == h0 && nw == w0) {           // data_augment.py:52: no resize, a plain copy
-    const uint8_t* row = im + (int64_t)ys * w0 * 3;
+    const uint8_t* row = im + (int64_t)ys * row_pitch;
 #pragma unroll
     for (int i = 0; i < kLbPix; ++i) {
       const int xs = x0 + i - left;
       const bool in = xs >= 0 && xs < nw;
 #pragma unroll
-      for (int c = 0; c < 3; ++c) o[c][i] = in ? __ldg(row + xs * 3 + 2 - c) : (uint8_t)114;
+      for (int c = 0; c < 3; ++c) o[c][i] = in ? __ldg(row + ch[c] + xs * px) : (uint8_t)114;
     }
   } else {
     const double sy_scale = lin_scale(nh, h0);
     const double sx_scale = lin_scale(nw, w0);
     const LinTap v = lin_tap(ys, sy_scale, h0, false);
-    const uint8_t* r0 = im + (int64_t)v.s0 * w0 * 3;
-    const uint8_t* r1 = im + (int64_t)v.s1 * w0 * 3;
+    const uint8_t* r0 = im + (int64_t)v.s0 * row_pitch;
+    const uint8_t* r1 = im + (int64_t)v.s1 * row_pitch;
 #pragma unroll
     for (int i = 0; i < kLbPix; ++i) {
       const int xs = x0 + i - left;
@@ -64,7 +81,7 @@ __global__ void __launch_bounds__(256) letterbox_kernel(const uint8_t* __restric
       }
       const LinTap hz = lin_tap(xs, sx_scale, w0, true);
 #pragma unroll
-      for (int c = 0; c < 3; ++c) o[c][i] = lin_pixel(r0, r1, v, hz, 2 - c);      // BGR -> RGB
+      for (int c = 0; c < 3; ++c) o[c][i] = lin_pixel(r0 + ch[c], r1 + ch[c], v, hz, 0, px);
     }
   }
   const int64_t plane = (int64_t)H * W;
@@ -104,16 +121,28 @@ __global__ void rescale_boxes_kernel(const float* __restrict__ det, const int32_
 
 using namespace yv6;
 
+static int launch_letterbox(const yv6_lb_src* srcs, const uint8_t* packed, const int32_t* geo, int32_t B, int32_t H, int32_t W,
+                            uint8_t* dst, void* stream) {
+  YV6_REQUIRE(W % kLbPix == 0 && ((uintptr_t)dst & 15) == 0, "letterbox: W (%d) must be a multiple of 16 and dst 16-byte aligned", W);
+  YV6_REQUIRE(B <= 65535, "letterbox: batch %d too large", B);
+  const int chunks = H * (W / kLbPix);
+  letterbox_kernel<<<dim3((chunks + 255) / 256, B), 256, 0, (cudaStream_t)stream>>>(srcs, packed, geo, H, W, dst);
+  YV6_CHECK_CUDA(cudaGetLastError());
+  return YV6_OK;
+}
+
 extern "C" int yv6_letterbox(yv6_handle* h, const uint8_t* src, const int32_t* geo, int32_t B, int32_t H, int32_t W, uint8_t* dst,
                              void* stream) {
   yv6_device_guard _dev(h);
   YV6_REQUIRE(h && src && geo && dst && B > 0 && H > 0 && W > 0, "letterbox: bad argument");
-  YV6_REQUIRE(W % kLbPix == 0 && ((uintptr_t)dst & 15) == 0, "letterbox: W (%d) must be a multiple of 16 and dst 16-byte aligned", W);
-  YV6_REQUIRE(B <= 65535, "letterbox: batch %d too large", B);
-  const int chunks = H * (W / kLbPix);
-  letterbox_kernel<<<dim3((chunks + 255) / 256, B), 256, 0, (cudaStream_t)stream>>>(src, geo, H, W, dst);
-  YV6_CHECK_CUDA(cudaGetLastError());
-  return YV6_OK;
+  return launch_letterbox(nullptr, src, geo, B, H, W, dst, stream);
+}
+
+extern "C" int yv6_letterbox_frames(yv6_handle* h, const yv6_lb_src* srcs, const int32_t* geo, int32_t B, int32_t H, int32_t W,
+                                    uint8_t* dst, void* stream) {
+  yv6_device_guard _dev(h);
+  YV6_REQUIRE(h && srcs && geo && dst && B > 0 && H > 0 && W > 0, "letterbox_frames: bad argument");
+  return launch_letterbox(srcs, nullptr, geo, B, H, W, dst, stream);
 }
 
 extern "C" int yv6_rescale_boxes(yv6_handle* h, const float* det, const int32_t* count, const int32_t* geo, int32_t B, int32_t max_det,

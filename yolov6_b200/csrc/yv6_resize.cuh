@@ -1,7 +1,8 @@
 // yv6_resize.cuh -- one axis of OpenCV's uint8 INTER_LINEAR cv2.resize, shared by yv6_letterbox.cu and yv6_augment.cu.
 // The rule (see yv6_letterbox.cu for why each part matters): source coordinate in double from the inverted inverse scale,
 // 11-bit coefficients, horizontal border taps clamped with a zero fraction, vertical rows clamped with the unreset fraction,
-// and the truncating vertical pass of OpenCV's SIMD kernel.
+// and the truncating vertical pass of OpenCV's SIMD kernel.  Every channel is resized on its own, so the layout of the
+// channels changes only the address of a tap.
 #pragma once
 #include <cstdint>
 
@@ -31,10 +32,12 @@ __device__ __forceinline__ LinTap lin_tap(int d, double scale, int src, bool res
 // cv::resize keeps the inverse scale and inverts it: the per-axis scale of an n0 -> n resize.
 __device__ __forceinline__ double lin_scale(int n, int n0) { return __ddiv_rn(1.0, __ddiv_rn((double)n, (double)n0)); }
 
-// One channel of the resized pixel from the two vertical taps' rows r0, r1 (uint8 HWC, 3 channels) and horizontal tap hz.
-__device__ __forceinline__ uint8_t lin_pixel(const uint8_t* r0, const uint8_t* r1, const LinTap& v, const LinTap& hz, int ch) {
-  const int S0 = __ldg(r0 + hz.s0 * 3 + ch) * hz.c0 + __ldg(r0 + hz.s1 * 3 + ch) * hz.c1;
-  const int S1 = __ldg(r1 + hz.s0 * 3 + ch) * hz.c0 + __ldg(r1 + hz.s1 * 3 + ch) * hz.c1;
+// One channel of the resized pixel from the two vertical taps' rows r0, r1 and horizontal tap hz: the channel's byte of
+// pixel x lies at r + x * px + ch (px = 3 for uint8 HWC with 3 channels, px = 1 for one plane of CHW).
+__device__ __forceinline__ uint8_t lin_pixel(const uint8_t* r0, const uint8_t* r1, const LinTap& v, const LinTap& hz, int ch,
+                                             int px = 3) {
+  const int S0 = __ldg(r0 + hz.s0 * px + ch) * hz.c0 + __ldg(r0 + hz.s1 * px + ch) * hz.c1;
+  const int S1 = __ldg(r1 + hz.s0 * px + ch) * hz.c0 + __ldg(r1 + hz.s1 * px + ch) * hz.c1;
   const int t = (((v.c0 * (S0 >> 4)) >> 16) + ((v.c1 * (S1 >> 4)) >> 16) + 2) >> 2;
   return (uint8_t)min(max(t, 0), 255);
 }

@@ -12,16 +12,24 @@ stream instead: with two pipelines used alternately (see `DetectRing`) the copy 
 copy engine while the kernels of batch i run on the SMs, so a serving loop is bound by max(copy, compute)
 instead of their sum.
 
-`raw_input=True` serves decoded frames (OpenCV `imread` layout: uint8 HWC BGR, any size, sizes mixed freely within a batch) instead
-of letterboxed batches: the frames' bytes and a per-image geometry table go through a fixed-capacity pinned staging buffer
-(`max_src_bytes`) and are copied to the device on the copy stream, and the graph runs letterbox -> network -> NMS -> rescale
--> D2H (`yolov6_b200.preprocess`).  Results are per-image [k, 6] rows in source pixels, what `Inferer.infer` holds in `det` after
-core/inferer.py:103.  The geometry is data, so one captured graph serves any mix of image sizes.
+`raw_input=True` serves decoded frames (any size, sizes mixed freely within a batch) instead of letterboxed batches, in OpenCV's
+`imread` layout (uint8 HWC BGR, `layout="bgr_hwc"`, the default) or torchvision's decoders' (uint8 RGB CHW, `layout="rgb_chw"`).
+A host frame (numpy array or CPU tensor) goes through a fixed-capacity pinned staging buffer (`max_src_bytes`, host frames
+only) that is copied to the device on the copy stream; a CUDA tensor on the pipeline's device is read in place.  Per-image
+source records and geometry go up on the copy stream too, and the graph runs letterbox -> network -> NMS -> rescale -> D2H
+(`yolov6_b200.preprocess`).  Results are per-image [k, 6] rows in source pixels, what `Inferer.infer` holds in `det` after
+core/inferer.py:103.  Records and geometry are data, so one captured graph serves any mix of image sizes, layouts and
+locations.
+
+Device frames are read in stream order: the copy stream waits for the work enqueued on the caller's current stream before
+the call, so frames a kernel wrote there are complete when the graph reads them.  They are read in place, so the caller
+must not write to them until `collect()` has returned their batch (`DetectPipeline.__call__` returns after the batch is
+done); the pipeline keeps a reference to them until then, so dropping them early is safe.
 """
 import torch
 
 from .nms import nms_batched_head, workspace_bytes
-from .preprocess import GEO, letterbox_launch, pack_frames, rescale_launch
+from .preprocess import GEO, REC, check_frames, letterbox_frames_launch, pack_sources, rescale_launch
 
 RAW_DEFAULT_BYTES = 1920 * 1080 * 3        # staging bytes per batch slot when max_src_bytes is not given: one 1080p frame each
 
@@ -30,16 +38,27 @@ def raw_buffers(batch, height, width, max_det, max_src_bytes, dev):
     """Pinned staging + device buffers of one raw-frame slot."""
     cap = int(max_src_bytes) if max_src_bytes else batch * RAW_DEFAULT_BYTES
     geo = torch.tensor([[0, height, width, 0, 0, 0, 0, 0]] * batch, dtype=torch.int32)     # all border until frames arrive
-    return dict(src_host=torch.empty(cap, dtype=torch.uint8).pin_memory(), geo_host=geo.pin_memory(),
-                src_dev=torch.zeros(cap, dtype=torch.uint8, device=dev), geo_dev=geo.to(dev), res_geo=geo.to(dev),
-                res=torch.zeros(batch, max_det, 6, device=dev), nbytes=0)
+    rec = torch.zeros(batch * REC, dtype=torch.uint8)          # null records: an all-border slot reads no source
+    return dict(src_host=torch.empty(cap, dtype=torch.uint8).pin_memory(), geo_host=geo.pin_memory(), rec_host=rec.pin_memory(),
+                src_dev=torch.zeros(cap, dtype=torch.uint8, device=dev), geo_dev=geo.to(dev), rec_dev=rec.to(dev), res_geo=geo.to(dev),
+                res=torch.zeros(batch, max_det, 6, device=dev), nbytes=0, frames=[])
+
+
+def raw_pack(slot, frames, height, width, layout, dev):
+    """Validate 1..B frames and lay them out in one raw-frame slot's host tables; RuntimeError before anything is written
+    when a frame is unusable.  Returns the device frames (read in place by the slot's next launch)."""
+    srcs = check_frames(frames, slot["geo_host"].shape[0], layout, dev)
+    slot["nbytes"], _, devs = pack_sources(srcs, slot["geo_host"].shape[0], height, width, True, layout, slot["src_host"],
+                                           slot["geo_host"], slot["rec_host"], slot["src_dev"].data_ptr())
+    return devs
 
 
 def raw_h2d(slot):
-    """Copy the used staging bytes and the geometry of one raw-frame slot to the device (current stream)."""
+    """Copy the used staging bytes, the source records and the geometry of one raw-frame slot to the device (current stream)."""
     n = slot["nbytes"]
     if n:
         slot["src_dev"][:n].copy_(slot["src_host"][:n], non_blocking=True)
+    slot["rec_dev"].copy_(slot["rec_host"], non_blocking=True)
     slot["geo_dev"].copy_(slot["geo_host"], non_blocking=True)
 
 
@@ -52,7 +71,7 @@ class DetectPipeline:
         if self.dev.type != "cuda":
             raise RuntimeError("DetectPipeline needs a CUDA model")
         if raw_input and not host_input:
-            raise RuntimeError("DetectPipeline: raw_input takes host frames (host_input=True)")
+            raise RuntimeError("DetectPipeline: raw_input returns detections in host memory (host_input=True)")
         self.kw = dict(conf_thres=conf_thres, iou_thres=iou_thres, classes=classes, agnostic=agnostic,
                        multi_label=multi_label, max_det=max_det)
         self.host_input = host_input
@@ -63,6 +82,8 @@ class DetectPipeline:
             self.copy_stream = copy_stream or torch.cuda.Stream(device=self.dev)
             self.ev_copied = torch.cuda.Event()
             self.ev_done = torch.cuda.Event()
+            self.ev_ready = torch.cuda.Event()
+            self._ready = None       # event the next copy waits for: the caller's stream when device frames were given
             self._used = False
         dt = torch.uint8 if host_input else torch.float32
         self.x_dev = torch.zeros(batch, 3, height, width, dtype=dt, device=self.dev)
@@ -80,7 +101,7 @@ class DetectPipeline:
 
     def _body(self):
         if self.raw:
-            letterbox_launch(self.raw["src_dev"], self.raw["geo_dev"], self.x_dev)
+            letterbox_frames_launch(self.raw["rec_dev"], self.raw["geo_dev"], self.x_dev)
         elif self.host_input and not self.overlap_h2d:
             self.x_dev.copy_(self.x_host, non_blocking=True)
         # the [B, A, 5+nc] prediction tensor of Detect.forward (effidehead.py:131-139) is never materialised here: the NMS
@@ -113,6 +134,9 @@ class DetectPipeline:
             cur = torch.cuda.current_stream(self.dev)
             if self._used:
                 self.copy_stream.wait_event(self.ev_done)      # the previous batch of THIS pipeline is done with x_dev
+            if self._ready is not None:
+                self.copy_stream.wait_event(self._ready)       # the producer of the device frames
+                self._ready = None
             with torch.cuda.stream(self.copy_stream):
                 if self.raw:
                     raw_h2d(self.raw)
@@ -126,14 +150,18 @@ class DetectPipeline:
             return
         self.graph.replay()
 
-    def __call__(self, images=None):
-        """images: uint8 [B,3,H,W] host tensor (host_input) or fp32 device tensor; with raw_input, a list of 1..B uint8 HWC BGR
-        frames (numpy arrays or CPU tensors).  Returns the list of per-image [k,6] detections (host tensors when host_input)
-        like `non_max_suppression`; with raw_input in source pixels, rounded (Inferer.rescale(...).round())."""
+    def __call__(self, images=None, layout="bgr_hwc"):
+        """images: uint8 [B,3,H,W] host tensor (host_input) or fp32 device tensor; with raw_input, a list of 1..B uint8 frames
+        in `layout` (see the module docstring), each a numpy array, a CPU tensor or a CUDA tensor on the pipeline's device.
+        Returns the list of per-image [k,6] detections (host tensors when host_input) like `non_max_suppression`; with
+        raw_input in source pixels, rounded (Inferer.rescale(...).round())."""
+        devs = None          # device frames of this batch, referenced until the batch is done
         if images is not None:
             if self.raw:
-                self.raw["nbytes"], _ = pack_frames(images, self.x_dev.shape[0], self.x_dev.shape[2], self.x_dev.shape[3], True,
-                                                    self.raw["src_host"], self.raw["geo_host"])
+                devs = raw_pack(self.raw, images, self.x_dev.shape[2], self.x_dev.shape[3], layout, self.dev)
+                if devs:
+                    self.ev_ready.record(torch.cuda.current_stream(self.dev))
+                    self._ready = self.ev_ready
                 self.n_frames = len(images)
             else:
                 (self.x_host if self.host_input else self.x_dev).copy_(images)
@@ -198,8 +226,9 @@ class DetectStream:
     host_input=True: uint8 images come from pinned host memory (H2D of batch i + 1 on a copy stream under the kernels of
     batch i, as in DetectRing) and detections go back to pinned host memory inside the NMS branch.
 
-    raw_input=True: `submit(frames)` takes 1..B decoded uint8 HWC BGR frames of any sizes (see the module docstring); the step
-    graph letterboxes them before the network and the NMS branch rescales the previous batch's rows to its source pixels.
+    raw_input=True: `submit(frames, layout=...)` takes 1..B decoded uint8 frames of any sizes, host or CUDA (see the module
+    docstring); the step graph letterboxes them before the network and the NMS branch rescales the previous batch's rows to
+    its source pixels.
     """
 
     def __init__(self, model, batch, height, width, conf_thres=0.25, iou_thres=0.45, classes=None, agnostic=False,
@@ -209,7 +238,7 @@ class DetectStream:
         if self.dev.type != "cuda":
             raise RuntimeError("DetectStream needs a CUDA model")
         if raw_input and not host_input:
-            raise RuntimeError("DetectStream: raw_input takes host frames (host_input=True)")
+            raise RuntimeError("DetectStream: raw_input returns detections in host memory (host_input=True)")
         self.kw = dict(conf_thres=conf_thres, iou_thres=iou_thres, classes=classes, agnostic=agnostic,
                        multi_label=multi_label, max_det=max_det)
         self.host_input = bool(host_input)
@@ -237,6 +266,8 @@ class DetectStream:
         self.ev_fork, self.ev_join = torch.cuda.Event(), torch.cuda.Event()
         self.ev_copied = [torch.cuda.Event(), torch.cuda.Event()]
         self.ev_done = [torch.cuda.Event(), torch.cuda.Event()]
+        self.ev_ready = torch.cuda.Event()
+        self._ready = None        # event the next copy waits for: the producer of the submitted device frames
         self.steps = 0            # submitted batches
         self.collected = 0
         self.graphs = [None, None]
@@ -277,7 +308,7 @@ class DetectStream:
 
     def _letterbox(self, k):
         if self.raw:
-            letterbox_launch(self.raw[k]["src_dev"], self.raw[k]["geo_dev"], self.x_dev[k])
+            letterbox_frames_launch(self.raw[k]["rec_dev"], self.raw[k]["geo_dev"], self.x_dev[k])
             self.raw[k]["res_geo"].copy_(self.raw[k]["geo_dev"])
 
     def _build(self):
@@ -305,6 +336,9 @@ class DetectStream:
         if self.host_input:
             if self.steps >= 2:
                 self.copy_stream.wait_event(self.ev_done[k])   # the step that last read x_dev[k] has finished
+            if self._ready is not None:
+                self.copy_stream.wait_event(self._ready)
+                self._ready = None
             with torch.cuda.stream(self.copy_stream):
                 if self.raw:
                     raw_h2d(self.raw[k])
@@ -316,9 +350,10 @@ class DetectStream:
         self.ev_done[k].record(cur)
         self.steps += 1
 
-    def submit(self, images):
+    def submit(self, images, layout="bgr_hwc", ready=None):
         """Enqueue batch number `steps`.  Its graph also post-processes batch steps - 1 into the result slot that batch
-        steps - 3 used, so at most two batches may be waiting for `collect()`."""
+        steps - 3 used, so at most two batches may be waiting for `collect()`.  With raw_input, device frames are read after
+        the work enqueued before this call on the current stream, or after the event `ready` when one is given."""
         if self.steps - self.collected > 2:
             raise RuntimeError("DetectStream: collect() the oldest batch before submitting another (result slots would be overwritten)")
         k = self.steps & 1
@@ -326,8 +361,16 @@ class DetectStream:
             if self.steps >= 2:
                 self.ev_done[k].synchronize()                  # x_host[k] was copied by the step two submissions ago
             if self.raw:
-                self.raw[k]["nbytes"], _ = pack_frames(images, self.B, self.x_dev[k].shape[2], self.x_dev[k].shape[3], True,
-                                                       self.raw[k]["src_host"], self.raw[k]["geo_host"])
+                devs = raw_pack(self.raw[k], images, self.x_dev[k].shape[2], self.x_dev[k].shape[3], layout, self.dev)
+                # the step that read the slot's previous device frames is complete (ev_done[k] above): release them now
+                self.raw[k]["frames"] = devs
+                # only device frames need it: the caller's stream usually holds the previous step, and a copy that waited for
+                # it would no longer overlap that step
+                if devs:
+                    if ready is None:
+                        ready = self.ev_ready
+                        ready.record(torch.cuda.current_stream(self.dev))
+                    self._ready = ready
                 self.n_frames[self.steps] = len(images)
             else:
                 self.x_host[k].copy_(images)
@@ -394,6 +437,7 @@ class DetectFarm:
         self.n = 0
         self._ev = [torch.cuda.Event() for _ in range(lanes)]
         self._go = torch.cuda.Event()
+        self._ready = torch.cuda.Event()
 
     def lane_of_next(self):
         return self.lanes[self.n % len(self.lanes)]
@@ -404,10 +448,12 @@ class DetectFarm:
             self.lanes[i].launch()
         self.n += 1
 
-    def submit(self, images):
+    def submit(self, images, layout="bgr_hwc"):
         i = self.n % len(self.lanes)
+        # recorded on the caller's stream, where device frames were produced, before the lane's stream becomes current
+        self._ready.record(torch.cuda.current_stream(self.dev))
         with torch.cuda.stream(self.streams[i]):
-            self.lanes[i].submit(images)
+            self.lanes[i].submit(images, layout=layout, ready=self._ready)
         self.n += 1
 
     def fence(self):

@@ -2,9 +2,11 @@
 
 `Inferer.process_image` (core/inferer.py:161-171) letterboxes each image on the host with cv2 (data/data_augment.py:29-58)
 and `Inferer.rescale` (:173-188) maps the boxes back.  Here both run on the device for a whole batch per launch
-(`yv6_letterbox`, `yv6_rescale_boxes`): images of any size -- OpenCV `imread` layout, uint8 HWC BGR -- are packed back to
-back in one byte buffer, and a per-image int32 table carries the geometry the host computed with the reference's Python
-expressions.  Because the geometry is data, a CUDA graph that contains these kernels serves any mix of image sizes.
+(`yv6_letterbox_frames`, `yv6_rescale_boxes`): images of any size -- OpenCV `imread` layout, uint8 HWC BGR, or the RGB CHW
+of torchvision's decoders -- are read where they lie: host images are packed back to back in one staging buffer, CUDA
+tensors in place.  A per-image record table says where each image is and in which layout, and a per-image int32 table
+carries the geometry the host computed with the reference's Python expressions.  Because both are data, a CUDA graph that
+contains these kernels serves any mix of image sizes, layouts and locations.
 
 Only letterbox(..., auto=False) is provided: it pads every image to the full H x W canvas, so a batch has one shape.
 Inferer's own default, auto=True, pads to a stride multiple and gives each image its own shape; that does not fit a
@@ -53,34 +55,94 @@ class LetterboxMeta:
         self.geo, self.n, self.H, self.W, self.shapes, self.geo_dev = geo, n, H, W, shapes, geo_dev
 
 
-def pack_frames(frames, B, H, W, scaleup, src_host, geo_host):
-    """Validate `frames`, copy their bytes back to back into the pinned `src_host` and fill `geo_host` [B, GEO].
-    Raises RuntimeError before anything is written when a frame is malformed or the bytes exceed the buffer.
-    Returns (bytes used, shapes)."""
-    frames = [as_frame(f) for f in frames]
+LAYOUTS = {"bgr_hwc": _lib.LB_BGR_HWC, "rgb_chw": _lib.LB_RGB_CHW}
+REC = C.sizeof(_lib.LbSrc)    # bytes per image in the yv6_lb_src record table
+
+
+def source_pitches(shape, strides, layout):
+    """(h0, w0, row_pitch, plane_pitch) of a uint8 frame with these sizes and element strides in `layout` ("bgr_hwc":
+    [h0, w0, 3], pixel stride 3; "rgb_chw": [3, h0, w0]); RuntimeError when yv6_letterbox_frames cannot address it."""
+    if layout not in LAYOUTS:
+        raise RuntimeError(f"letterbox: layout must be one of {sorted(LAYOUTS)}, got {layout!r}")
+    hwc = layout == "bgr_hwc"
+    if len(shape) != 3 or shape[2 if hwc else 0] != 3:
+        raise RuntimeError(f"letterbox: {layout} frames must be {'HWC with 3 channels last' if hwc else 'CHW with 3 channels first'}, "
+                           f"got shape {tuple(shape)}")
+    h0, w0 = (shape[0], shape[1]) if hwc else (shape[1], shape[2])
+    if h0 < 1 or w0 < 1:
+        raise RuntimeError(f"letterbox: empty frame, shape {tuple(shape)}")
+    if strides[2] != 1:
+        raise RuntimeError(f"letterbox: the unit-stride axis of a {layout} frame must be the innermost one, got strides {tuple(strides)}")
+    if hwc and strides[1] != 3:
+        raise RuntimeError(f"letterbox: a bgr_hwc frame needs a pixel stride of 3 bytes, got strides {tuple(strides)}")
+    return int(h0), int(w0), int(strides[0] if hwc else strides[1]), 0 if hwc else int(strides[0])
+
+
+def check_frames(frames, B, layout, dev):
+    """Validate 1..B frames for one letterbox launch; nothing is copied or enqueued.  A frame is a host numpy array or CPU
+    tensor (staged: returned as a contiguous CPU tensor) or a uint8 tensor on `dev` (read in place).  Returns one
+    (tensor, on_device, h0, w0, row_pitch, plane_pitch) per frame; RuntimeError when any frame is unusable."""
     if not 1 <= len(frames) <= B:
         raise RuntimeError(f"letterbox: {len(frames)} frames for a batch of {B}")
-    used = sum(f.numel() for f in frames)
+    out = []
+    for im in frames:
+        t = torch.from_numpy(np.ascontiguousarray(im)) if isinstance(im, np.ndarray) else im
+        if not isinstance(t, torch.Tensor):
+            raise RuntimeError(f"letterbox: frames must be numpy arrays or tensors, got {type(im).__name__}")
+        on_dev = t.device.type != "cpu"
+        if on_dev and t.device != dev:
+            raise RuntimeError(f"letterbox: a frame on {t.device}, the pipeline runs on {dev}")
+        if t.dtype != torch.uint8:
+            raise RuntimeError(f"letterbox: frames must be uint8, got {t.dtype}")
+        if not on_dev:
+            t = t.contiguous()
+        out.append((t, on_dev) + source_pitches(tuple(t.shape), t.stride(), layout))
+    return out
+
+
+def pack_sources(srcs, B, H, W, scaleup, layout, src_host, geo_host, rec_host, src_dev_ptr):
+    """Lay out checked frames (`check_frames`) for yv6_letterbox_frames: copy the host frames back to back into `src_host`
+    (the device buffer at `src_dev_ptr` receives these bytes before the launch), fill the geometry table `geo_host` [B, GEO]
+    and the record table `rec_host` (B * REC bytes).  A device frame's record points at the frame itself.  Raises
+    RuntimeError before anything is written when the host frames exceed `src_host`.
+    Returns (host bytes used, shapes, the device frames)."""
+    used = sum(t.numel() for t, on_dev, *_ in srcs if not on_dev)
     if used > src_host.numel():
-        raise RuntimeError(f"letterbox: the frames hold {used} bytes, the staging buffer {src_host.numel()} (raise max_src_bytes)")
-    rows, shapes, off = [], [], 0
-    for f in frames:
-        h0, w0 = int(f.shape[0]), int(f.shape[1])
+        raise RuntimeError(f"letterbox: the host frames hold {used} bytes, the staging buffer {src_host.numel()} (raise max_src_bytes)")
+    recs = (_lib.LbSrc * B)()
+    rows, shapes, devs, off = [], [], [], 0
+    for i, (t, on_dev, h0, w0, row_pitch, plane_pitch) in enumerate(srcs):
         r, (nw, nh), top, left = letterbox_geometry(h0, w0, H, W, scaleup)
-        src_host[off:off + f.numel()].copy_(f.view(-1))
-        rows.append([off, h0, w0, nh, nw, top, left, 0])
+        if on_dev:
+            base, src_off = t.data_ptr(), 0
+            devs.append(t)
+        else:
+            src_host[off:off + t.numel()].copy_(t.view(-1))
+            base, src_off = src_dev_ptr + off, off
+            off += t.numel()
+        recs[i] = _lib.LbSrc(base, row_pitch, plane_pitch, LAYOUTS[layout], 0)
+        rows.append([src_off, h0, w0, nh, nw, top, left, 0])
         shapes.append(((h0, w0), ((h0 * r / h0, w0 * r / w0), (left, top))))
-        off += f.numel()
-    rows += [[0, H, W, 0, 0, 0, 0, 0]] * (B - len(frames))         # unused slots: all border, rescale well defined
+    rows += [[0, H, W, 0, 0, 0, 0, 0]] * (B - len(srcs))         # unused slots: all border, rescale well defined
     geo_host.copy_(torch.tensor(rows, dtype=torch.int32))
+    C.memmove(rec_host.data_ptr(), recs, C.sizeof(recs))
+    return used, shapes, devs
+
+
+def pack_frames(frames, B, H, W, scaleup, src_host, geo_host):
+    """Validate host frames (uint8 HWC BGR), copy their bytes back to back into the pinned `src_host` and fill `geo_host`
+    [B, GEO].  Raises RuntimeError before anything is written when a frame is malformed or the bytes exceed the buffer.
+    Returns (bytes used, shapes)."""
+    srcs = check_frames(frames, B, "bgr_hwc", torch.device("cpu"))
+    used, shapes, _ = pack_sources(srcs, B, H, W, scaleup, "bgr_hwc", src_host, geo_host, torch.empty(B * REC, dtype=torch.uint8), 0)
     return used, shapes
 
 
-def letterbox_launch(src_dev, geo_dev, out, stream=None):
-    """yv6_letterbox on device buffers: src_dev packed uint8 sources, geo_dev int32 [B, GEO], out uint8 [B, 3, H, W]."""
+def letterbox_frames_launch(rec_dev, geo_dev, out, stream=None):
+    """yv6_letterbox_frames on device tables: rec_dev the B yv6_lb_src records, geo_dev int32 [B, GEO], out uint8 [B, 3, H, W]."""
     B, _, H, W = out.shape
-    _lib.check(_lib.lib().yv6_letterbox(_lib.handle(out.device.index or 0), C.c_void_p(src_dev.data_ptr()), C.c_void_p(geo_dev.data_ptr()),
-                                        B, H, W, C.c_void_p(out.data_ptr()), _lib.stream_ptr(stream)))
+    _lib.check(_lib.lib().yv6_letterbox_frames(_lib.handle(out.device.index or 0), C.c_void_p(rec_dev.data_ptr()),
+                                               C.c_void_p(geo_dev.data_ptr()), B, H, W, C.c_void_p(out.data_ptr()), _lib.stream_ptr(stream)))
     return out
 
 
@@ -95,25 +157,33 @@ def rescale_launch(out, count, geo_dev, H, W, res=None, stream=None):
     return res
 
 
-def letterbox_batch(images, H, W, scaleup=True, out=None, device=None):
-    """Letterbox a list of uint8 HWC BGR host images (numpy arrays or CPU tensors, any sizes) onto the uint8 NCHW RGB
-    canvas [B, 3, H, W] on the device -- letterbox(im, (H, W), auto=False, scaleup) + HWC->CHW + BGR->RGB of
-    Inferer.process_image, bit-exact against cv2.  `scaleup=True` is Inferer's setting, False the Evaler dataset's.
-    Returns (canvas, LetterboxMeta).  `out` (uint8 [B, 3, H, W] CUDA tensor, B >= len(images)) is filled in place."""
+def letterbox_batch(images, H, W, scaleup=True, out=None, device=None, layout="bgr_hwc"):
+    """Letterbox a list of uint8 frames of any sizes onto the uint8 NCHW RGB canvas [B, 3, H, W] on the device --
+    letterbox(im, (H, W), auto=False, scaleup) + HWC->CHW + BGR->RGB of Inferer.process_image, bit-exact against cv2.
+    Each frame is a host numpy array or CPU tensor (staged through pinned memory) or a CUDA tensor on the canvas's device
+    (read in place, in stream order after the work already on the current stream).  `layout` applies to every frame:
+    "bgr_hwc" is cv2 imread's [h0, w0, 3] (rows may be padded, e.g. a crop view), "rgb_chw" torchvision's decoders'
+    [3, h0, w0]; both give the canvas of the equivalent BGR HWC image.  `scaleup=True` is Inferer's setting, False the
+    Evaler dataset's.  Returns (canvas, LetterboxMeta).  `out` (uint8 [B, 3, H, W] CUDA tensor, B >= len(images)) is
+    filled in place."""
     if out is None:
         out = torch.empty(len(images), 3, H, W, dtype=torch.uint8, device=device or torch.device("cuda", torch.cuda.current_device()))
     if out.device.type != "cuda" or out.dtype != torch.uint8 or tuple(out.shape[1:]) != (3, H, W):
         raise RuntimeError("letterbox_batch: out must be a uint8 CUDA tensor [B, 3, H, W]")
     B = out.shape[0]
-    frames = [as_frame(f) for f in images]
-    src_host = torch.empty(max(1, sum(f.numel() for f in frames)), dtype=torch.uint8).pin_memory()
+    srcs = check_frames(images, B, layout, out.device)
+    nbytes = max(1, sum(t.numel() for t, on_dev, *_ in srcs if not on_dev))
+    src_host = torch.empty(nbytes, dtype=torch.uint8).pin_memory()
     geo_host = torch.empty(B, GEO, dtype=torch.int32).pin_memory()
-    used, shapes = pack_frames(frames, B, H, W, scaleup, src_host, geo_host)
-    src_dev = src_host.to(out.device, non_blocking=True)
+    rec_host = torch.empty(B * REC, dtype=torch.uint8).pin_memory()
+    src_dev = torch.empty(nbytes, dtype=torch.uint8, device=out.device)
+    _, shapes, _ = pack_sources(srcs, B, H, W, scaleup, layout, src_host, geo_host, rec_host, src_dev.data_ptr())
+    src_dev.copy_(src_host, non_blocking=True)
     geo_dev = geo_host.to(out.device, non_blocking=True)
-    letterbox_launch(src_dev, geo_dev, out)
+    rec_dev = rec_host.to(out.device, non_blocking=True)
+    letterbox_frames_launch(rec_dev, geo_dev, out)
     torch.cuda.current_stream(out.device).synchronize()      # the pinned staging buffers die with this call
-    return out, LetterboxMeta(geo_host.clone(), len(frames), H, W, shapes, geo_dev)
+    return out, LetterboxMeta(geo_host.clone(), len(images), H, W, shapes, geo_dev)
 
 
 def rescale_boxes(out, count, meta):
