@@ -34,6 +34,7 @@
 //     multicast into both CTAs.
 #include <algorithm>
 #include <cstdarg>
+#include <type_traits>
 
 #include "yv6_common.cuh"
 #include "yv6_handle.h"
@@ -405,17 +406,39 @@ __device__ __forceinline__ void stage_out_tile_t(const ConvKParams& p, float (&a
 
 // One K block of a 128-row tile: 2 x KSTEPS k16 MMAs (rows 0-63 from descriptor ad, rows 64-127 from ad + a_hi, the same
 // B operand), issued back to back as ONE commit group.  KSTEPS must be known at compile time: an MMA under a runtime
-// condition makes ptxas split the group and inject warpgroup.arrive around it (warning C7519).
-template <int BN, int KSTEPS>
+// condition makes ptxas split the group and inject warpgroup.arrive around it (warning C7519).  LO: the same group with the
+// rows 0-63 MMAs only, for a tile whose rows 64-127 all lie outside the output (upper_half_dead); acc[1] is left as it is.
+template <int BN, int KSTEPS, bool LO = false>
 __device__ __forceinline__ void mma_kblock(float (&acc)[2][BN / 2], uint64_t ad, uint32_t a_hi, uint64_t bd, uint32_t scale_d) {
   wgmma_fence();
 #pragma unroll
   for (int k = 0; k < KSTEPS; ++k) {
     const uint32_t sd = k == 0 ? scale_d : 1u;
     Wgmma<BN, 0, 0>::mma(acc[0], ad + (uint64_t)(2 * k), bd + (uint64_t)(2 * k), sd);
-    Wgmma<BN, 0, 0>::mma(acc[1], ad + (uint64_t)(a_hi + 2 * k), bd + (uint64_t)(2 * k), sd);
+    if constexpr (!LO) Wgmma<BN, 0, 0>::mma(acc[1], ad + (uint64_t)(a_hi + 2 * k), bd + (uint64_t)(2 * k), sd);
   }
   wgmma_commit();
+}
+
+// A tile's upper half is dead when every row 64-127 of its BW x BH x BI box (pixel-major: row = bw + BW (bh + BH bi)) is
+// outside the output or beyond the box, so that nothing computed for them is ever stored.  The box rows from 64 on are the
+// (bi, bh, bw) at or after row 64's in lexicographic order; the rows inside the output are a product of ranges from 0, whose
+// lexicographic last is (ni - 1, nh - 1, nw - 1).  For the 8 x 16 halo tiles this is t.h0 + 8 >= Ho; the empty second tile of
+// a CTA pair's last unit (placed on image N) counts as dead too.  Row 64's coordinates are worked out once per kernel: with
+// the divisions done per tile, the BN-64 1x1 layers of YOLOv6-S (about 12 tiles per CTA) ran about 1 % slower on an H100.
+struct Row64 {
+  int w, h, i;   // box coordinates of row 64; i = BI when the box has <= 64 rows
+};
+__device__ __forceinline__ Row64 row64_of(const ConvKParams& p) {
+  const int q = 64 / p.BW;
+  return Row64{64 % p.BW, q % p.BH, p.rows <= 64 ? p.BI : q / p.BH};
+}
+__device__ __forceinline__ bool upper_half_dead(const ConvKParams& p, const Row64& r, const TileCoord& t) {
+  const int ni = min(p.N - t.i0, p.BI), nh = min(p.Ho - t.h0, p.BH), nw = min(p.Wo - t.w0, p.BW);
+  if (ni <= 0 || nh <= 0 || nw <= 0) return true;
+  if (ni - 1 != r.i) return ni - 1 < r.i;
+  if (nh - 1 != r.h) return nh - 1 < r.h;
+  return nw - 1 < r.w;
 }
 
 // The same K block of a BN = 64 halo tile computed transposed, D[64 channels x 128 pixels]: the 64-row weight tile (wd) is the
@@ -607,10 +630,16 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     bool first = true;
     float* sCw = sC + wg * 64 * stage_pitch(BN);         // this warpgroup's half of the staging tile
     float* sbias = sCw + 64 * BN;                        // TMA-store epilogue: the tile's bias, after the staged tile
+    const Row64 row64 = row64_of(p);
     for (int tile = unit0 + wg * ustep; tile < num_tiles; tile += 2 * ustep) {
+      const TileCoord t = coord(tile);
       // TMA-store epilogue: the tile's bias goes to shared memory before the MMAs (this warpgroup's last epilogue read its
       // previous contents before its final barrier), so that its load latency hides under the wait for the tensor cores
-      if (p.tma_store && p.bias != nullptr && ct < BN) sbias[ct] = __ldg(p.bias + coord(tile).n0 + ct);
+      if (p.tma_store && p.bias != nullptr && ct < BN) sbias[ct] = __ldg(p.bias + t.n0 + ct);
+      // rows 64-127 lie wholly outside the output (the last tile row of a map with Ho % 16 in 1..8, a box of <= 64 rows): the
+      // K loop issues only the rows 0-63 MMAs and the epilogue skips acc[1].  The transposed BN = 64 halo tiles keep one
+      // m64n128 per k16 step over all 128 pixels.
+      const bool dead_hi = !SWAP && upper_half_dead(p, row64, t);
       if (tile != unit0) {                               // the other warpgroup owns the preceding tile
         if constexpr (HALO) {
           skip_stages(sa, pha, pcs, p.a_stages);
@@ -621,103 +650,111 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         mbar_wait(&mma_turn[wg], turn_ph);
         turn_ph ^= 1;
       }
-      if constexpr (HALO) {
-        // A descriptors walk the halo tile: 8-row groups are the 8 pixels of one output row, SH halo rows apart;
-        // tap (r,s) shifts the start address by (W r + s) pixels, rows 64-127 start 8 output rows further.  At BN = 64 the same
-        // descriptor is the B operand and spans all 16 groups.
-        const uint32_t row_bytes = (uint32_t)(HG::W * 128 * HG::SH);
-        const uint64_t desc_a = wgmma_desc(16u, row_bytes, 1u);
-        const uint64_t desc_b = wgmma_desc(16u, 1024u, 1u);
-        const uint32_t halo_step = (uint32_t)HG::kStageBytes >> 4, b_step = (uint32_t)p.b_stage_bytes >> 4;
-        const uint32_t a_hi = 8u * (row_bytes >> 4);
-        const int skip_cb = p.skip_cb, cin_blocks = p.cin_blocks, b_stages = p.b_stages;
-        int slot = 0;
-        uint32_t started = 0;
-        // Stages whose MMAs may still be in flight: the B stage of the last committed group and the A stage of the previous
-        // channel block.  Each is released once a later group has been committed and wgmma_wait<1> has returned, so the
-        // pipe never drains at a channel-block boundary; the one full wait per tile comes before the epilogue.
-        int prev_sb = -1, prev_sa = -1;
-        for (int pc = 0; pc < pcs; ++pc) {
-          mbar_wait(&a_full[sa], pha);
-          const uint32_t a0 = a_base + (uint32_t)sa * halo_step;
-          const bool skip_s0 = (HG::SH == 2) && (pc % cin_blocks) < skip_cb;      // this channel block of the s = 0 taps is all zero
+      // The tile's K loop, in two copies whose commit groups hold a fixed number of MMAs each (see mma_kblock): lo_only =
+      // std::true_type issues rows 0-63 only.  The K order, stage releases and hand-over are the same in both.
+      auto mainloop = [&](auto lo_only) {
+        [[maybe_unused]] constexpr bool LO = decltype(lo_only)::value;   // (the transposed BN = 64 tiles ignore it)
+        if constexpr (HALO) {
+          // A descriptors walk the halo tile: 8-row groups are the 8 pixels of one output row, SH halo rows apart;
+          // tap (r,s) shifts the start address by (W r + s) pixels, rows 64-127 start 8 output rows further.  At BN = 64 the same
+          // descriptor is the B operand and spans all 16 groups.
+          const uint32_t row_bytes = (uint32_t)(HG::W * 128 * HG::SH);
+          const uint64_t desc_a = wgmma_desc(16u, row_bytes, 1u);
+          const uint64_t desc_b = wgmma_desc(16u, 1024u, 1u);
+          const uint32_t halo_step = (uint32_t)HG::kStageBytes >> 4, b_step = (uint32_t)p.b_stage_bytes >> 4;
+          [[maybe_unused]] const uint32_t a_hi = 8u * (row_bytes >> 4);
+          const int skip_cb = p.skip_cb, cin_blocks = p.cin_blocks, b_stages = p.b_stages;
+          int slot = 0;
+          uint32_t started = 0;
+          // Stages whose MMAs may still be in flight: the B stage of the last committed group and the A stage of the previous
+          // channel block.  Each is released once a later group has been committed and wgmma_wait<1> has returned, so the
+          // pipe never drains at a channel-block boundary; the one full wait per tile comes before the epilogue.
+          int prev_sb = -1, prev_sa = -1;
+          for (int pc = 0; pc < pcs; ++pc) {
+            mbar_wait(&a_full[sa], pha);
+            const uint32_t a0 = a_base + (uint32_t)sa * halo_step;
+            const bool skip_s0 = (HG::SH == 2) && (pc % cin_blocks) < skip_cb;      // this channel block of the s = 0 taps is all zero
 #pragma unroll
-          for (int tap = 0; tap < HG::TAPS; ++tap) {
-            if (HG::SH == 2 && (tap % HG::KW) == 0 && skip_s0) continue;
-            const int bs = BRES ? slot : sb;
-            // resident weights were loaded during the CTA's first tile; each warpgroup waits for them before its first tile
-            if (!BRES || first) mbar_wait(&b_full[bs], BRES ? 0u : phb);
-            const uint64_t ad = desc_a | (uint64_t)(a0 + (uint32_t)((tap / HG::KW) * HG::W + (tap % HG::KW)) * 8u);
-            const uint64_t bd = desc_b | (uint64_t)(b_base + (uint32_t)bs * b_step);
-            if constexpr (SWAP) mma_kblock_t<4>(acc, bd, ad, started);
-            else mma_kblock<BN, 4>(acc, ad, a_hi, bd, started);
-            started = 1u;
-            if (!BRES || prev_sa >= 0) {
-              wgmma_wait<1>();
-              if (arrive_lane) {
-                if (!BRES && prev_sb >= 0) release_b(&b_empty[prev_sb]);
-                if (prev_sa >= 0) mbar_arrive(&a_empty[prev_sa]);
+            for (int tap = 0; tap < HG::TAPS; ++tap) {
+              if (HG::SH == 2 && (tap % HG::KW) == 0 && skip_s0) continue;
+              const int bs = BRES ? slot : sb;
+              // resident weights were loaded during the CTA's first tile; each warpgroup waits for them before its first tile
+              if (!BRES || first) mbar_wait(&b_full[bs], BRES ? 0u : phb);
+              const uint64_t ad = desc_a | (uint64_t)(a0 + (uint32_t)((tap / HG::KW) * HG::W + (tap % HG::KW)) * 8u);
+              const uint64_t bd = desc_b | (uint64_t)(b_base + (uint32_t)bs * b_step);
+              if constexpr (SWAP) mma_kblock_t<4>(acc, bd, ad, started);
+              else mma_kblock<BN, 4, LO>(acc, ad, a_hi, bd, started);
+              started = 1u;
+              if (!BRES || prev_sa >= 0) {
+                wgmma_wait<1>();
+                if (arrive_lane) {
+                  if (!BRES && prev_sb >= 0) release_b(&b_empty[prev_sb]);
+                  if (prev_sa >= 0) mbar_arrive(&a_empty[prev_sa]);
+                }
+                prev_sa = -1;
               }
-              prev_sa = -1;
+              if (!BRES) {
+                prev_sb = sb;
+                if (++sb == b_stages) { sb = 0; phb ^= 1; }
+              }
+              ++slot;
             }
-            if (!BRES) {
-              prev_sb = sb;
-              if (++sb == b_stages) { sb = 0; phb ^= 1; }
+            prev_sa = sa;
+            if (++sa == p.a_stages) { sa = 0; pha ^= 1; }
+          }
+          mbar_arrive(&mma_turn[wg ^ 1]);                  // the other warpgroup may start its tile's MMAs
+          wgmma_wait<0>();
+          if (arrive_lane) {
+            if (!BRES && prev_sb >= 0) release_b(&b_empty[prev_sb]);
+            if (prev_sa >= 0) mbar_arrive(&a_empty[prev_sa]);
+          }
+        } else {
+          const uint64_t desc = wgmma_desc(16u, (uint32_t)p.sbo_bytes, (uint32_t)p.layout_type);
+          const uint32_t a_step = (uint32_t)p.a_stage_bytes >> 4, b_step = (uint32_t)p.b_stage_bytes >> 4;
+          const uint32_t a_hi = (uint32_t)(64 * p.kb_bytes) >> 4;
+          int prev = -1;
+          for (int kb = 0; kb < kblocks; ++kb) {
+            mbar_wait(&full[stage], phase);
+            const uint64_t ad = desc | (uint64_t)(a_base + (uint32_t)stage * a_step);
+            const uint64_t bd = desc | (uint64_t)(b_base + (uint32_t)stage * b_step);
+            const uint32_t scale_d = (uint32_t)(kb != 0);
+            switch (ksteps) {          // 16-, 32- or 64-channel K blocks
+              case 1: mma_kblock<BN, 1, LO>(acc, ad, a_hi, bd, scale_d); break;
+              case 2: mma_kblock<BN, 2, LO>(acc, ad, a_hi, bd, scale_d); break;
+              default: mma_kblock<BN, 4, LO>(acc, ad, a_hi, bd, scale_d); break;
             }
-            ++slot;
+            wgmma_wait<1>();
+            if (prev >= 0 && arrive_lane) release_b(&empty[prev]);
+            prev = stage;
+            if (++stage == nstages) {
+              stage = 0;
+              phase ^= 1;
+            }
           }
-          prev_sa = sa;
-          if (++sa == p.a_stages) { sa = 0; pha ^= 1; }
-        }
-        mbar_arrive(&mma_turn[wg ^ 1]);                  // the other warpgroup may start its tile's MMAs
-        wgmma_wait<0>();
-        if (arrive_lane) {
-          if (!BRES && prev_sb >= 0) release_b(&b_empty[prev_sb]);
-          if (prev_sa >= 0) mbar_arrive(&a_empty[prev_sa]);
-        }
-      } else {
-        const uint64_t desc = wgmma_desc(16u, (uint32_t)p.sbo_bytes, (uint32_t)p.layout_type);
-        const uint32_t a_step = (uint32_t)p.a_stage_bytes >> 4, b_step = (uint32_t)p.b_stage_bytes >> 4;
-        const uint32_t a_hi = (uint32_t)(64 * p.kb_bytes) >> 4;
-        int prev = -1;
-        for (int kb = 0; kb < kblocks; ++kb) {
-          mbar_wait(&full[stage], phase);
-          const uint64_t ad = desc | (uint64_t)(a_base + (uint32_t)stage * a_step);
-          const uint64_t bd = desc | (uint64_t)(b_base + (uint32_t)stage * b_step);
-          const uint32_t scale_d = (uint32_t)(kb != 0);
-          switch (ksteps) {          // 16-, 32- or 64-channel K blocks
-            case 1: mma_kblock<BN, 1>(acc, ad, a_hi, bd, scale_d); break;
-            case 2: mma_kblock<BN, 2>(acc, ad, a_hi, bd, scale_d); break;
-            default: mma_kblock<BN, 4>(acc, ad, a_hi, bd, scale_d); break;
-          }
-          wgmma_wait<1>();
+          mbar_arrive(&mma_turn[wg ^ 1]);                  // the other warpgroup may start its tile's MMAs
+          wgmma_wait<0>();
           if (prev >= 0 && arrive_lane) release_b(&empty[prev]);
-          prev = stage;
-          if (++stage == nstages) {
-            stage = 0;
-            phase ^= 1;
-          }
         }
-        mbar_arrive(&mma_turn[wg ^ 1]);                  // the other warpgroup may start its tile's MMAs
-        wgmma_wait<0>();
-        if (prev >= 0 && arrive_lane) release_b(&empty[prev]);
-      }
+      };
+      if (dead_hi) mainloop(std::true_type());
+      else mainloop(std::false_type());
       wgmma_fence_operand(acc[0]);
       wgmma_fence_operand(acc[1]);
       first = false;
 
-      const TileCoord t = coord(tile);
       const int r0 = (warp & 3) * 16 + (lane >> 2);      // this thread's fragment rows r0 + 8 i (+ 64 for acc[1]) and
       const int c0 = 2 * (lane & 3);                     // columns 8 j + c0, + 1
       if (p.tma_store) {
         // ---- epilogue through the output tensor map: bias, activation and rounding in registers, the tile staged in the
         //      output dtype (bf16: all 128 rows in one pass; fp32: one 64-row pass per accumulator half), one bulk tensor
-        //      store per column group.  The stores clip at the output's edges. ----
+        //      store per column group.  The stores clip at the output's edges, so a dead upper half (dead_hi) is neither
+        //      computed nor staged: bf16 stores whatever its staging rows hold, which lie outside the output; fp32 skips
+        //      its second pass. ----
         const bool f32 = p.y_dtype == YV6_DT_F32;
         uint8_t* stage = reinterpret_cast<uint8_t*>(sCw);
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
-          if (h == 1 && !f32) break;
+          if (h == 1 && (!f32 || dead_hi)) break;
           if (ct == 0) bulk_wait_read();               // the last store has read the staging half
           warpgroup_bar_sync(wg);
           if constexpr (SWAP) {
@@ -731,7 +768,7 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             stage_out_tile<BN, true>(p, acc[h], sbias, stage, r0, c0);
           } else {
             stage_out_tile<BN, false>(p, acc[0], sbias, stage, r0, c0);
-            stage_out_tile<BN, false>(p, acc[1], sbias, stage, r0 + 64, c0);
+            if (!dead_hi) stage_out_tile<BN, false>(p, acc[1], sbias, stage, r0 + 64, c0);
           }
           fence_proxy_async();
           warpgroup_bar_sync(wg);
@@ -752,7 +789,7 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const int rows = min(64, p.rows - 64 * h);
-        if (rows <= 0) break;
+        if (rows <= 0 || (h == 1 && dead_hi)) break;
         warpgroup_bar_sync(wg);                  // the previous pass's chunks have all been read from the staging half
         if constexpr (SWAP) {                    // transposed: channels r0 + 8 i of pixels 8 j + c0 + c
 #pragma unroll
