@@ -38,7 +38,6 @@ class ComputeLoss(_DetLoss):
         self.distill_feat = bool(distill_feat)       # needs `model.return_featmaps = True` on student and teacher (real neck outputs)
         self.distill_weight = distill_weight
         self._norm_gt_zero = 1
-        self._defer_fn = False
 
     def _cw_term(self, s_featmaps, t_featmaps, decay, terms):
         """distill_loss_cw (:223-245), temperature 1: per level KL over the H*W positions of every (image, channel) row, / (N*C).
@@ -59,12 +58,15 @@ class ComputeLoss(_DetLoss):
             grads.append(g)
         return grads
 
-    def __call__(self, outputs, t_outputs, s_featmaps, t_featmaps, targets, epoch_num, max_epoch, temperature, step_num,
-                 batch_height, batch_width):
-        feats, pred_scores, pred_distri = outputs
-        t_pred_scores, t_pred_distri = t_outputs[-2], t_outputs[-1]            # loss_distill.py:76 (a fuse_ab teacher returns five)
-        sizes = [tuple(f.shape[2:]) for f in feats]
-        state = self.forward_backward(pred_scores, pred_distri, sizes, targets, epoch_num, batch_height, batch_width)
+    def distill_forward_backward(self, pred_scores, pred_distri, t_pred_scores, t_pred_distri, sizes, targets, epoch_num, max_epoch,
+                                 temperature, batch_height, batch_width, s_featmaps=(), t_featmaps=(), max_gt=None, grad_scores=None,
+                                 grad_distri=None):
+        """The whole loss and its gradients on the device (no autograd, no host read), as `forward_backward` is for the detection
+        loss: returns its state with "out" = float64[8] (loss, iou, dfl, cls, target_scores_sum, num_pos, cwd, 0) -- iou / dfl / cls
+        include the distillation terms as in loss_items -- and "feat_grads", the NCHW fp32 gradients w.r.t. s_featmaps[:3]
+        (distill_feat).  `max_gt` and `grad_*` as in forward_backward: step.TrainStep passes its engine's buffers."""
+        state = self.forward_backward(pred_scores, pred_distri, sizes, targets, epoch_num, batch_height, batch_width, max_gt=max_gt,
+                                      grad_scores=grad_scores, grad_distri=grad_distri)
         dev = pred_scores.device
         lib, h, sp = _lib.lib(), _lib.handle(dev.index or 0), _lib.stream_ptr()
         B, A, nc = pred_scores.shape
@@ -92,17 +94,27 @@ class ComputeLoss(_DetLoss):
         total[0] = out[0] + terms[0] + terms[1] + terms[2]
         total[2] = out[2] + terms[1]               # loss_weight['dfl'] * loss_dfl_all
         total[3] = out[3] + terms[0]               # loss_weight['class'] * loss_cls_all
+        total[6] = terms[2]
         state["out"] = total
-        state["cwd"] = terms[2:3]
         state["keep_distill"] = (ts, td, terms)
         state["feat_grads"] = feat_grads
-        self._last_state = state
-        if self._defer_fn:                           # ComputeLossNS adds its third tensor and builds the function itself
-            return None, None
-        loss = _GradsFn.apply(state, [state["grad_scores"], state["grad_distri"]] + feat_grads, pred_scores, pred_distri,
+        return state
+
+    def __call__(self, outputs, t_outputs, s_featmaps, t_featmaps, targets, epoch_num, max_epoch, temperature, step_num,
+                 batch_height, batch_width):
+        feats, pred_scores, pred_distri = outputs
+        t_pred_scores, t_pred_distri = t_outputs[-2], t_outputs[-1]            # loss_distill.py:76 (a fuse_ab teacher returns five)
+        sizes = [tuple(f.shape[2:]) for f in feats]
+        state = self.distill_forward_backward(pred_scores, pred_distri, t_pred_scores, t_pred_distri, sizes, targets, epoch_num, max_epoch,
+                                              temperature, batch_height, batch_width, s_featmaps, t_featmaps)
+        loss = _GradsFn.apply(state, [state["grad_scores"], state["grad_distri"]] + state["feat_grads"], pred_scores, pred_distri,
                               *list(s_featmaps[:3] if self.distill_feat else []))
-        items = torch.cat([total[1:4], terms[2:3]])   # (iou, dfl_all, cls_all, cwd)
-        return loss, items.detach()
+        return loss, _items(state["out"])
+
+
+def _items(out):
+    """(iou, dfl_all, cls_all, cwd): the reference's loss_items."""
+    return torch.cat([out[1:4], out[6:7]]).detach()
 
 
 class _GradsFn(torch.autograd.Function):
@@ -130,27 +142,28 @@ class ComputeLossNS(ComputeLoss):
         super().__init__(*args, **kw)
         self.warmup_epoch = 0          # loss_distill_ns.py never calls its warm-up assigner
 
-    def __call__(self, outputs, t_outputs, s_featmaps, t_featmaps, targets, epoch_num, max_epoch, temperature, step_num,
-                 batch_height, batch_width):
-        feats, pred_scores, pred_distri, pred_lrtb = outputs
-        self._defer_fn = True
-        try:
-            super().__call__((feats, pred_scores, pred_distri), t_outputs, s_featmaps, t_featmaps, targets, epoch_num, max_epoch,
-                             temperature, step_num, batch_height, batch_width)
-        finally:
-            self._defer_fn = False
-        state = self._last_state
-        sizes = [tuple(f.shape[2:]) for f in feats]
-        # IoU of the lrtb branch against the same targets / assignment; no class or DFL term (reg_ch = 4)
+    def distill_forward_backward(self, pred_scores, pred_distri, t_pred_scores, t_pred_distri, sizes, targets, epoch_num, max_epoch,
+                                 temperature, batch_height, batch_width, s_featmaps=(), t_featmaps=(), max_gt=None, grad_scores=None,
+                                 grad_distri=None, pred_lrtb=None, grad_lrtb=None):
+        """ComputeLoss.distill_forward_backward plus the IoU term of the lrtb branch `pred_lrtb` (its gradient into `grad_lrtb`,
+        when given) against the same targets and assignment: no class or DFL term (reg_ch = 4)."""
+        state = super().distill_forward_backward(pred_scores, pred_distri, t_pred_scores, t_pred_distri, sizes, targets, epoch_num,
+                                                 max_epoch, temperature, batch_height, batch_width, s_featmaps, t_featmaps, max_gt,
+                                                 grad_scores, grad_distri)
         st2 = self.forward_backward(pred_scores, pred_lrtb, sizes, targets, epoch_num, batch_height, batch_width, reuse=state,
-                                    weights=(0.0, float(self.loss_weight['iou']), 0.0))
+                                    grad_distri=grad_lrtb, weights=(0.0, float(self.loss_weight['iou']), 0.0))
         total = state["out"].clone()
         total[0] = total[0] + st2["out"][0]
         total[1] = total[1] + st2["out"][1]
-        state = dict(state, out=total, keep_lrtb=st2)
         # (the class-score gradient of the second call is exactly zero: w_cls = 0)
-        fg = state["feat_grads"]
-        loss = _GradsFn.apply(state, [state["grad_scores"], state["grad_distri"], st2["grad_distri"]] + fg, pred_scores, pred_distri, pred_lrtb,
-                              *list(s_featmaps[:3] if self.distill_feat else []))
-        items = torch.cat([total[1:4], state["cwd"]])
-        return loss, items.detach()
+        return dict(state, out=total, keep_lrtb=st2)
+
+    def __call__(self, outputs, t_outputs, s_featmaps, t_featmaps, targets, epoch_num, max_epoch, temperature, step_num,
+                 batch_height, batch_width):
+        feats, pred_scores, pred_distri, pred_lrtb = outputs
+        sizes = [tuple(f.shape[2:]) for f in feats]
+        state = self.distill_forward_backward(pred_scores, pred_distri, t_outputs[-2], t_outputs[-1], sizes, targets, epoch_num, max_epoch,
+                                              temperature, batch_height, batch_width, s_featmaps, t_featmaps, pred_lrtb=pred_lrtb)
+        grads = [state["grad_scores"], state["grad_distri"], state["keep_lrtb"]["grad_distri"]] + state["feat_grads"]
+        loss = _GradsFn.apply(state, grads, pred_scores, pred_distri, pred_lrtb, *list(s_featmaps[:3] if self.distill_feat else []))
+        return loss, _items(state["out"])

@@ -165,7 +165,7 @@ class Model(nn.Module):
 
     def __getstate__(self):
         st = self.__dict__.copy()
-        for k in ("_graph", "_engine", "_engine_key", "_train_engine"):
+        for k in ("_graph", "_engine", "_engine_key", "_train_engine", "_teacher_engine"):
             st.pop(k, None)
         st["_engine"], st["_engine_key"] = None, None
         return st
@@ -264,6 +264,18 @@ class Model(nn.Module):
             from .train import TrainEngine
             eng = TrainEngine(self, n_buckets or 1)
             self.__dict__["_train_engine"] = eng
+        return eng
+
+    def teacher_engine(self, rebuild=False):
+        """The forward-only training engine of this model as a self-distillation teacher (train.py, `teacher=True`):
+        batch-statistics BatchNorm that leaves the running statistics alone, no backward; step.TrainStep(teacher=...) runs it."""
+        if self.graph.lite:
+            raise NotImplementedError(LITE_TRAINING)
+        eng = self.__dict__.get("_teacher_engine")
+        if eng is None or rebuild or eng.dev != next(self.parameters()).device or not eng.flat.valid():
+            from .train import TrainEngine
+            eng = TrainEngine(self, teacher=True)
+            self.__dict__["_teacher_engine"] = eng
         return eng
 
     def forward(self, x):

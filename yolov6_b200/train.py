@@ -188,8 +188,18 @@ class _Scratch:
         return pools[-1]
 
 
+FWD_ARENA_KEYS = ("fsum", "fcnt", "qsum", "qcnt")     # the zero-arena slots the forward pass uses (batch-statistics sums)
+
+
 class TrainEngine:
-    def __init__(self, model, n_buckets=1):
+    """`teacher=True` plans the forward pass only, for the teacher of self-distillation (core/engine.py:429-441): batch-statistics
+    BatchNorm with `track_running_stats = False` (the finalize launches get null running statistics, num_batches_tracked stays),
+    no gradient buffers, scratch or backward launches, and no anchor-aided pred convs of a fuse_ab model (the distillation loss
+    reads the anchor-free head, loss_distill.py:76).  step.TrainStep runs it next to the student's step."""
+    teacher = False
+
+    def __init__(self, model, n_buckets=1, teacher=False):
+        self.teacher = bool(teacher)
         self.model = model
         self.g = model.graph
         self.dev = next(model.parameters()).device
@@ -223,6 +233,8 @@ class TrainEngine:
 
         def ztake(key, nbytes):
             nonlocal ztot
+            if self.teacher and key[1] not in FWD_ARENA_KEYS:
+                return
             zoff[key] = ztot
             ztot += (int(nbytes) + 15) // 16 * 16
 
@@ -272,28 +284,30 @@ class TrainEngine:
 
         bf16 = self._bf
         for i, op in enumerate(g.ops):
-            if op.kind == "pool":
+            if op.kind == "pool" or not self._planned(op):
                 continue
             W = self.wts[i] = {}
             if op.kind == "pred":
                 ch, cin, chp = op.cout, op.cin, (op.cout + 15) // 16 * 16
                 W["w"] = bf16(ch, 1, 1, cin)
                 W["bias"] = ops.bias_buffer(ch, dev)
-                W["wt"] = bf16(cin, 1, 1, chp)                                   # dgrad: [Cin][ch_pad], zero padded
                 wsrc, bsrc = fl.ptr(op.name + ".weight"), fl.ptr(op.name + ".bias")
                 pack.append(_seg(W["w"].data_ptr(), wsrc, [ch * cin], [1], [1], XF_BF16, XF_F32))
                 pack.append(_seg(W["bias"].data_ptr(), bsrc, [ch], [1], [1], XF_F32, XF_F32))
-                pack.append(_seg(W["wt"].data_ptr(), wsrc, [cin, ch], [chp, 1], [1, cin], XF_BF16, XF_F32))
+                if not self.teacher:
+                    W["wt"] = bf16(cin, 1, 1, chp)                               # dgrad: [Cin][ch_pad], zero padded
+                    pack.append(_seg(W["wt"].data_ptr(), wsrc, [cin, ch], [chp, 1], [1, cin], XF_BF16, XF_F32))
                 self.ctx[i] = dict(w=W["w"])
                 continue
             if op.kind == "convT":
                 co, ci = op.cout, op.cin
                 W["w"] = bf16(4, co, 1, 1, ci)                                   # quadrant q = dy*2+dx: [Cout][Cin]
-                W["wt"] = bf16(4, ci, 1, 1, co)                                  # dgrad of quadrant q: [Cin][Cout]
                 W["bias"] = ops.bias_buffer(co, dev)
                 wsrc = fl.ptr(op.name + ".upsample_transpose.weight")            # [Cin][Cout][2][2]
                 pack.append(_seg(W["w"].data_ptr(), wsrc, [4, co, ci], [co * ci, ci, 1], [1, 4, co * 4], XF_BF16, XF_F32))
-                pack.append(_seg(W["wt"].data_ptr(), wsrc, [4, ci, co], [ci * co, co, 1], [1, co * 4, 4], XF_BF16, XF_F32))
+                if not self.teacher:
+                    W["wt"] = bf16(4, ci, 1, 1, co)                              # dgrad of quadrant q: [Cin][Cout]
+                    pack.append(_seg(W["wt"].data_ptr(), wsrc, [4, ci, co], [ci * co, co, 1], [1, co * 4, 4], XF_BF16, XF_F32))
                 pack.append(_seg(W["bias"].data_ptr(), fl.ptr(op.name + ".upsample_transpose.bias"), [co], [1], [1], XF_F32, XF_F32))
                 self.ctx[i] = dict(w=[W["w"][q] for q in range(4)])
                 continue
@@ -302,7 +316,8 @@ class TrainEngine:
             nb, co, ci = len(br), op.cout, op.cin
             # QA blocks: stats [0] = BN_d (rbr_dense.bn), [1] = the post-sum bn; coef [0] / [1] = their backward coefficients
             self.stat_out[i] = torch.zeros(nb, 4, co, dtype=torch.float32, device=dev)
-            self.coef_out[i] = torch.zeros(nb, 2, co, dtype=torch.float32, device=dev)
+            if not self.teacher:
+                self.coef_out[i] = torch.zeros(nb, 2, co, dtype=torch.float32, device=dev)
             W["br"] = []
             for b, (prefix, k) in enumerate(br):
                 ent = dict(prefix=prefix, k=k, w=None)
@@ -321,6 +336,9 @@ class TrainEngine:
                 kk = k * k
                 ent["w"] = bf16(co, k, k, ci)                                    # forward: KRSC
                 pack.append(_seg(ent["w"].data_ptr(), wsrc, [co, kk, ci], [kk * ci, ci, 1], [ci * kk, 1, kk], XF_BF16, XF_F32))
+                W["br"].append(ent)
+                if self.teacher:
+                    continue
                 if op.s == 1:   # dgrad = conv with the 180-degree rotated, transposed filter [Cin][k][k][Cout]
                     ent["wt"] = [bf16(ci, k, k, co)]
                     pack.append(_seg(ent["wt"][0].data_ptr(), wsrc + 4 * (kk - 1), [ci, kk, co], [kk * co, co, 1], [kk, -1, ci * kk],
@@ -338,9 +356,12 @@ class TrainEngine:
                             pack.append(_seg(wt.data_ptr(), wsrc + 4 * (r0 * 3 + c0), [ci, nr, ncol, co],
                                              [nr * ncol * co, ncol * co, co, 1], [9, 3 * dr, dc, ci * 9], XF_BF16, XF_F32))
                             ent["wt"].append(wt)
-                W["br"].append(ent)
             self.ctx[i] = dict(branches=[dict(prefix=e["prefix"], k=e["k"], w=e["w"], x=None) for e in W["br"]])
         self.pack_table = XformTable(pack, dev)
+        self._zero_bytes = ztot
+        if self.teacher:
+            self.grad_tables, self.bucket_range = [], []
+            return
 
         # ---- gradient unpack table, in backward order = flat gradient order; buckets = contiguous op ranges
         ops_with_params = [i for i in range(len(g.ops) - 1, -1, -1) if g.ops[i].kind != "pool"]
@@ -368,7 +389,6 @@ class TrainEngine:
         self.last_op_of_bucket = {}
         for i in ops_with_params:
             self.last_op_of_bucket[self.bucket_of_op[i]] = i      # ops are visited in backward order: the last one wins
-        self._zero_bytes = ztot
 
     def _grad_segs(self, i, op):
         """xform segments that move op i's gradients (fp32 KRSC arena / float64 sums) into the flat gradient buffer."""
@@ -450,8 +470,9 @@ class TrainEngine:
             fl = self.flat
             for b, (prefix, st) in enumerate(finalize):
                 d.gamma[b], d.beta[b] = fl.ptr(prefix + ".weight") + 4 * row0, fl.ptr(prefix + ".bias") + 4 * row0
-                d.running_mean[b] = fl.ptr(prefix + ".running_mean") + 4 * row0
-                d.running_var[b] = fl.ptr(prefix + ".running_var") + 4 * row0
+                if not self.teacher:      # a teacher's running statistics stay as they are (null: no update)
+                    d.running_mean[b] = fl.ptr(prefix + ".running_mean") + 4 * row0
+                    d.running_var[b] = fl.ptr(prefix + ".running_var") + 4 * row0
                 d.stats[b] = st.data_ptr()
         return d
 
@@ -466,7 +487,9 @@ class TrainEngine:
         q.t, q.t_pitch = t.data_ptr(), t.shape[3]
         q.sums, q.counter, q.zeroed, q.eps, q.momentum = sums_ptr, cnt_ptr, 1, BN_EPS, BN_MOMENTUM
         q.gamma, q.beta = fl.ptr(bn + ".weight"), fl.ptr(bn + ".bias")
-        q.running_mean, q.running_var, q.stats = fl.ptr(bn + ".running_mean"), fl.ptr(bn + ".running_var"), st[1].data_ptr()
+        q.stats = st[1].data_ptr()
+        if not self.teacher:
+            q.running_mean, q.running_var = fl.ptr(bn + ".running_mean"), fl.ptr(bn + ".running_var")
         return q
 
     def _dgrad_descs(self, dc, ent, stride, gsrc, g_off):
@@ -482,6 +505,10 @@ class TrainEngine:
     def _bf(self, *shape):
         return torch.zeros(*shape, dtype=torch.bfloat16, device=self.dev)
 
+    def _planned(self, op):
+        """False for the pred convs a teacher leaves out: every head but the anchor-free cls / reg pair."""
+        return not (self.teacher and op.kind == "pred" and op.head[0] not in ("cls", "reg"))
+
     def _view(self, t):
         return self.bufs[t.buf], self.gbufs[t.buf]
 
@@ -492,14 +519,16 @@ class TrainEngine:
                 d.res, d.alpha = 0, 0.0
         return _desc_launch("conv", "yv6_conv_fwd", d, writes=[Write(op.src.buf, op.src.c_off, op.cin, full, assign, group)])
 
-    def _plan(self, N, H, W, in_dtype):
+    def _plan(self, N, H, W, in_dtype, x_static=None):
+        """Plans the step for one input shape.  x_static: an existing [N,3,H,W] input buffer for the stem to read (a teacher reads
+        its student's), instead of one of the engine's own."""
         key = (N, H, W, in_dtype)
-        if self._shape == key:
+        if self._shape == key and (x_static is None or x_static is self.x_static):
             return
         self._shape = key
         g, dev = self.g, self.dev
         self.bufs = [self._bf(N, H >> b.level, W >> b.level, b.c_total) for b in g.bufs]
-        self.gbufs = [torch.zeros_like(t) for t in self.bufs]
+        self.gbufs = [None] * len(self.bufs) if self.teacher else [torch.zeros_like(t) for t in self.bufs]
         self.sizes = [(H // s, W // s) for s in g.strides]
         self.offs = [0]
         for h, w in self.sizes:
@@ -507,6 +536,15 @@ class TrainEngine:
         A = self.offs[-1]
         self.cls = torch.empty(N, A, g.num_classes, dtype=torch.float32, device=dev)
         self.reg = torch.empty(N, A, 4 * (g.reg_max + 1), dtype=torch.float32, device=dev)
+        self.x_static = x_static if x_static is not None else torch.zeros(N, 3, H, W, dtype=in_dtype, device=dev)   # graph-stable address
+        self.fwd_calls = []
+        planners = {"pool": self._plan_pool, "pred": self._plan_pred, "convT": self._plan_convT}
+        if self.teacher:                      # forward launches only: every planner returns no backward launches
+            for i, op in enumerate(g.ops):
+                if self._planned(op):
+                    planners.get(op.kind, self._plan_bn_block)(i, op)
+            self.bwd_calls, self.zero_gbufs = [], []
+            return
         self.grad_cls = torch.zeros_like(self.cls)
         self.grad_reg = torch.zeros_like(self.reg)
         if getattr(g, "distill_ns", False):   # N / S distillation student: DFL logits next to the 4 lrtb distances
@@ -519,11 +557,8 @@ class TrainEngine:
             self.grad_cls_ab = torch.zeros_like(self.cls_ab)
             self.grad_reg_ab = torch.zeros_like(self.reg_ab)
             self._ab = {}                     # level -> {"cls_ab" / "reg_ab": (fp32 conv output, bf16 gradient)}
-        self.x_static = torch.zeros(N, 3, H, W, dtype=in_dtype, device=dev)   # the stem reads this buffer (graph-stable address)
         self.scratch = _Scratch(dev, max([N * (H >> g.bufs[op.dst.buf].level) * (W >> g.bufs[op.dst.buf].level) * op.cout
                                           for op in g.ops if op.kind in ("conv", "stem")] + [1]))
-        planners = {"pool": self._plan_pool, "pred": self._plan_pred, "convT": self._plan_convT}
-        self.fwd_calls = []
         bwd_of_op = [planners.get(op.kind, self._plan_bn_block)(i, op) for i, op in enumerate(g.ops)]
         self.bwd_calls = []
         for i in range(len(g.ops) - 1, -1, -1):
@@ -541,6 +576,8 @@ class TrainEngine:
         n, h, w, ct = buf.shape
         c = op.cin
         self.fwd_calls.append(Launch("pool", "yv6_sppf_pool", (buf.data_ptr(), n, h, w, c, ct, 1, 0)))
+        if self.teacher:
+            return []
         scr = self.scratch.grown(self.scratch.pool, n * h * w * c, 1, torch.float32)[0]
         bwd = []
         for j in (3, 2, 1):
@@ -561,6 +598,13 @@ class TrainEngine:
         N, A, ch = src.shape[0], self.offs[-1], op.cout
         lh, lw = self.sizes[lvl]
         chp = (ch + 15) // 16 * 16
+        if not which.endswith("_ab"):
+            out = {"cls": self.cls, "reg": self.reg, "reg_dist": getattr(self, "reg_dist", None)}[which]
+            self.fwd_calls.append(_desc_launch("conv", "yv6_conv_fwd", self._conv_desc(src, op.src.c_off, Wt["w"], out, bias=Wt["bias"],
+                                                                                      act=op.act, y_strides=(A * ch, lw * ch, ch),
+                                                                                      y_elem_off=self.offs[lvl] * ch)))
+            if self.teacher:
+                return []
         dl = self._bf(N, lh, lw, chp)               # bf16 gradient of the conv's output, zero padded to chp channels
         self.scratch.dl.append(dl)
         bwd = []
@@ -583,11 +627,7 @@ class TrainEngine:
                                                               raw_r.data_ptr(), N, lh * lw, *rows, dl_c.shape[3], dl_r.shape[3],
                                                               dl_c.data_ptr(), dl_r.data_ptr())))
         else:
-            out, grad = {"cls": (self.cls, self.grad_cls), "reg": (self.reg, self.grad_reg),
-                         "reg_dist": (getattr(self, "reg_dist", None), getattr(self, "grad_reg_dist", None))}[which]
-            self.fwd_calls.append(_desc_launch("conv", "yv6_conv_fwd", self._conv_desc(src, op.src.c_off, Wt["w"], out, bias=Wt["bias"],
-                                                                                      act=op.act, y_strides=(A * ch, lw * ch, ch),
-                                                                                      y_elem_off=self.offs[lvl] * ch)))
+            grad = {"cls": self.grad_cls, "reg": self.grad_reg, "reg_dist": getattr(self, "grad_reg_dist", None)}[which]
             bwd.append(Launch("hgp", "yv6_head_grad_prep", (grad.data_ptr(), self.cls.data_ptr() if which == "cls" else 0, N, A, ch,
                                                              self.offs[lvl], lh * lw, chp, dl.data_ptr())))
         bwd.append(_desc_launch("wgrad", "yv6_conv_wgrad", self._wgrad_desc(src, op.src.c_off, op.cin, dl, 0, ch, 1, 1, z(i, "dw")), side=True))
@@ -607,6 +647,8 @@ class TrainEngine:
             self.fwd_calls.append(_desc_launch("conv", "yv6_conv_fwd", self._conv_desc(
                 src, op.src.c_off, Wt["w"][q], dst, op.dst.c_off, bias=Wt["bias"], y_strides=(dh * dw * dct, 2 * dw * dct, 2 * dct),
                 y_elem_off=(dy * dw + dx) * dct)))
+        if self.teacher:
+            return []
         gd = gdst[..., op.dst.c_off:op.dst.c_off + op.cout]
         # bias gradient = column sums of the whole upsampled gradient slice
         bwd = [_desc_launch("stats", "yv6_bn_stats_finalize", self._stats_desc([(gdst, op.dst.c_off)], op.cout, N * dh * dw, z(i, "bsum"),
@@ -626,7 +668,7 @@ class TrainEngine:
     def _plan_bn_block(self, i, op):
         """BatchNorm-ed block (stem / rep / cba / cm / qa): raw convs of its branches -> batch statistics -> BN apply +
         activation.  Backward: BN backward into the dc scratch pair of the block's parity, then _plan_branch_grads."""
-        z, sc = self._z, self.scratch
+        z = self._z
         dst, gdst = self._view(op.dst)
         src, gsrc = self._view(op.src) if op.kind != "stem" else (None, None)
         n, ho, wo, dct = dst.shape
@@ -653,14 +695,25 @@ class TrainEngine:
             fin = [(ent["prefix"] + (".bn" if ent["k"] else ""), st[b]) for b, ent in enumerate(br)]
             self.fwd_calls.append(_desc_launch("stats", "yv6_bn_stats_finalize", self._stats_desc(
                 xs, op.cout, count, z(i, "fsum"), z(i, "fcnt"), fin, op.w_row0)))
-        par, sc.bn_ops = sc.bn_ops & 1, sc.bn_ops + 1
         d = BnDesc()
         d.nb, d.act, d.C, d.pixels = len(xs), ACT_CODES[op.act], op.cout, count
-        dcs, writes = [], []     # writes: the gradient slices this launch writes besides the scratch tensors
         for b, (t, off) in enumerate(xs):
             d.x[b], d.x_pitch[b] = t.data_ptr() + off * 2, t.shape[3]
             d.mean[b], d.invstd[b] = st[b, 0].data_ptr(), st[b, 1].data_ptr()
             d.scale[b], d.shift[b] = st[b, 2].data_ptr(), st[b, 3].data_ptr()
+        d.y, d.y_pitch = dst.data_ptr() + op.dst.c_off * 2, dct
+        if op.res is not None:
+            rbuf, grbuf = self._view(op.res)
+            d.res, d.res_pitch, d.res_alpha = rbuf.data_ptr() + op.res.c_off * 2, rbuf.shape[3], 1.0
+            if op.alpha in self.params:
+                d.res_alpha_dev = self.flat.ptr(op.alpha)
+        self.fwd_calls.append(_desc_launch("apply", "yv6_bn_apply_fwd", d))
+        if self.teacher:
+            return []
+        sc = self.scratch        # the backward launch runs on the same descriptor
+        par, sc.bn_ops = sc.bn_ops & 1, sc.bn_ops + 1
+        dcs, writes = [], []     # writes: the gradient slices this launch writes besides the scratch tensors
+        for b in range(len(xs)):
             d.s2[b] = z(i, "s2") + 8 * b * op.cout
             if br[b]["k"] == 0:      # identity branch: its input gradient goes straight into g(src)
                 d.dx[b], d.dx_pitch[b], d.accumulate[b] = gsrc.data_ptr() + op.src.c_off * 2, gsrc.shape[3], 1
@@ -673,18 +726,12 @@ class TrainEngine:
                 dc = sc.dc_view(par, len([t for t in dcs if t is not None]), (n, ho, wo, op.cout))
                 d.dx[b], d.dx_pitch[b], d.accumulate[b] = dc.data_ptr(), op.cout, 0
                 dcs.append(dc)
-        d.y, d.y_pitch = dst.data_ptr() + op.dst.c_off * 2, dct
         d.dy, d.dy_pitch = gdst.data_ptr() + op.dst.c_off * 2, dct
         d.s1 = z(i, "s1")
         d.work, d.counter, d.coef, d.zeroed = z(i, "work"), z(i, "bcnt"), self.coef_out[i].data_ptr(), 1
         if op.res is not None:
-            rbuf, grbuf = self._view(op.res)
-            d.res, d.res_pitch, d.res_alpha = rbuf.data_ptr() + op.res.c_off * 2, rbuf.shape[3], 1.0
-            if op.alpha in self.params:
-                d.res_alpha_dev = self.flat.ptr(op.alpha)
             d.dres, d.dres_pitch, d.dalpha = grbuf.data_ptr() + op.res.c_off * 2, grbuf.shape[3], z(i, "dalpha")
             writes.append(Write(op.res.buf, op.res.c_off, op.cout, True, lambda a: setattr(d, "dres_assign", int(a))))
-        self.fwd_calls.append(_desc_launch("apply", "yv6_bn_apply_fwd", d))
         bwd = [_desc_launch("bn_bwd", "yv6_bn_bwd", d, kernels=2, parity=par, writes=writes,
                             snapshot=(i, gdst[..., op.dst.c_off:op.dst.c_off + op.cout]))]
         if op.layout == "qa":
@@ -822,7 +869,8 @@ class TrainEngine:
             self.x_static.copy_(x)
         sp = _lib.stream_ptr()
         self.begin_step(sp)
-        self.flat.iflat.add_(1)                     # BatchNorm.num_batches_tracked
+        if not self.teacher:
+            self.flat.iflat.add_(1)                 # BatchNorm.num_batches_tracked
         self.run_forward(sp)
         return self.cls, self.reg
 
@@ -900,6 +948,10 @@ class TrainEngine:
         if overlap:
             wait_pending()      # every call (and every captured graph segment) ends joined
 
+    def neck_outputs(self):
+        """The neck outputs of the last forward as NCHW fp32 copies (the reference's `featmaps`, yolo.py:37-39)."""
+        return [self.bufs[t.buf][..., t.c_off:t.c_off + t.c].permute(0, 3, 1, 2).float().contiguous() for t in self.g.feat]
+
     def bucket_call_index(self):
         """Indices into the backward call list right after each bucket's unpack (segment boundaries for graph capture)."""
         return [j + 1 for j, c in enumerate(self.bwd_calls) if c.bucket is not None]
@@ -920,9 +972,7 @@ class _HeadFn(torch.autograd.Function):
         if getattr(engine.g, "distill_ns", False):
             heads += [engine.reg_dist.clone()]
         ctx.n_heads = len(heads)
-        feats = []
-        if engine.external_feat_grads:       # neck outputs, NCHW fp32 copies (reference `featmaps`, yolo.py:37-39)
-            feats = [engine.bufs[t.buf][..., t.c_off:t.c_off + t.c].permute(0, 3, 1, 2).float().contiguous() for t in engine.g.feat]
+        feats = engine.neck_outputs() if engine.external_feat_grads else []
         return (*heads, *feats)
 
     @staticmethod
