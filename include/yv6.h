@@ -277,6 +277,52 @@ int yv6_pr_metric(yv6_handle* h, const yv6_pr_state* st, int32_t n_images, const
                   int64_t workspace_bytes, double* out, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * COCO box mAP (pycocotools COCOeval, iouType 'bbox', default Params) over a dataset, in float64, as the reference's
+ * Evaler.eval_model computes it (core/evaler.py:231-321).  Images are slots 0 .. n_images - 1 in np.unique(imgIds) order,
+ * categories 0 .. n_cats - 1 the sorted gt category ids.  The caller owns every buffer: the gt table (uploaded once) and
+ * the per-(slot, row) accumulators; it zeroes ndet and flags before the first image.  Area ranges, IoU and recall
+ * thresholds are Params' float64 values, copied to the device by the caller.
+ *
+ * yv6_coco_update: one launch per batch on the batched NMS tensors.  det [B,max_det,6] / count [B] as yv6_nms_batched writes
+ *   them, meta [B,6] as for yv6_eval_boxes, cls_cat [n_cls] int32 (class -> category index, -1: not a gt category),
+ *   slots [B] int32 (-1: image not evaluated).  Each row becomes the detection pycocotools reads back from the Evaler's
+ *   predictions.json: yv6_eval_boxes' box, then x_r = rint(x * 1e3) / 1e3 and s_r = rint(conf * 1e5) / 1e5 in double
+ *   (round(v, 3) / round(v, 5) and a json round trip), area = w_r * h_r.
+ * yv6_coco_load: the same for result rows given as doubles: rows [n][6] = (x, y, w, h, score, category index), grouped by
+ *   image in result order, image b owning rows row_off[b] .. row_off[b+1] - 1 (at most state max_det).
+ * Both then match per (image, category): stable sort by descending score, the first 100 kept, bbIou against the pair's gts
+ *   and the greedy match of evaluateImg for every (area range, IoU threshold); bit a * 10 + t of tp / fp holds the
+ *   outcome, rank the detection's place in its pair (255: beyond the 100 kept).  flags[0] bit 1: a detection class
+ *   outside [0, n_cls) or not whole.
+ * yv6_coco_accumulate: COCOeval.accumulate over every slot: precision and scores [10][101][n_cats][4][3], recall
+ *   [10][n_cats][4][3] (device float64), -1 where pycocotools leaves -1.
+ * ---------------------------------------------------------------------------------------------- */
+typedef struct yv6_coco_state {
+  int32_t n_images, n_cats, max_det, max_gts;           /* max_gts: the most gts of one (image, category)                 */
+  const int32_t* gt_off;                                /* [n_images * n_cats + 1] CSR by (slot, category), file order   */
+  const double* gt_box;                                 /* [G][4] x, y, w, h                                              */
+  const double* gt_area;                                /* [G] the annotation's area field                                */
+  const uint8_t* gt_flags;                              /* [G] bit 0: iscrowd, bit 1: id != 0                             */
+  const int32_t* npig;                                  /* [n_cats][4] gts that are not ignored, per area range           */
+  const double* area_rng;                               /* [4][2]                                                         */
+  const double* iou_thrs;                               /* [10]                                                           */
+  const double* rec_thrs;                               /* [101]                                                          */
+  double* score;                                        /* [n_images][max_det] s_r                                        */
+  int32_t* cat;                                         /* [n_images][max_det] category index, -1: dropped                */
+  uint8_t* rank;                                        /* [n_images][max_det]                                            */
+  uint64_t* tp; uint64_t* fp;                           /* [n_images][max_det]                                            */
+  int32_t* ndet;                                        /* [n_images] rows stored                                         */
+  int32_t* flags;                                       /* [1]                                                            */
+} yv6_coco_state;
+int64_t yv6_coco_workspace_bytes(int32_t n_images, int32_t max_det, int32_t n_cats);
+int yv6_coco_update(yv6_handle* h, const yv6_coco_state* st, const float* det, const int32_t* count, const float* meta,
+                    const int32_t* cls_cat, int32_t n_cls, const int32_t* slots, int32_t B, int32_t max_det, void* stream);
+int yv6_coco_load(yv6_handle* h, const yv6_coco_state* st, const double* rows, const int32_t* row_off, const int32_t* slots, int32_t B,
+                  void* stream);
+int yv6_coco_accumulate(yv6_handle* h, const yv6_coco_state* st, void* workspace, int64_t workspace_bytes, double* precision,
+                        double* recall, double* scores, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Serving from decoded frames: the two steps of the reference's Inferer around the model, for a whole batch per launch.
  * Per-image geometry table geo [B][YV6_LB_GEO] int32 (device) = (src_off, h0, w0, nh, nw, top, left, 0):
  *   src_off   byte offset of the image in `src` (images packed back to back, each uint8 HWC BGR [h0][w0][3]);

@@ -121,6 +121,17 @@ class PrState(C.Structure):
     ]
 
 
+class CocoState(C.Structure):
+    """Mirror of `yv6_coco_state` (include/yv6.h)."""
+    _fields_ = [
+        ("n_images", C.c_int32), ("n_cats", C.c_int32), ("max_det", C.c_int32), ("max_gts", C.c_int32),
+        ("gt_off", C.c_void_p), ("gt_box", C.c_void_p), ("gt_area", C.c_void_p), ("gt_flags", C.c_void_p), ("npig", C.c_void_p),
+        ("area_rng", C.c_void_p), ("iou_thrs", C.c_void_p), ("rec_thrs", C.c_void_p),
+        ("score", C.c_void_p), ("cat", C.c_void_p), ("rank", C.c_void_p), ("tp", C.c_void_p), ("fp", C.c_void_p),
+        ("ndet", C.c_void_p), ("flags", C.c_void_p),
+    ]
+
+
 class DwDesc(C.Structure):
     """Mirror of `yv6_dw_desc` (include/yv6.h)."""
     _fields_ = [
@@ -244,6 +255,12 @@ _SIGNATURES = {
                                C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p]),
     "yv6_pr_metric": (C.c_int, [C.c_void_p, C.POINTER(PrState), C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p,
                                 C.c_void_p]),
+    "yv6_coco_workspace_bytes": (C.c_int64, [C.c_int32, C.c_int32, C.c_int32]),
+    "yv6_coco_update": (C.c_int, [C.c_void_p, C.POINTER(CocoState), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p,
+                                  C.c_int32, C.c_int32, C.c_void_p]),
+    "yv6_coco_load": (C.c_int, [C.c_void_p, C.POINTER(CocoState), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]),
+    "yv6_coco_accumulate": (C.c_int, [C.c_void_p, C.POINTER(CocoState), C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
+                                      C.c_void_p]),
     "yv6_dwconv_fwd": (C.c_int, [C.c_void_p, C.POINTER(DwDesc), C.c_void_p]),
     "yv6_se_fwd": (C.c_int, [C.c_void_p, C.POINTER(SeDesc), C.c_void_p]),
     "yv6_qa_fwd": (C.c_int, [C.c_void_p, C.POINTER(QaDesc), C.c_void_p]),

@@ -21,6 +21,7 @@
 #include "yv6_common.cuh"
 #include "yv6_handle.h"
 #include "yv6_scale_coords.cuh"
+#include "yv6_sort.cuh"
 
 namespace yv6 {
 
@@ -28,7 +29,6 @@ constexpr int kPrNiou = 10;
 constexpr int kPrCurve = 1000;       // np.linspace(0, 1, 1000) of ap_per_class
 constexpr int kPrAp = 101;           // np.linspace(0, 1, 101) of compute_ap
 constexpr int kMatchThreads = 256;
-constexpr int kRsThreads = 256, kRsItems = 16, kRsTile = kRsThreads * kRsItems, kRsWarps = kRsThreads / 32;
 constexpr int kApThreads = 256, kApItems = 8, kApChunk = kApThreads * kApItems;
 enum { kPrErrLabelCls = 1, kPrErrDetCls = 2, kPrErrLabels = 4 };
 
@@ -187,7 +187,7 @@ __global__ void __launch_bounds__(kMatchThreads) pr_match_kernel(PrMatchArgs a) 
 }
 
 // ------------------------------------------------------------------------------------------------
-// stable LSD radix sort of (class << 32 | ~ordered(conf)) keys, 8-bit digits
+// keys of the stable LSD radix sort (yv6_sort.cuh): (class << 32 | ~ordered(conf)) keys, 8-bit digits
 // ------------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t conf_desc_bits(float f) {
   const uint32_t u = __float_as_uint(f);
@@ -211,89 +211,6 @@ __global__ void pr_keys_kernel(yv6_pr_state st, int64_t N, uint64_t* keys, uint3
   vals[s] = (uint32_t)s;
 }
 
-__global__ void __launch_bounds__(kRsThreads) rs_hist_kernel(const uint64_t* __restrict__ keys, int64_t N, int shift, int nblk,
-                                                             uint32_t* __restrict__ hist) {
-  __shared__ uint32_t h[256];
-  h[threadIdx.x] = 0;
-  __syncthreads();
-  const int64_t base = (int64_t)blockIdx.x * kRsTile;
-  for (int i = threadIdx.x; i < kRsTile; i += kRsThreads)
-    if (base + i < N) atomicAdd(&h[(keys[base + i] >> shift) & 255], 1u);
-  __syncthreads();
-  hist[(int64_t)threadIdx.x * nblk + blockIdx.x] = h[threadIdx.x];
-}
-
-// exclusive scan of n counters in one CTA (n = 256 * blocks of the sort, a few hundred thousand at most)
-__global__ void __launch_bounds__(1024) rs_scan_kernel(uint32_t* __restrict__ v, int64_t n) {
-  __shared__ uint32_t s_w[32];
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int64_t per = (n + 1023) / 1024, lo = min(n, (int64_t)tid * per), hi = min(n, lo + per);
-  uint32_t sum = 0;
-  for (int64_t i = lo; i < hi; ++i) sum += v[i];
-  uint32_t x = sum;
-  for (int o = 1; o < 32; o <<= 1) {
-    const uint32_t y = __shfl_up_sync(0xffffffffu, x, o);
-    if (lane >= o) x += y;
-  }
-  if (lane == 31) s_w[warp] = x;
-  __syncthreads();
-  if (warp == 0) {
-    uint32_t w = s_w[lane];
-    for (int o = 1; o < 32; o <<= 1) {
-      const uint32_t y = __shfl_up_sync(0xffffffffu, w, o);
-      if (lane >= o) w += y;
-    }
-    s_w[lane] = w;
-  }
-  __syncthreads();
-  uint32_t run = x - sum + (warp > 0 ? s_w[warp - 1] : 0);
-  for (int64_t i = lo; i < hi; ++i) {
-    const uint32_t c = v[i];
-    v[i] = run;
-    run += c;
-  }
-}
-
-// stable scatter: rounds of 256 consecutive keys; within a warp __match_any gives the rank among equal digits, warps are
-// ordered through per-warp digit counts
-__global__ void __launch_bounds__(kRsThreads) rs_scatter_kernel(const uint64_t* __restrict__ kin, const uint32_t* __restrict__ vin,
-                                                                uint64_t* __restrict__ kout, uint32_t* __restrict__ vout, int64_t N,
-                                                                int shift, int nblk, const uint32_t* __restrict__ hist) {
-  __shared__ uint32_t s_cnt[kRsWarps][256];
-  __shared__ uint32_t s_run[256];
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  s_run[tid] = hist[(int64_t)tid * nblk + blockIdx.x];
-  const int64_t base = (int64_t)blockIdx.x * kRsTile;
-  for (int r = 0; r < kRsItems; ++r) {
-#pragma unroll
-    for (int w = 0; w < kRsWarps; ++w) s_cnt[w][tid] = 0;
-    __syncthreads();
-    const int64_t i = base + (int64_t)r * kRsThreads + tid;
-    const bool valid = i < N;
-    const uint64_t k = valid ? kin[i] : 0;
-    const uint32_t d = valid ? (uint32_t)(k >> shift) & 255u : 256u;
-    const uint32_t peers = __match_any_sync(0xffffffffu, d);
-    const uint32_t rank = __popc(peers & ((1u << lane) - 1u));
-    if (valid && rank == 0) s_cnt[warp][d] = __popc(peers);
-    __syncthreads();
-    uint32_t run = s_run[tid];
-#pragma unroll
-    for (int w = 0; w < kRsWarps; ++w) {
-      const uint32_t c = s_cnt[w][tid];
-      s_cnt[w][tid] = run;
-      run += c;
-    }
-    s_run[tid] = run;
-    __syncthreads();
-    if (valid) {
-      const uint32_t pos = s_cnt[warp][d] + rank;
-      kout[pos] = k;
-      vout[pos] = vin[i];
-    }
-    __syncthreads();
-  }
-}
-
 // ------------------------------------------------------------------------------------------------
 // per (class, threshold): running TP counts, precision envelope, 101-point interpolated AP (compute_ap)
 // ------------------------------------------------------------------------------------------------
@@ -301,48 +218,6 @@ __device__ __forceinline__ int seg_start(const int32_t* npred, int c) {
   int s = 0;
   for (int k = 0; k < c; ++k) s += npred[k];
   return s;
-}
-
-// exclusive prefix sum over the CTA; returns the CTA total in *total
-__device__ __forceinline__ int block_excl_sum(int v, int* s_w, int* total) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
-  int x = v;
-  for (int o = 1; o < 32; o <<= 1) {
-    const int y = __shfl_up_sync(0xffffffffu, x, o);
-    if (lane >= o) x += y;
-  }
-  __syncthreads();
-  if (lane == 31) s_w[warp] = x;
-  __syncthreads();
-  int off = 0, tot = 0;
-  for (int w = 0; w < nw; ++w) {
-    off += w < warp ? s_w[w] : 0;
-    tot += s_w[w];
-  }
-  *total = tot;
-  return off + x - v;
-}
-
-// max over the threads with a higher index (exclusive suffix max); every value is >= 0, the empty max is 0
-__device__ __forceinline__ double block_excl_sufmax(double v, double* s_w, double* total) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
-  double x = v;
-  for (int o = 1; o < 32; o <<= 1) {
-    const double y = __shfl_down_sync(0xffffffffu, x, o);
-    if (lane + o < 32) x = fmax(x, y);
-  }
-  double nxt = __shfl_down_sync(0xffffffffu, x, 1);
-  if (lane == 31) nxt = 0.0;
-  __syncthreads();
-  if (lane == 0) s_w[warp] = x;
-  __syncthreads();
-  double later = 0.0, tot = 0.0;
-  for (int w = 0; w < nw; ++w) {
-    if (w > warp) later = fmax(later, s_w[w]);
-    tot = fmax(tot, s_w[w]);
-  }
-  *total = tot;
-  return fmax(nxt, later);
 }
 
 struct PrMetricArgs {
@@ -620,14 +495,13 @@ struct PrWs {
 };
 
 static int64_t pr_layout(int64_t N, PrWs* w, char* base) {
-  const int64_t nblk = (N + kRsTile - 1) / kRsTile;
   int64_t off = 0;
   auto take = [&](int64_t bytes) { const int64_t o = off; off += align256(bytes); return base ? base + o : (char*)nullptr; };
   w->ka = (uint64_t*)take(N * 8);
   w->kb = (uint64_t*)take(N * 8);
   w->va = (uint32_t*)take(N * 4);
   w->vb = (uint32_t*)take(N * 4);
-  w->hist = (uint32_t*)take(256 * nblk * 4);
+  w->hist = (uint32_t*)take(rs_hist_words(N) * 4);
   w->tpc0 = (int32_t*)take(N * 4);
   return off;
 }
@@ -708,13 +582,10 @@ extern "C" int yv6_pr_metric(yv6_handle* h, const yv6_pr_state* st, int32_t n_im
   a.out = out;
   if (N > 0) {
     pr_keys_kernel<<<(unsigned)((N + 255) / 256), 256, 0, s>>>(*st, N, w.ka, w.va);
-    const int nblk = (int)((N + kRsTile - 1) / kRsTile);
     uint64_t *kin = w.ka, *kout = w.kb;
     uint32_t *vin = w.va, *vout = w.vb;
     for (int shift = 0; shift < 32 || (shift < 64 && ((uint64_t)nc >> (shift - 32)) != 0); shift += 8) {
-      rs_hist_kernel<<<nblk, kRsThreads, 0, s>>>(kin, N, shift, nblk, w.hist);
-      rs_scan_kernel<<<1, 1024, 0, s>>>(w.hist, (int64_t)256 * nblk);
-      rs_scatter_kernel<<<nblk, kRsThreads, 0, s>>>(kin, vin, kout, vout, N, shift, nblk, w.hist);
+      rs_pass(kin, vin, kout, vout, N, shift, w.hist, s);
       std::swap(kin, kout);
       std::swap(vin, vout);
     }

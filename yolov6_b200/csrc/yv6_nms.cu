@@ -762,14 +762,11 @@ __global__ void eval_boxes_kernel(const float* __restrict__ det, const int32_t* 
     return;
   }
   const float* r = det + (int64_t)i * 6;
-  const float4 s = scale_coords_rn(r[0], r[1], r[2], r[3], meta + b * 6);
-  const float x1 = s.x, y1 = s.y, x2 = s.z, y2 = s.w;
-  const float xc = __fdiv_rn(__fadd_rn(x1, x2), 2.f), yc = __fdiv_rn(__fadd_rn(y1, y2), 2.f);
-  const float w = __fsub_rn(x2, x1), hh = __fsub_rn(y2, y1);
-  o[0] = __fsub_rn(xc, __fdiv_rn(w, 2.f));
-  o[1] = __fsub_rn(yc, __fdiv_rn(hh, 2.f));
-  o[2] = w;
-  o[3] = hh;
+  const float4 c = coco_xywh_rn(scale_coords_rn(r[0], r[1], r[2], r[3], meta + b * 6));
+  o[0] = c.x;
+  o[1] = c.y;
+  o[2] = c.z;
+  o[3] = c.w;
   o[4] = r[4];
   o[5] = r[5];
 }
