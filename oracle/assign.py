@@ -10,9 +10,37 @@ Everything derived from the ground truth is float64, as in the reference (its ta
 numpy float64, SURVEY.md F5).  `torch.topk` is used for the top-k steps because its tie order is
 part of what the reference observes on CPU.  Pinned against the live reference by
 tests/golden/make_golden.py.
+
+`ties="index"` replaces `torch.topk`, whose order among equal values is unspecified, by the rule the
+CUDA assigners state (yv6_assign.cu): a stable sort on (-metric, anchor index) for TAL and on
+(distance, anchor index) for ATSS, so ties go to the lower anchor index.  In that mode ATSS also
+forms the mean and the standard deviation of the candidate IoUs as the kernel does (sequential
+float64 sums over the candidates in level, then rank order), so an IoU equal to the threshold falls
+on the same side.  Duplicate top-k indices are counted with `scatter_add` there, which keeps the
+memory at [G, A] per image.
 """
 import torch
 import torch.nn.functional as F
+
+TIE_RULES = ("topk", "index")
+
+
+def _lowest_k(keys, k):
+    """Indices of the k smallest keys along the last dim, equal keys in index order."""
+    return torch.sort(keys, dim=-1, stable=True)[1][..., :k]
+
+
+def _count(idx, n):
+    """[G, k] indices -> [G, n] number of times each index occurs in its row."""
+    return torch.zeros(idx.shape[0], n, dtype=torch.int64).scatter_add_(1, idx, torch.ones_like(idx))
+
+
+def _seq_sum(x):
+    """Sum over the last dim, left to right, keepdim."""
+    s = torch.zeros_like(x[..., :1])
+    for j in range(x.shape[-1]):
+        s = s + x[..., j:j + 1]
+    return s
 
 
 def train_anchors(sizes, strides, cell_size=5.0, cell_offset=0.5, dtype=torch.float32):
@@ -59,10 +87,12 @@ def resolve_conflicts(mask_pos, overlaps):
 
 
 def tal_assign(pd_scores, pd_bboxes, anc_points, gt_labels, gt_bboxes, mask_gt, topk=13, num_classes=80,
-               alpha=1.0, beta=6.0, eps=1e-9):
+               alpha=1.0, beta=6.0, eps=1e-9, ties="topk"):
     """pd_scores [B,A,nc] f32, pd_bboxes [B,A,4] f32 (pixels), anc_points [A,2], gt_labels [B,G,1],
     gt_bboxes [B,G,4] f64, mask_gt [B,G,1].  Returns labels i64 [B,A], bboxes [B,A,4], scores
-    [B,A,nc], fg bool [B,A], gt_idx i64 [B,A]."""
+    [B,A,nc], fg bool [B,A], gt_idx i64 [B,A].  `ties`: see the module docstring."""
+    if ties not in TIE_RULES:
+        raise ValueError(f"ties={ties!r}")
     B, A, _ = pd_scores.shape
     G = gt_bboxes.shape[1]
     if G == 0:  # tal_assigner.py:48-53
@@ -77,9 +107,12 @@ def tal_assign(pd_scores, pd_bboxes, anc_points, gt_labels, gt_bboxes, mask_gt, 
         sc = pd_scores[b].T[gl]                                          # :123-128 (label -1 -> last class)
         al = sc.pow(alpha) * ov.pow(beta)                                # :131
         ing = centres_in_gts(anc_points, gb)                             # :108
-        _, idx = torch.topk(al * ing, topk, dim=-1, largest=True)        # :141-142
+        if ties == "index":
+            idx = _lowest_k(-(al * ing), topk)
+        else:
+            _, idx = torch.topk(al * ing, topk, dim=-1, largest=True)    # :141-142
         idx = torch.where(mg.bool().expand(-1, topk), idx, torch.zeros_like(idx))
-        cnt = F.one_hot(idx, A).sum(-2)
+        cnt = _count(idx, A) if ties == "index" else F.one_hot(idx, A).sum(-2)
         in_topk = torch.where(cnt > 1, torch.zeros_like(cnt), cnt).to(al.dtype)   # :146-149
         mask_pos = in_topk * ing * mg                                    # :113
         gt_idx, fg, mask_pos = resolve_conflicts(mask_pos, ov)
@@ -108,8 +141,11 @@ def bbox_overlaps_max_eps(b1, b2, eps=1e-6):
     return inter / union
 
 
-def atss_assign(anc_bboxes, n_level, gt_labels, gt_bboxes, mask_gt, pd_bboxes, topk=9, num_classes=80):
-    """ATSSAssigner.forward.  Returns labels i64 [B,A] (bg = num_classes), bboxes, scores f32->f64, fg."""
+def atss_assign(anc_bboxes, n_level, gt_labels, gt_bboxes, mask_gt, pd_bboxes, topk=9, num_classes=80, ties="topk"):
+    """ATSSAssigner.forward.  Returns labels i64 [B,A] (bg = num_classes), bboxes, scores f32->f64, fg, gt_idx.
+    `ties`: see the module docstring."""
+    if ties not in TIE_RULES:
+        raise ValueError(f"ties={ties!r}")
     B, G = gt_bboxes.shape[:2]
     A = anc_bboxes.shape[0]
     if G == 0:  # atss_assigner.py:45-50
@@ -128,17 +164,25 @@ def atss_assign(anc_bboxes, n_level, gt_labels, gt_bboxes, mask_gt, pd_bboxes, t
         cand_mask, cand_idx, start = [], [], 0
         for n in n_level:                                                     # :88-116
             k = min(topk, n)
-            _, idx = dist[:, start:start + n].topk(k, dim=-1, largest=False)
+            if ties == "index":
+                idx = _lowest_k(dist[:, start:start + n], k)
+            else:
+                _, idx = dist[:, start:start + n].topk(k, dim=-1, largest=False)
             cand_idx.append(idx + start)
             idx = torch.where(mg.bool().expand(-1, k), idx, torch.zeros_like(idx))
-            cnt = F.one_hot(idx, n).sum(-2)
+            cnt = _count(idx, n) if ties == "index" else F.one_hot(idx, n).sum(-2)
             cand_mask.append(torch.where(cnt > 1, torch.zeros_like(cnt), cnt).to(dist.dtype))
             start += n
         is_cand = torch.cat(cand_mask, -1)
         cand_idx = torch.cat(cand_idx, -1)
         cov = torch.where(is_cand > 0, ov, torch.zeros_like(ov))              # :124-125
         sel = torch.gather(cov, 1, cand_idx)
-        thr = sel.mean(-1, keepdim=True) + sel.std(-1, keepdim=True)          # :132-134
+        if ties == "index":
+            n_c = sel.shape[-1]
+            mean = _seq_sum(sel) / n_c
+            thr = mean + (_seq_sum((sel - mean) * (sel - mean)) / (n_c - 1)).sqrt()
+        else:
+            thr = sel.mean(-1, keepdim=True) + sel.std(-1, keepdim=True)      # :132-134
         is_pos = torch.where(cov > thr, is_cand, torch.zeros_like(is_cand))   # :65-67
         mask_pos = is_pos * centres_in_gts(ac.to(gb.dtype), gb) * mg          # :69-70
         gt_idx, fg, mask_pos = resolve_conflicts(mask_pos, ov)
