@@ -3,7 +3,10 @@
 `test_train_step_matches_reference_op_by_op` checks whole buffers at 1e-2 relative L2, which a wrong edge column or a wrong tap
 in the border pixels of one dgrad parity does not move.  Here the engine plans a step -- YOLOv6-N / M / L6 at 96-128 px, N-QA
 (the QA block's qa_bwd and its second bn_bwd on BN_d), N with the fuse_ab head (head_ab_grad), and the shapes the benchmark
-trains: YOLOv6-S at 640, batch 32, uint8 input, and YOLOv6-M at 640, batch 8 -- and every launch of its backward call list --
+trains: YOLOv6-S at 640, batch 32, uint8 input, and YOLOv6-M at 640, batch 8; the N / S self-distillation student at the
+distillation benchmark's shape (S, 640, batch 32, uint8: the reg_preds_dist pred conv's 68-channel head gradient, its wgrad,
+bias sums and a dgrad accumulating into the lrtb pred's input gradient); M with external neck-output gradients (every writer
+of those slices accumulates) -- and every launch of its backward call list --
 dgrad convs (grouped per op and branch: four parity launches for a 3x3 stride-2 conv, one for 1x1 stride 2), weight
 gradients, BatchNorm backward (with the BottleRep shortcut), qa_bwd, the sums-only statistics of the pred and ConvTranspose
 bias gradients, the head-gradient repacks, the SPPF max-pool backward chain and the stem im2col -- runs on its own descriptor:
@@ -64,6 +67,10 @@ MODELS = {
     "yolov6l6": dict(cfg="yolov6l6", size=128, batch=2), "yolov6n_qa": dict(cfg="yolov6n_qa", size=96, batch=2),
     "yolov6n_fuse_ab": dict(cfg="yolov6n", size=128, batch=2, fuse_ab=True),
     "yolov6s_640_b32_u8": dict(cfg="yolov6s", size=640, batch=32, u8=True), "yolov6m_640_b8": dict(cfg="yolov6m", size=640, batch=8),
+    # the N / S self-distillation student (third pred conv per level, reg_preds_dist) at the shape tools/bench_distill.py
+    # trains, and M with the neck outputs' gradients injected by the channel-wise distillation term
+    "yolov6s_640_b32_u8_distill_ns": dict(cfg="yolov6s", size=640, batch=32, u8=True, distill_ns=True),
+    "yolov6m_96_b2_feat": dict(cfg="yolov6m", size=96, batch=2, feat=True),
 }
 GOLDEN_KEYS = ("yolov6n", "yolov6s", "yolov6m", "yolov6l6")
 BN_EPS = 1e-3
@@ -694,22 +701,37 @@ def check_im2col(lib, h, sp, img_ptr, img, x_dt, scale, N, H, W, patches, patche
 
 
 # ---------------------------------------------------------------------------------------------------------------- the engine's launches
+def seeded_model(cfg, dev, fuse_ab=False, distill_ns=False, dfl=False):
+    """The model with seeded weights: the fabricated golden state of its config where golden keys exist, else randomize_.  A
+    distill_ns student (and a DFL-head teacher, `dfl`) has the DFL head: its weights are fabricated over the model's own keys."""
+    from yolov6_b200 import configs
+    from yolov6_b200.model import build_model
+    from yolov6_b200.synth import randomize_
+    spec = cfg
+    if distill_ns or dfl:
+        spec = configs.get_config(cfg)
+        spec["head"]["use_dfl"], spec["head"]["reg_max"] = True, 16
+    m = build_model(spec, 80, dev, fuse_ab=fuse_ab, distill_ns=distill_ns)
+    if distill_ns or dfl:
+        m.load_state_dict(fab.fabricate_state_dict([(k, tuple(v.shape)) for k, v in m.state_dict().items()], seed=0))
+    elif cfg in GOLDEN_KEYS:
+        m.load_state_dict(fab.fabricate_state_dict(golden_keys(cfg + ("_fuseab" if fuse_ab else "")), seed=0))
+    else:
+        randomize_(m, seed=0)
+    return m
+
+
 @functools.lru_cache(maxsize=1)
 def _engine(name):
     """The model's training engine, planned at the configuration's shape, and its master weights: the fabricated ones and
     integers in [-2, 2] (use_weights repacks one set or the other)."""
-    from yolov6_b200.model import build_model
-    from yolov6_b200.synth import randomize_
     c = MODELS[name]
-    size, batch, cfg, fuse_ab = c["size"], c["batch"], c["cfg"], c.get("fuse_ab", False)
+    size, batch = c["size"], c["batch"]
     dev = torch.device("cuda:0")
-    m = build_model(cfg, 80, dev, fuse_ab=fuse_ab)
-    if cfg in GOLDEN_KEYS:
-        m.load_state_dict(fab.fabricate_state_dict(golden_keys(cfg + ("_fuseab" if fuse_ab else "")), seed=0))
-    else:
-        randomize_(m, seed=0)
+    m = seeded_model(c["cfg"], dev, fuse_ab=c.get("fuse_ab", False), distill_ns=c.get("distill_ns", False))
     m.train()
     eng = m.train_engine()
+    eng.external_feat_grads = bool(c.get("feat"))      # before planning, as TrainStep sets it for distill_feat
     x = fab.synthetic_images(batch, size, size, seed=11)
     if c.get("u8"):
         x = (x * 255).round().to(torch.uint8)
@@ -740,6 +762,8 @@ def engine_mem(eng):
     named += [("dc", t) for t in sc.dc] + [("dq", t) for q in sc.quad for t in q] + [("poolscr", t) for p in sc.pool for t in p]
     named += [("stat", t) for t in eng.stat_out.values()] + [("coef", t) for t in eng.coef_out.values()]
     named += [("head", t) for t in (eng.cls, eng.reg, eng.grad_cls, eng.grad_reg)] + [("img", eng.x_static)]
+    if getattr(eng.g, "distill_ns", False):
+        named += [("head", t) for t in (eng.reg_dist, eng.grad_reg_dist)]
     named += [("dl", t) for t in sc.dl]
     named += [("patch", t) for t in getattr(eng, "_stem_patches", ())]
     named += [("raw", br["x"]) for ctx in eng.ctx if ctx and "branches" in ctx for br in ctx["branches"] if br["k"]]

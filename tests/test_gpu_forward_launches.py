@@ -42,8 +42,9 @@ depthwise, copy and decode kernels compute each output element in one thread.  A
 finished reads the sentinel left in its input and is off by ~2^100.
 
 Part 3 (test_every_training_forward_launch_matches_float64).  The same per-launch pattern over the training engine's forward
-launch records (eng.fwd_calls) for YOLOv6-N / M / L6 (the backward test's set-up), N-QA, N with the fuse_ab head and S at
-640, batch 32.  Each distinct descriptor runs once on fresh seeded inputs; the elements it computes first hold the sentinel,
+launch records (eng.fwd_calls) for YOLOv6-N / M / L6 (the backward test's set-up), N-QA, N with the fuse_ab head, S at
+640, batch 32, and the N / S self-distillation student at the same shape (its reg_preds_dist pred conv writes fp32 rows of
+A * 68).  Each distinct descriptor runs once on fresh seeded inputs; the elements it computes first hold the sentinel,
 and every other element of the tensors it writes must keep its value bit for bit.  Kinds and references:
   raw branch conv (no bias, no activation, bf16), head / fuse_ab pred (bias, sigmoid, fp32), ConvTranspose quadrant: the
     conv bars above;
@@ -686,21 +687,16 @@ TRAIN_CONFIGS = {
     "yolov6n": ("yolov6n", 128, 2, False), "yolov6m": ("yolov6m", 96, 2, False), "yolov6l6": ("yolov6l6", 128, 2, False),
     "yolov6n_qa": ("yolov6n_qa", 96, 2, False), "yolov6n_fuse_ab": ("yolov6n", 128, 2, True),
     "yolov6s_640_b32": ("yolov6s", 640, 32, False),
+    # the N / S self-distillation student: a third pred conv per level (reg_preds_dist), fp32 rows of A * 68
+    "yolov6s_640_b32_distill_ns": ("yolov6s", 640, 32, False, True),
 }
 TRAIN_KINDS = ("stem", "conv", "stats", "apply", "qa", "pool", "abp")
 
 
-def train_engine(cfg, size, batch, fuse_ab):
+def train_engine(cfg, size, batch, fuse_ab, distill_ns=False):
     """The training engine of a model with seeded weights, planned for [batch, 3, size, size] fp32 images (as the backward test)."""
-    from yolov6_b200.model import build_model
-    from yolov6_b200.synth import randomize_
     dev = torch.device("cuda:0")
-    m = build_model(cfg, 80, dev, fuse_ab=fuse_ab)
-    keys = cfg + ("_fuseab" if fuse_ab else "")
-    if cfg in GOLDEN_KEYS:
-        m.load_state_dict(fab.fabricate_state_dict(golden_keys(keys), seed=0))
-    else:
-        randomize_(m, seed=0)
+    m = bwd.seeded_model(cfg, dev, fuse_ab=fuse_ab, distill_ns=distill_ns)
     m.train()
     eng = m.train_engine()
     with torch.no_grad():

@@ -34,8 +34,12 @@ References and bars (per element unless said otherwise):
 A lost row, a wrong class column, a dropped focal-weight gradient, a wrong tie rule or a lost grid-stride iteration moves a
 value by O(its size), far above every bar.  The float64 references run in torch on the GPU; assignment oracles on the CPU.
 
+ComputeLossNS's second det_loss call (the IoU term of the lrtb branch against the first call's assignment: weights
+(0, 2.5, 0), reg_ch = 4, division by target_scores_sum whenever it is > 0) runs on the assignment of a DFL first call at the
+same shapes: the box term under the bars above, out[2] and out[3] exactly 0, and the class gradient it writes all zero.
+
 Then, on whole forward_backward calls: padding G from the largest per-image count up to 64 changes no output bit; two runs
-are bit-identical; with an image of 70 boxes gt_count reports the overflow TrainStep.overflowed reads, and that image's
+are bit-identical; the lrtb call with reuse= leaves the first call's outputs bit for bit; with an image of 70 boxes gt_count reports the overflow TrainStep.overflowed reads, and that image's
 assignment is the oracle's on its first 64 rows in input order.
 """
 import ctypes as C
@@ -193,7 +197,7 @@ def run_assign(c, gt, pboxes, topk, kind):
     return gi, fg, norm, mask
 
 
-def run_det_loss(c, distri, gt, gi, fg, norm, iou, ngz, gscale):
+def run_det_loss(c, distri, gt, gi, fg, norm, iou, ngz, gscale, weights=(W_CLS, W_IOU, W_DFL)):
     from yolov6_b200 import _lib
     l, h, sp, check = lib()
     A, R = distri.shape[1], distri.shape[2]
@@ -204,7 +208,8 @@ def run_det_loss(c, distri, gt, gi, fg, norm, iou, ngz, gscale):
     d.gt = gt.data_ptr() if gt.shape[1] else 0
     d.gt_idx, d.fg, d.norm = gi.data_ptr(), fg.data_ptr(), norm.data_ptr()
     d.B, d.A, d.G, d.nc, d.reg_ch, d.iou_type = B, A, gt.shape[1], NC, R, IOU[iou]
-    d.w_cls, d.w_iou, d.w_dfl, d.grad_scale = W_CLS, W_IOU, W_DFL, gscale
+    d.w_cls, d.w_iou, d.w_dfl = weights
+    d.grad_scale = gscale
     d.grad_scores, d.grad_distri, d.out = gs.data_ptr(), gd.data_ptr(), out.data_ptr()
     d.workspace, d.workspace_bytes, d.norm_gt_zero = ws.data_ptr(), ws.numel(), ngz
     check(l.yv6_det_loss(h, C.byref(d), sp))
@@ -255,8 +260,9 @@ def assign_ref(c, gt, pboxes, topk, kind):
     return r[4], r[3], norm, r
 
 
-def loss_refs(c, distri, gt, gi, fg, norm, iou, ngz, gscale):
+def loss_refs(c, distri, gt, gi, fg, norm, iou, ngz, gscale, weights=(W_CLS, W_IOU, W_DFL)):
     """float64 references of det_loss on the values in memory: (grad_scores, bar), (grad_distri, bar), out[0..5], out bars."""
+    W_CLS, W_IOU, W_DFL = weights
     dev = norm.device
     fgb = fg.bool()
     tss = norm[fgb].sum()
@@ -520,3 +526,39 @@ def test_overflowing_image_is_reported_and_truncated_in_input_order():
     mask = (gt0[..., 1:].sum(-1, keepdim=True) > 0).float()
     r = oassign.tal_assign(c.ps[:1].cpu(), pb, c.pts.cpu(), gt0[..., :1], gt0[..., 1:], mask, num_classes=NC, ties="index")
     assert torch.equal(res[1][0].cpu().bool(), r[3][0]) and torch.equal(res[0][0].cpu().long(), r[4][0])
+
+
+def test_det_loss_lrtb_second_call_launch():
+    """ComputeLossNS's second yv6_det_loss launch: the lrtb distances scored against the assignment of the DFL first call
+    (config m: YOLOv6 P5 anchors at 640, the n / s shapes, DFL reg_max 16), weights (0, 2.5, 0), reg_ch = 4, norm_gt_zero = 1."""
+    c, gt, _, _, gi, fg, norm, _ = checked_assignment("m")
+    lrtb = case("n").pd                          # plain (l, t, r, b) distances of the same anchors
+    assert lrtb.shape[:2] == c.pd.shape[:2] and lrtb.shape[2] == 4
+    w = (0.0, W_IOU, 0.0)
+    gs, gd, out = run_det_loss(c, lrtb, gt, gi, fg, norm, "giou", 1, 1.0, weights=w)
+    (_, _), (rb, bb), ro, ob = loss_refs(c, lrtb, gt, gi, fg, norm, "giou", 1, 1.0, weights=w)
+    assert not bool(gs.any()), "lrtb call: the class gradient of a zero class weight"
+    assert out[2].item() == 0.0 and out[3].item() == 0.0, "lrtb call: dfl and class terms"
+    assert (gd[~fg.bool()] == 0).all(), "lrtb call: background rows of grad_distri"
+    assert_within(gd, rb, bb, "lrtb call: grad_distri")
+    assert_within(out[:6], ro, ob, "lrtb call: out[0..5]")
+    assert out[1].item() > 0 and out[5].item() == fg.sum().item()
+
+
+def test_lrtb_second_call_leaves_the_first_calls_outputs():
+    """Whole calls as ComputeLossNS makes them: the DFL call, then the lrtb call with reuse=; the first call's gradients,
+    outputs and assignment are bit for bit what they were, and the second call's class gradient is all zero."""
+    from yolov6_b200.loss_distill import ComputeLossNS
+    cm, cn = case("m"), case("n")
+    cl = ComputeLossNS(num_classes=NC, ori_img_size=cm.W, use_dfl=True, reg_max=16)
+    st = cl.forward_backward(cm.ps, cm.pd, cm.sizes, cm.rows.cuda(), 10, cm.H, cm.W, max_gt=G)
+    torch.cuda.synchronize()
+    a = st["assignment"]
+    before = [t.clone() for t in (st["grad_scores"], st["grad_distri"], st["out"], a.gt_idx, a.fg, a.norm, st["gt"])]
+    st2 = cl.forward_backward(cm.ps, cn.pd, cm.sizes, None, 10, cm.H, cm.W, reuse=st, weights=(0.0, W_IOU, 0.0))
+    torch.cuda.synchronize()
+    after = (st["grad_scores"], st["grad_distri"], st["out"], a.gt_idx, a.fg, a.norm, st["gt"])
+    for x, y in zip(before, after):
+        assert torch.equal(x.view(torch.uint8), y.view(torch.uint8)), "the lrtb call changed an output of the first call"
+    assert st2["grad_scores"].data_ptr() != st["grad_scores"].data_ptr() and not bool(st2["grad_scores"].any())
+    assert st2["out"][2].item() == 0.0 and st2["out"][3].item() == 0.0
