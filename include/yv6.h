@@ -33,7 +33,7 @@ enum {
 
 /* HARDSWISH = x * min(max(x + 3, 0), 6) / 6 (nn.Hardswish), HARDSIGMOID = min(max(x + 3, 0), 6) / 6 (nn.Hardsigmoid) */
 enum { YV6_ACT_NONE = 0, YV6_ACT_RELU = 1, YV6_ACT_SILU = 2, YV6_ACT_SIGMOID = 3, YV6_ACT_HARDSWISH = 4, YV6_ACT_HARDSIGMOID = 5 };
-enum { YV6_DT_BF16 = 0, YV6_DT_F32 = 1, YV6_DT_U8 = 2 };
+enum { YV6_DT_BF16 = 0, YV6_DT_F32 = 1, YV6_DT_U8 = 2, YV6_DT_F16 = 3 };
 #define YV6_PAD_SAME (-1000000)
 
 typedef struct yv6_handle yv6_handle;
@@ -64,6 +64,9 @@ int yv6_abi_version(void);
  * nsplit = 1: bf16 operands, fp32 accumulate.
  * nsplit = 3: "bf16x3" fp32-equivalent mode -- x, w and y are three bf16 planes (hi, mid, lo) whose
  *             sum is the fp32 value; six plane-pair products are accumulated in fp32.
+ * reserved0 = YV6_DT_F16 (operand dtype; 0 = bf16): x, w and res are fp16 and y is fp16 (y_dtype = YV6_DT_F16) or fp32;
+ *             fp16 wgmma with fp32 accumulation, nsplit must be 1.  Outputs beyond fp16's range (65504) become +-inf.
+ *             The tile plan is the one the bf16 operands get.
  * ---------------------------------------------------------------------------------------------- */
 typedef struct yv6_conv_desc {
   /* input */
@@ -109,7 +112,7 @@ typedef struct yv6_conv_desc {
    * mainloop (one 9 x 33 input box per 8 x 16 output tile instead of one box per tap) then skips the all-zero 64-channel
    * blocks, so the view costs no extra MACs when Cin/2 % 64 == 0.  0 = no promise (every block is multiplied). */
   int32_t pair_view;
-  int32_t reserved0;        /* keeps the struct size a multiple of 8; must be 0 */
+  int32_t reserved0;        /* operand dtype: 0 = bf16, YV6_DT_F16 = fp16 (see above); anything else is YV6_ERR_ARG */
 } yv6_conv_desc;
 
 int yv6_conv_fwd(yv6_handle* h, const yv6_conv_desc* d, void* stream);
@@ -146,12 +149,17 @@ typedef struct yv6_stem_desc {
                                (fp32 images with 16-byte aligned rows) */
 } yv6_stem_desc;
 int yv6_stem_fwd(yv6_handle* h, const yv6_stem_desc* d, void* stream);
+/* The same with fp16 output (one plane, tensor cores: fp16 image / weights, fp32 accumulate; nsplit = 1, fp32_math = 0). */
+int yv6_stem_fwd_f16(yv6_handle* h, const yv6_stem_desc* d, void* stream);
 
 /* SPPF / CSPSPPF pooling (reference yolov6/layers/common.py:106-112,150-158): buf is the 4C-wide
  * NHWC concat buffer whose channel slice [0,C) holds x; writes the 5x5 / 9x9 / 13x13 clipped-window
  * maxima (= three chained MaxPool2d(5,1,2)) into slices [C,2C), [2C,3C), [3C,4C). */
 int yv6_sppf_pool(yv6_handle* h, void* buf, int32_t N, int32_t H, int32_t W, int32_t C, int32_t c_total,
                   int32_t nsplit, int64_t plane_stride, void* stream);
+/* The same on an fp16 buffer (nsplit = 1, C % 16 == 0). */
+int yv6_sppf_pool_f16(yv6_handle* h, void* buf, int32_t N, int32_t H, int32_t W, int32_t C, int32_t c_total,
+                      int32_t nsplit, int64_t plane_stride, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * YOLOv6Lite (reference yolov6/models/yolo_lite.py; layers/common.py:740-934): the layers that are not dense convolutions.
@@ -162,10 +170,13 @@ int yv6_sppf_pool(yv6_handle* h, void* buf, int32_t N, int32_t H, int32_t W, int
  * yv6_dwconv_fwd: depthwise conv (groups = C), k in {3, 5}, stride 1 or 2, padding k / 2, output ((H-1)/s+1) x ((W-1)/s+1);
  *   y = act(conv(x, w) + bias), act NONE or HARDSWISH.  w fp32 [k*k][C] (tap-major, channel innermost), bias fp32 [C] or NULL.
  *   Any C and slice offset; channels of y outside the slice are not written.
+ * yv6_dwconv_fwd_f16: the same on fp16 activations (nsplit = 1); the weights stay fp32.
  * yv6_se_fwd: SEBlock in place on x: s = hardsigmoid(W2 relu(W1 mean_hw(x) + b1) + b2), x *= s per (image, channel).
  *   w1 fp32 [Cr][C], b1 [Cr], w2 [C][Cr], b2 [C]; C <= 512, Cr <= 128.  Deterministic: fixed summation order, no atomics.
+ *   reserved0 = operand dtype: 0 = bf16, YV6_DT_F16 = fp16 x (nsplit = 1); anything else is YV6_ERR_ARG.
  * yv6_channel_shuffle: channel_shuffle(cat(a, b), 2) of two C-channel slices: y[.., 2j] = a[.., j], y[.., 2j+1] = b[.., j].
  * yv6_upsample2x: nearest 2x upsample of an [N, H, W, C] slice into a [N, 2H, 2W, .] slice.
+ *   Both copy 16-bit elements bit for bit, so they serve fp16 activations as they are.
  * ---------------------------------------------------------------------------------------------- */
 typedef struct yv6_dw_desc {
   const void* x;
@@ -178,6 +189,7 @@ typedef struct yv6_dw_desc {
   void* y;
 } yv6_dw_desc;
 int yv6_dwconv_fwd(yv6_handle* h, const yv6_dw_desc* d, void* stream);
+int yv6_dwconv_fwd_f16(yv6_handle* h, const yv6_dw_desc* d, void* stream);
 
 typedef struct yv6_se_desc {
   void* x;
@@ -187,7 +199,7 @@ typedef struct yv6_se_desc {
   const float* b1;
   const float* w2;
   const float* b2;
-  int32_t nsplit, reserved0;
+  int32_t nsplit, reserved0;   /* reserved0: operand dtype (0 = bf16, YV6_DT_F16) */
 } yv6_se_desc;
 int yv6_se_fwd(yv6_handle* h, const yv6_se_desc* d, void* stream);
 

@@ -11,7 +11,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libyolov6_b200.so")
 
 ACT_NONE, ACT_RELU, ACT_SILU, ACT_SIGMOID, ACT_HARDSWISH = 0, 1, 2, 3, 4
-DT_BF16, DT_F32, DT_U8 = 0, 1, 2
+DT_BF16, DT_F32, DT_U8, DT_F16 = 0, 1, 2, 3
 PAD_SAME = -1000000
 ACT_CODES = {None: ACT_NONE, "none": ACT_NONE, "relu": ACT_RELU, "silu": ACT_SILU, "sigmoid": ACT_SIGMOID, "hardswish": ACT_HARDSWISH}
 
@@ -34,7 +34,8 @@ class ConvDesc(C.Structure):
         ("force_bw", C.c_int32), ("force_bh", C.c_int32), ("force_bi", C.c_int32), ("force_bn", C.c_int32),
         ("force_stages", C.c_int32), ("force_grid", C.c_int32), ("force_direct", C.c_int32), ("force_halo", C.c_int32),
         ("pad_w", C.c_int32), ("out_h", C.c_int32), ("out_w", C.c_int32), ("force_groups", C.c_int32),
-        ("trace", C.c_void_p), ("stride_w", C.c_int32), ("force_pair", C.c_int32), ("pair_view", C.c_int32), ("reserved0", C.c_int32),
+        ("trace", C.c_void_p), ("stride_w", C.c_int32), ("force_pair", C.c_int32), ("pair_view", C.c_int32),
+        ("reserved0", C.c_int32),     # operand dtype: 0 = bf16, DT_F16 = fp16
     ]
 
 
@@ -147,7 +148,8 @@ class SeDesc(C.Structure):
     _fields_ = [
         ("x", C.c_void_p), ("N", C.c_int32), ("HW", C.c_int32), ("C", C.c_int32), ("Cr", C.c_int32),
         ("c_total", C.c_int64), ("plane_stride", C.c_int64),
-        ("w1", C.c_void_p), ("b1", C.c_void_p), ("w2", C.c_void_p), ("b2", C.c_void_p), ("nsplit", C.c_int32), ("reserved0", C.c_int32),
+        ("w1", C.c_void_p), ("b1", C.c_void_p), ("w2", C.c_void_p), ("b2", C.c_void_p), ("nsplit", C.c_int32),
+        ("reserved0", C.c_int32),     # operand dtype: 0 = bf16, DT_F16 = fp16
     ]
 
 
@@ -190,8 +192,11 @@ _SIGNATURES = {
     "yv6_conv_plan": (C.c_int, [C.c_void_p, C.POINTER(ConvDesc), C.POINTER(C.c_int32)]),
     "yv6_conv_plan_host": (C.c_int, [C.c_int, C.c_int, C.c_int, C.POINTER(ConvDesc), C.POINTER(C.c_int32)]),
     "yv6_stem_fwd": (C.c_int, [C.c_void_p, C.POINTER(StemDesc), C.c_void_p]),
+    "yv6_stem_fwd_f16": (C.c_int, [C.c_void_p, C.POINTER(StemDesc), C.c_void_p]),
     "yv6_sppf_pool": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                 C.c_int32, C.c_int64, C.c_void_p]),
+    "yv6_sppf_pool_f16": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                    C.c_int32, C.c_int64, C.c_void_p]),
     "yv6_head_decode": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
                                   C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_float),
                                   C.c_void_p]),
@@ -262,6 +267,7 @@ _SIGNATURES = {
     "yv6_coco_accumulate": (C.c_int, [C.c_void_p, C.POINTER(CocoState), C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
                                       C.c_void_p]),
     "yv6_dwconv_fwd": (C.c_int, [C.c_void_p, C.POINTER(DwDesc), C.c_void_p]),
+    "yv6_dwconv_fwd_f16": (C.c_int, [C.c_void_p, C.POINTER(DwDesc), C.c_void_p]),
     "yv6_se_fwd": (C.c_int, [C.c_void_p, C.POINTER(SeDesc), C.c_void_p]),
     "yv6_qa_fwd": (C.c_int, [C.c_void_p, C.POINTER(QaDesc), C.c_void_p]),
     "yv6_qa_bwd": (C.c_int, [C.c_void_p, C.POINTER(QaDesc), C.c_void_p]),

@@ -1,7 +1,9 @@
 // yv6_aux.cu -- the HBM-bound helpers around the conv kernel (sm_90a, CUDA cores):
-//   * yv6_stem_fwd   : first 3x3 s2 conv on the 3-channel NCHW image (fp32 or uint8/255) -> NHWC bf16
+//   * yv6_stem_fwd   : first 3x3 s2 conv on the 3-channel NCHW image (fp32 or uint8/255) -> NHWC bf16 (yv6_stem_fwd_f16: fp16)
 //   * yv6_sppf_pool  : the three chained 5x5 max-pools of (CSP)SPPF written straight into concat slices
 //   * yv6_head_decode: DFL expectation + ltrb -> xywh + x stride + [xywh, 1, cls] assembly
+#include <type_traits>
+
 #include "yv6_common.cuh"
 #include "yv6_handle.h"
 
@@ -97,19 +99,44 @@ __global__ void __launch_bounds__(256) stem_kernel(const StemParams p) {
   }
 }
 
+// The 16-bit activation dtype T of the tensor-core stems (__nv_bfloat16, or __half in the fp16 mode): a pair of values rounded to
+// it, and one m16n8k16 mma.sync on T operands with fp32 accumulation.
+template <typename T>
+__device__ __forceinline__ uint32_t stem_pack2(float a, float b) {
+  if constexpr (std::is_same_v<T, __half>) {
+    __half2 v = __floats2half2_rn(a, b);
+    return *reinterpret_cast<uint32_t*>(&v);
+  } else {
+    __nv_bfloat162 v = __floats2bfloat162_rn(a, b);
+    return *reinterpret_cast<uint32_t*>(&v);
+  }
+}
+template <typename T>
+__device__ __forceinline__ void stem_mma16816(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+  if constexpr (std::is_same_v<T, __half>)
+    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+  else
+    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+
 // Tensor-core stem for bf16 activations: the 3x3 stride-2 conv over 3 input channels is a GEMM with K = 27
 // (padded to 32).  Persistent CTAs walk tiles of 8 output rows x 32 output columns; the 17 x 65 x 3 input
 // patch is staged in shared memory as bf16 with 16-byte global loads, each warp owns one output row (two
 // 16-pixel m-tiles) and gathers its mma.sync A fragments straight from the patch; the weights live in
 // registers as B fragments for the whole kernel.  The work is bound by HBM (read the image once, write
-// N*Ho*Wo*Cout bf16 once), so legacy mma.sync is ample; what matters is the instruction count per pixel.
-template <int COUT>
-__global__ void __launch_bounds__(256, 2) stem_mma_kernel(const StemParams p) {
+// N*Ho*Wo*Cout bf16 once), so legacy mma.sync is ample; what matters is the instruction count per pixel.  T: the activation
+// dtype (the body of stem_mma_kernel and stem_mma_f16_kernel below).
+template <int COUT, typename T>
+__device__ __forceinline__ void stem_mma_body(const StemParams& p) {
   constexpr int TH = 8, TW = 32, PH = 2 * TH + 1, PW = 2 * TW + 1, NT = COUT / 8;
   constexpr int PWP = 68;                                  // patch row pitch; element j of a row = input column wi0 + j - 1
   static_assert(PW + 1 <= PWP, "patch pitch");
   constexpr int PITCH = COUT * 2 + 16;                     // staged output row pitch (bytes): conflict-free
-  __shared__ __align__(16) __nv_bfloat16 patch[3 * PH * PWP];
+  __shared__ __align__(16) T patch[3 * PH * PWP];
   __shared__ __align__(16) uint8_t stage[8 * 32 * PITCH];
   const int tiles_w = (p.Wo + TW - 1) / TW, tiles_h = (p.Ho + TH - 1) / TH;
   const int num_tiles = tiles_w * tiles_h * p.N;
@@ -126,8 +153,7 @@ __global__ void __launch_bounds__(256, 2) stem_mma_kernel(const StemParams p) {
         const int k = ks * 16 + h2 * 8 + 2 * t, nn = nt * 8 + g;
         const float w0 = (k < 27) ? __ldg(p.w + k * COUT + nn) : 0.f;
         const float w1 = (k + 1 < 27) ? __ldg(p.w + (k + 1) * COUT + nn) : 0.f;
-        __nv_bfloat162 v = __floats2bfloat162_rn(w0, w1);
-        bfrag[nt][ks][h2] = *reinterpret_cast<uint32_t*>(&v);
+        bfrag[nt][ks][h2] = stem_pack2<T>(w0, w1);
       }
   float bias[NT][2];
 #pragma unroll
@@ -208,13 +234,13 @@ __global__ void __launch_bounds__(256, 2) stem_mma_kernel(const StemParams p) {
       const int item = threadIdx.x + it * 256;
       if (item < 3 * PH * 17) {
         const int rc = item / 17, q = item - rc * 17;
-        __nv_bfloat16* dst = patch + rc * PWP;
+        T* dst = patch + rc * PWP;
         if (q == 0) {
-          dst[1] = __float2bfloat16_rn(pre[it].x);
+          dst[1] = T(pre[it].x);
         } else {
-          __nv_bfloat162* d2 = reinterpret_cast<__nv_bfloat162*>(dst + 2 + 4 * (q - 1));
-          d2[0] = __floats2bfloat162_rn(pre[it].x, pre[it].y);
-          d2[1] = __floats2bfloat162_rn(pre[it].z, pre[it].w);
+          uint32_t* d2 = reinterpret_cast<uint32_t*>(dst + 2 + 4 * (q - 1));
+          d2[0] = stem_pack2<T>(pre[it].x, pre[it].y);
+          d2[1] = stem_pack2<T>(pre[it].z, pre[it].w);
         }
       }
     }
@@ -242,12 +268,7 @@ __global__ void __launch_bounds__(256, 2) stem_mma_kernel(const StemParams p) {
           a[2 * h2 + 1] = lo1 | (hi1v << 16);
         }
 #pragma unroll
-        for (int nt = 0; nt < NT; ++nt) {
-          asm volatile(
-              "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-              : "+f"(acc[mt][nt][0]), "+f"(acc[mt][nt][1]), "+f"(acc[mt][nt][2]), "+f"(acc[mt][nt][3])
-              : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(bfrag[nt][ks][0]), "r"(bfrag[nt][ks][1]));
-        }
+        for (int nt = 0; nt < NT; ++nt) stem_mma16816<T>(acc[mt][nt], a, bfrag[nt][ks][0], bfrag[nt][ks][1]);
       }
     }
     // ---- bias + activation -> staged row of this warp -> coalesced 16-byte stores ----
@@ -257,8 +278,8 @@ __global__ void __launch_bounds__(256, 2) stem_mma_kernel(const StemParams p) {
       for (int nt = 0; nt < NT; ++nt) {
         const float v0 = act_apply(acc[mt][nt][0] + bias[nt][0], p.act), v1 = act_apply(acc[mt][nt][1] + bias[nt][1], p.act);
         const float v2 = act_apply(acc[mt][nt][2] + bias[nt][0], p.act), v3 = act_apply(acc[mt][nt][3] + bias[nt][1], p.act);
-        *reinterpret_cast<__nv_bfloat162*>(wstage + (mt * 16 + g) * PITCH + (nt * 8 + 2 * t) * 2) = __floats2bfloat162_rn(v0, v1);
-        *reinterpret_cast<__nv_bfloat162*>(wstage + (mt * 16 + g + 8) * PITCH + (nt * 8 + 2 * t) * 2) = __floats2bfloat162_rn(v2, v3);
+        *reinterpret_cast<uint32_t*>(wstage + (mt * 16 + g) * PITCH + (nt * 8 + 2 * t) * 2) = stem_pack2<T>(v0, v1);
+        *reinterpret_cast<uint32_t*>(wstage + (mt * 16 + g + 8) * PITCH + (nt * 8 + 2 * t) * 2) = stem_pack2<T>(v2, v3);
       }
     __syncwarp();
     const int py = py0 + warp;
@@ -273,6 +294,16 @@ __global__ void __launch_bounds__(256, 2) stem_mma_kernel(const StemParams p) {
     }
     __syncwarp();
   }
+}
+
+template <int COUT>
+__global__ void __launch_bounds__(256, 2) stem_mma_kernel(const StemParams p) {
+  stem_mma_body<COUT, __nv_bfloat16>(p);
+}
+// fp16 activations (yv6_stem_fwd_f16)
+template <int COUT>
+__global__ void __launch_bounds__(256, 2) stem_mma_f16_kernel(const StemParams p) {
+  stem_mma_body<COUT, __half>(p);
 }
 
 // fp32 images, asynchronous variant: the register prefetch above keeps 13 KB per CTA (26 KB per SM) of loads in flight, ~60 % of
@@ -291,9 +322,10 @@ template <int N>
 __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
 
 // ACT = the layer's activation (YV6_ACT_*) at compile time: a runtime act_apply in the epilogue costs an indirect branch per
-// element, and its SiLU / sigmoid divisions bring a CALL that pins the register allocation of every instance.
-template <int COUT, int ACT>
-__global__ void __launch_bounds__(256, 2) stem_mma_async_kernel(const StemParams p) {
+// element, and its SiLU / sigmoid divisions bring a CALL that pins the register allocation of every instance.  T: the activation
+// dtype (the body of stem_mma_async_kernel and stem_mma_async_f16_kernel below).
+template <int COUT, int ACT, typename T>
+__device__ __forceinline__ void stem_mma_async_body(const StemParams& p) {
   constexpr int TH = 8, TW = 32, PH = 2 * TH + 1, NT = COUT / 8;
   constexpr int PWP = 72;                                  // fp32 patch row pitch; element j = input column 64 * tw + j - 4
   constexpr int PATCH = 3 * PH * PWP;                      // floats per stage
@@ -316,8 +348,7 @@ __global__ void __launch_bounds__(256, 2) stem_mma_async_kernel(const StemParams
         const int k = ks * 16 + h2 * 8 + 2 * t, nn = nt * 8 + g;
         const float w0 = (k < 27) ? __ldg(p.w + k * COUT + nn) : 0.f;
         const float w1 = (k + 1 < 27) ? __ldg(p.w + (k + 1) * COUT + nn) : 0.f;
-        __nv_bfloat162 v = __floats2bfloat162_rn(w0, w1);
-        bfrag[nt][ks][h2] = *reinterpret_cast<uint32_t*>(&v);
+        bfrag[nt][ks][h2] = stem_pack2<T>(w0, w1);
       }
   float bias[NT][2];
 #pragma unroll
@@ -392,17 +423,11 @@ __global__ void __launch_bounds__(256, 2) stem_mma_async_kernel(const StemParams
           const int o0 = koff[ks][h2][0], o1 = koff[ks][h2][1];
           const float l0 = o0 >= 0 ? P[base0 + o0] : 0.f, h0 = o1 >= 0 ? P[base0 + o1] : 0.f;
           const float l1 = o0 >= 0 ? P[base1 + o0] : 0.f, h1 = o1 >= 0 ? P[base1 + o1] : 0.f;
-          __nv_bfloat162 q0 = __floats2bfloat162_rn(l0, h0), q1 = __floats2bfloat162_rn(l1, h1);
-          a[2 * h2 + 0] = *reinterpret_cast<uint32_t*>(&q0);
-          a[2 * h2 + 1] = *reinterpret_cast<uint32_t*>(&q1);
+          a[2 * h2 + 0] = stem_pack2<T>(l0, h0);
+          a[2 * h2 + 1] = stem_pack2<T>(l1, h1);
         }
 #pragma unroll
-        for (int nt = 0; nt < NT; ++nt) {
-          asm volatile(
-              "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-              : "+f"(acc[mt][nt][0]), "+f"(acc[mt][nt][1]), "+f"(acc[mt][nt][2]), "+f"(acc[mt][nt][3])
-              : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(bfrag[nt][ks][0]), "r"(bfrag[nt][ks][1]));
-        }
+        for (int nt = 0; nt < NT; ++nt) stem_mma16816<T>(acc[mt][nt], a, bfrag[nt][ks][0], bfrag[nt][ks][1]);
       }
     }
 #pragma unroll
@@ -411,8 +436,8 @@ __global__ void __launch_bounds__(256, 2) stem_mma_async_kernel(const StemParams
       for (int nt = 0; nt < NT; ++nt) {
         const float v0 = act_apply(acc[mt][nt][0] + bias[nt][0], ACT), v1 = act_apply(acc[mt][nt][1] + bias[nt][1], ACT);
         const float v2 = act_apply(acc[mt][nt][2] + bias[nt][0], ACT), v3 = act_apply(acc[mt][nt][3] + bias[nt][1], ACT);
-        *reinterpret_cast<__nv_bfloat162*>(wstage + (mt * 16 + g) * PITCH + (nt * 8 + 2 * t) * 2) = __floats2bfloat162_rn(v0, v1);
-        *reinterpret_cast<__nv_bfloat162*>(wstage + (mt * 16 + g + 8) * PITCH + (nt * 8 + 2 * t) * 2) = __floats2bfloat162_rn(v2, v3);
+        *reinterpret_cast<uint32_t*>(wstage + (mt * 16 + g) * PITCH + (nt * 8 + 2 * t) * 2) = stem_pack2<T>(v0, v1);
+        *reinterpret_cast<uint32_t*>(wstage + (mt * 16 + g + 8) * PITCH + (nt * 8 + 2 * t) * 2) = stem_pack2<T>(v2, v3);
       }
     __syncwarp();
     const int py = py0 + warp;
@@ -431,6 +456,15 @@ __global__ void __launch_bounds__(256, 2) stem_mma_async_kernel(const StemParams
   cp_async_wait<0>();
 }
 
+template <int COUT, int ACT>
+__global__ void __launch_bounds__(256, 2) stem_mma_async_kernel(const StemParams p) {
+  stem_mma_async_body<COUT, ACT, __nv_bfloat16>(p);
+}
+template <int COUT, int ACT>
+__global__ void __launch_bounds__(256, 2) stem_mma_async_f16_kernel(const StemParams p) {
+  stem_mma_async_body<COUT, ACT, __half>(p);
+}
+
 // ------------------------------------------------------------------------------------------------
 // SPPF pooling: reference SPPFModule / CSPSPPFModule (common.py:106-112, 150-158):
 //   y1 = pool5(x), y2 = pool5(y1), y3 = pool5(y2), cat([x, y1, y2, y3]).
@@ -439,7 +473,7 @@ __global__ void __launch_bounds__(256, 2) stem_mma_async_kernel(const StemParams
 // window sizes are formed separably, then column maxima; results go to slices 1..3 of the concat buffer.
 // ------------------------------------------------------------------------------------------------
 struct PoolParams {
-  __nv_bfloat16* buf;  // [planes][N,H,W,c_total]
+  __nv_bfloat16* buf;  // [planes][N,H,W,c_total] (fp16 for sppf_pool_f16_kernel, which only moves and compares its 16-bit values)
   int64_t plane_stride;
   int32_t N, H, W, C, c_total, planes;
 };
@@ -539,16 +573,19 @@ __global__ void __launch_bounds__(256) sppf_pool_kernel(const PoolParams p) {
 // bf16x2 values with no rounding anywhere -- bit-identical to the fp32 kernel above.  One CTA per (image, 16 channels):
 // a pixel's 32 bytes are one full DRAM sector (the fp32 kernel's 8-channel slices fetched half-used sectors at a 2 KB
 // stride: 0.6 TB/s), the staged plane and its three row-maximum planes take 4 x H*W*32 bytes of shared memory.
+// The same holds for fp16 (half2 maxima): T2 = __nv_bfloat162 or __half2.
+template <typename T2>
 __device__ __forceinline__ uint4 hmax8(uint4 a, uint4 b) {
   uint4 r;
-  *reinterpret_cast<__nv_bfloat162*>(&r.x) = __hmax2(*reinterpret_cast<__nv_bfloat162*>(&a.x), *reinterpret_cast<__nv_bfloat162*>(&b.x));
-  *reinterpret_cast<__nv_bfloat162*>(&r.y) = __hmax2(*reinterpret_cast<__nv_bfloat162*>(&a.y), *reinterpret_cast<__nv_bfloat162*>(&b.y));
-  *reinterpret_cast<__nv_bfloat162*>(&r.z) = __hmax2(*reinterpret_cast<__nv_bfloat162*>(&a.z), *reinterpret_cast<__nv_bfloat162*>(&b.z));
-  *reinterpret_cast<__nv_bfloat162*>(&r.w) = __hmax2(*reinterpret_cast<__nv_bfloat162*>(&a.w), *reinterpret_cast<__nv_bfloat162*>(&b.w));
+  *reinterpret_cast<T2*>(&r.x) = __hmax2(*reinterpret_cast<T2*>(&a.x), *reinterpret_cast<T2*>(&b.x));
+  *reinterpret_cast<T2*>(&r.y) = __hmax2(*reinterpret_cast<T2*>(&a.y), *reinterpret_cast<T2*>(&b.y));
+  *reinterpret_cast<T2*>(&r.z) = __hmax2(*reinterpret_cast<T2*>(&a.z), *reinterpret_cast<T2*>(&b.z));
+  *reinterpret_cast<T2*>(&r.w) = __hmax2(*reinterpret_cast<T2*>(&a.w), *reinterpret_cast<T2*>(&b.w));
   return r;
 }
 
-__global__ void __launch_bounds__(256) sppf_pool_bf16_kernel(const PoolParams p) {
+template <typename T2>
+__device__ __forceinline__ void sppf_pool_packed_body(const PoolParams& p) {
   extern __shared__ uint4 sq[];                 // [4][H*W][2] units of 8 channels: x, rowmax5, rowmax9, rowmax13
   const int cgs = p.C / 16;
   const int n = blockIdx.x / cgs, cg = blockIdx.x % cgs;
@@ -567,20 +604,20 @@ __global__ void __launch_bounds__(256) sppf_pool_bf16_kernel(const PoolParams p)
     uint4 m5 = sx[u], m9, m13;
 #pragma unroll
     for (int dx = 1; dx <= 2; ++dx) {
-      if (w - dx >= 0) m5 = hmax8(m5, sx[u - 2 * dx]);
-      if (w + dx < p.W) m5 = hmax8(m5, sx[u + 2 * dx]);
+      if (w - dx >= 0) m5 = hmax8<T2>(m5, sx[u - 2 * dx]);
+      if (w + dx < p.W) m5 = hmax8<T2>(m5, sx[u + 2 * dx]);
     }
     m9 = m5;
 #pragma unroll
     for (int dx = 3; dx <= 4; ++dx) {
-      if (w - dx >= 0) m9 = hmax8(m9, sx[u - 2 * dx]);
-      if (w + dx < p.W) m9 = hmax8(m9, sx[u + 2 * dx]);
+      if (w - dx >= 0) m9 = hmax8<T2>(m9, sx[u - 2 * dx]);
+      if (w + dx < p.W) m9 = hmax8<T2>(m9, sx[u + 2 * dx]);
     }
     m13 = m9;
 #pragma unroll
     for (int dx = 5; dx <= 6; ++dx) {
-      if (w - dx >= 0) m13 = hmax8(m13, sx[u - 2 * dx]);
-      if (w + dx < p.W) m13 = hmax8(m13, sx[u + 2 * dx]);
+      if (w - dx >= 0) m13 = hmax8<T2>(m13, sx[u - 2 * dx]);
+      if (w + dx < p.W) m13 = hmax8<T2>(m13, sx[u + 2 * dx]);
     }
     (void)half;
     r5[u] = m5;
@@ -597,14 +634,14 @@ __global__ void __launch_bounds__(256) sppf_pool_bf16_kernel(const PoolParams p)
 #pragma unroll
     for (int dy = 1; dy <= 6; ++dy) {
       if (h - dy >= 0) {
-        if (dy <= 2) m5 = hmax8(m5, r5[u - dy * rs]);
-        if (dy <= 4) m9 = hmax8(m9, r9[u - dy * rs]);
-        m13 = hmax8(m13, r13[u - dy * rs]);
+        if (dy <= 2) m5 = hmax8<T2>(m5, r5[u - dy * rs]);
+        if (dy <= 4) m9 = hmax8<T2>(m9, r9[u - dy * rs]);
+        m13 = hmax8<T2>(m13, r13[u - dy * rs]);
       }
       if (h + dy < p.H) {
-        if (dy <= 2) m5 = hmax8(m5, r5[u + dy * rs]);
-        if (dy <= 4) m9 = hmax8(m9, r9[u + dy * rs]);
-        m13 = hmax8(m13, r13[u + dy * rs]);
+        if (dy <= 2) m5 = hmax8<T2>(m5, r5[u + dy * rs]);
+        if (dy <= 4) m9 = hmax8<T2>(m9, r9[u + dy * rs]);
+        m13 = hmax8<T2>(m13, r13[u + dy * rs]);
       }
     }
     __nv_bfloat16* o = dst + (int64_t)i * p.c_total + (u & 1) * 8;
@@ -613,6 +650,9 @@ __global__ void __launch_bounds__(256) sppf_pool_bf16_kernel(const PoolParams p)
     *reinterpret_cast<uint4*>(o + (int64_t)3 * p.C) = m13;
   }
 }
+
+__global__ void __launch_bounds__(256) sppf_pool_bf16_kernel(const PoolParams p) { sppf_pool_packed_body<__nv_bfloat162>(p); }
+__global__ void __launch_bounds__(256) sppf_pool_f16_kernel(const PoolParams p) { sppf_pool_packed_body<__half2>(p); }
 
 // ------------------------------------------------------------------------------------------------
 // head decode: eval tail of Detect.forward (effidehead.py:106-139), generate_anchors(is_eval)
@@ -682,17 +722,23 @@ __global__ void __launch_bounds__(256) head_decode_kernel(const __grid_constant_
 using namespace yv6;
 
 using StemKernelFn = void (*)(const StemParams);
-#define YV6_STEM_ACTS(C)                                                                                               \
-  {stem_mma_async_kernel<C, YV6_ACT_NONE>, stem_mma_async_kernel<C, YV6_ACT_RELU>, stem_mma_async_kernel<C, YV6_ACT_SILU>, \
-   stem_mma_async_kernel<C, YV6_ACT_SIGMOID>, stem_mma_async_kernel<C, YV6_ACT_HARDSWISH>,                                 \
-   stem_mma_async_kernel<C, YV6_ACT_HARDSIGMOID>}
-// [Cout / 16 - 1][act]
-static const StemKernelFn kStemAsync[4][6] = {YV6_STEM_ACTS(16), YV6_STEM_ACTS(32), YV6_STEM_ACTS(48), YV6_STEM_ACTS(64)};
+#define YV6_STEM_ACTS(K, C)                                                                                          \
+  {K<C, YV6_ACT_NONE>, K<C, YV6_ACT_RELU>, K<C, YV6_ACT_SILU>, K<C, YV6_ACT_SIGMOID>, K<C, YV6_ACT_HARDSWISH>, \
+   K<C, YV6_ACT_HARDSIGMOID>}
+#define YV6_STEM_TABLE(K) {YV6_STEM_ACTS(K, 16), YV6_STEM_ACTS(K, 32), YV6_STEM_ACTS(K, 48), YV6_STEM_ACTS(K, 64)}
+// [fp16 output][Cout / 16 - 1][act]
+static const StemKernelFn kStemAsync[2][4][6] = {YV6_STEM_TABLE(stem_mma_async_kernel), YV6_STEM_TABLE(stem_mma_async_f16_kernel)};
+#undef YV6_STEM_TABLE
 #undef YV6_STEM_ACTS
+// [fp16 output][Cout / 16 - 1]
+static const StemKernelFn kStemSync[2][4] = {{stem_mma_kernel<16>, stem_mma_kernel<32>, stem_mma_kernel<48>, stem_mma_kernel<64>},
+                                             {stem_mma_f16_kernel<16>, stem_mma_f16_kernel<32>, stem_mma_f16_kernel<48>,
+                                              stem_mma_f16_kernel<64>}};
 
-extern "C" int yv6_stem_fwd(yv6_handle* h, const yv6_stem_desc* d, void* stream) {
+static int stem_fwd(yv6_handle* h, const yv6_stem_desc* d, void* stream, bool f16) {
   yv6_device_guard _dev(h);
   YV6_REQUIRE(h && d && d->x && d->w && d->y, "stem: null argument");
+  YV6_REQUIRE(!f16 || (d->nsplit == 1 && !d->fp32_math), "stem_f16: nsplit must be 1 and fp32_math 0");
   YV6_REQUIRE(d->Cout > 0 && d->Cout <= kStemMaxCout && d->Cout % 16 == 0, "stem: Cout=%d must be 16/32/48/64", d->Cout);
   YV6_REQUIRE(d->nsplit == 1 || d->nsplit == 3, "stem: nsplit must be 1 or 3");
   YV6_REQUIRE(d->x_dtype == YV6_DT_F32 || d->x_dtype == YV6_DT_U8, "stem: image must be fp32 or uint8");
@@ -723,22 +769,18 @@ extern "C" int yv6_stem_fwd(yv6_handle* h, const yv6_stem_desc* d, void* stream)
         d->force_sync_loads == 0) {
       const size_t smem = (size_t)3 * 3 * 17 * 72 * 4 + (size_t)8 * 32 * (d->Cout * 2 + 16);
       if (!(h->configured & YV6_CFG_STEM)) {
-        for (const auto& by_act : kStemAsync)
-          for (StemKernelFn fn : by_act) YV6_CHECK_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
+        for (const auto& by_dtype : kStemAsync)
+          for (const auto& by_act : by_dtype)
+            for (StemKernelFn fn : by_act) YV6_CHECK_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
         h->configured |= YV6_CFG_STEM;
       }
       // act_apply treats codes outside the enum as no activation
       const int act = (d->act >= YV6_ACT_NONE && d->act <= YV6_ACT_HARDSIGMOID) ? d->act : YV6_ACT_NONE;
-      kStemAsync[d->Cout / 16 - 1][act]<<<tiles, 256, smem, s>>>(p);
+      kStemAsync[f16][d->Cout / 16 - 1][act]<<<tiles, 256, smem, s>>>(p);
       YV6_CHECK_CUDA(cudaGetLastError());
       return YV6_OK;
     }
-    switch (d->Cout) {
-      case 16: stem_mma_kernel<16><<<tiles, 256, 0, s>>>(p); break;
-      case 32: stem_mma_kernel<32><<<tiles, 256, 0, s>>>(p); break;
-      case 48: stem_mma_kernel<48><<<tiles, 256, 0, s>>>(p); break;
-      default: stem_mma_kernel<64><<<tiles, 256, 0, s>>>(p); break;
-    }
+    kStemSync[f16][d->Cout / 16 - 1]<<<tiles, 256, 0, s>>>(p);
     YV6_CHECK_CUDA(cudaGetLastError());
     return YV6_OK;
   }
@@ -748,6 +790,28 @@ extern "C" int yv6_stem_fwd(yv6_handle* h, const yv6_stem_desc* d, void* stream)
     case 48: stem_kernel<48><<<grid, 256, 0, s>>>(p); break;
     default: stem_kernel<64><<<grid, 256, 0, s>>>(p); break;
   }
+  YV6_CHECK_CUDA(cudaGetLastError());
+  return YV6_OK;
+}
+
+extern "C" int yv6_stem_fwd(yv6_handle* h, const yv6_stem_desc* d, void* stream) { return stem_fwd(h, d, stream, false); }
+extern "C" int yv6_stem_fwd_f16(yv6_handle* h, const yv6_stem_desc* d, void* stream) { return stem_fwd(h, d, stream, true); }
+
+extern "C" int yv6_sppf_pool_f16(yv6_handle* h, void* buf, int32_t N, int32_t H, int32_t W, int32_t C, int32_t c_total,
+                                 int32_t nsplit, int64_t plane_stride, void* stream) {
+  yv6_device_guard _dev(h);
+  YV6_REQUIRE(h && buf, "sppf_pool_f16: null argument");
+  YV6_REQUIRE(nsplit == 1, "sppf_pool_f16: nsplit must be 1");
+  YV6_REQUIRE(C % 16 == 0 && c_total >= 4 * C && c_total % 8 == 0, "sppf_pool_f16: bad channels C=%d c_total=%d", C, c_total);
+  const size_t smem16 = (size_t)4 * H * W * 32;
+  YV6_REQUIRE(smem16 <= (size_t)h->max_smem_optin, "sppf_pool_f16: %dx%d plane does not fit in shared memory", H, W);
+  (void)plane_stride;                                    // one plane
+  PoolParams p{reinterpret_cast<__nv_bfloat16*>(buf), 0, N, H, W, C, c_total, 1};
+  if (!(h->configured & YV6_CFG_POOLF16)) {
+    YV6_CHECK_CUDA(cudaFuncSetAttribute(sppf_pool_f16_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->max_smem_optin));
+    h->configured |= YV6_CFG_POOLF16;
+  }
+  sppf_pool_f16_kernel<<<(unsigned)(N * (C / 16)), 256, smem16, (cudaStream_t)stream>>>(p);
   YV6_CHECK_CUDA(cudaGetLastError());
   return YV6_OK;
 }

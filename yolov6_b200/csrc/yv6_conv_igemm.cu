@@ -58,7 +58,7 @@ struct ConvKParams {
   int32_t act, y_dtype, out_planes, res_planes;
   void* y;
   int64_t y_img_stride, y_h_stride, y_w_stride, y_plane_stride;
-  const __nv_bfloat16* res;
+  const void* res;          // the operand dtype (bf16 or fp16)
   float alpha;
   int64_t res_img_stride, res_h_stride, res_w_stride, res_plane_stride;
   const float* bias;
@@ -185,7 +185,30 @@ __device__ __forceinline__ uint32_t pack_bf16x2(float a, float b) {
   return *reinterpret_cast<uint32_t*>(&v);
 }
 
+// The operand dtype T (__nv_bfloat16, or __half for the fp16 mode) of activations, weights and residuals: rounding to it,
+// and its packed pair.  fp16 rounds values beyond 65504 to +-inf.
+template <typename T> struct Pair2;
+template <> struct Pair2<__nv_bfloat16> { using type = __nv_bfloat162; };
+template <> struct Pair2<__half> { using type = __half2; };
+template <typename T>
+__device__ __forceinline__ uint32_t pack2(float a, float b) {
+  if constexpr (std::is_same_v<T, __half>) {
+    __half2 v = __floats2half2_rn(a, b);
+    return *reinterpret_cast<uint32_t*>(&v);
+  } else {
+    return pack_bf16x2(a, b);
+  }
+}
+template <typename T>
+__device__ __forceinline__ T round_to(float v) {
+  if constexpr (std::is_same_v<T, __half>) return __float2half_rn(v);
+  else return __float2bfloat16_rn(v);
+}
+__device__ __forceinline__ float to_float(__nv_bfloat16 v) { return __bfloat162float(v); }
+__device__ __forceinline__ float to_float(__half v) { return __half2float(v); }
+
 // Store 16 consecutive output channels of one pixel.
+template <typename T>
 __device__ __forceinline__ void store_chunk(const ConvKParams& p, int64_t off, int n, int ncol,
                                             const float (&v)[16]) {
   if (p.y_dtype == YV6_DT_F32) {
@@ -203,25 +226,25 @@ __device__ __forceinline__ void store_chunk(const ConvKParams& p, int64_t off, i
 #pragma unroll
   for (int j = 0; j < 16; ++j) rem[j] = v[j];
   for (int pl = 0; pl < p.out_planes; ++pl) {
-    __nv_bfloat16* y = reinterpret_cast<__nv_bfloat16*>(p.y) + pl * p.y_plane_stride + off + n;
+    T* y = reinterpret_cast<T*>(p.y) + pl * p.y_plane_stride + off + n;
     if (ncol == 16 && ((reinterpret_cast<uintptr_t>(y) & 15) == 0)) {
       uint4 q0, q1;
-      q0.x = pack_bf16x2(rem[0], rem[1]);
-      q0.y = pack_bf16x2(rem[2], rem[3]);
-      q0.z = pack_bf16x2(rem[4], rem[5]);
-      q0.w = pack_bf16x2(rem[6], rem[7]);
-      q1.x = pack_bf16x2(rem[8], rem[9]);
-      q1.y = pack_bf16x2(rem[10], rem[11]);
-      q1.z = pack_bf16x2(rem[12], rem[13]);
-      q1.w = pack_bf16x2(rem[14], rem[15]);
+      q0.x = pack2<T>(rem[0], rem[1]);
+      q0.y = pack2<T>(rem[2], rem[3]);
+      q0.z = pack2<T>(rem[4], rem[5]);
+      q0.w = pack2<T>(rem[6], rem[7]);
+      q1.x = pack2<T>(rem[8], rem[9]);
+      q1.y = pack2<T>(rem[10], rem[11]);
+      q1.z = pack2<T>(rem[12], rem[13]);
+      q1.w = pack2<T>(rem[14], rem[15]);
       reinterpret_cast<uint4*>(y)[0] = q0;
       reinterpret_cast<uint4*>(y)[1] = q1;
     } else {
-      for (int j = 0; j < ncol; ++j) y[j] = __float2bfloat16_rn(rem[j]);
+      for (int j = 0; j < ncol; ++j) y[j] = round_to<T>(rem[j]);
     }
     if (pl + 1 < p.out_planes) {
 #pragma unroll
-      for (int j = 0; j < 16; ++j) rem[j] -= __bfloat162float(__float2bfloat16_rn(rem[j]));
+      for (int j = 0; j < 16; ++j) rem[j] -= to_float(round_to<T>(rem[j]));
     }
   }
 }
@@ -271,6 +294,7 @@ __device__ __forceinline__ void activate(const ConvKParams& p, float (&v)[N]) {
 }
 
 // bias + activation (+ residual) for 16 consecutive output channels of one pixel
+template <typename T>
 __device__ __forceinline__ void epilogue_math(const ConvKParams& p, const uint32_t (&r)[16], int n, int ncol, int64_t roff,
                                               float (&v)[16]) {
   if (p.bias != nullptr) {
@@ -289,21 +313,21 @@ __device__ __forceinline__ void epilogue_math(const ConvKParams& p, const uint32
   activate(p, v);
   if (p.res != nullptr) {
     for (int pl = 0; pl < p.res_planes; ++pl) {
-      const __nv_bfloat16* rp = p.res + pl * p.res_plane_stride + roff + n;
+      const T* rp = reinterpret_cast<const T*>(p.res) + pl * p.res_plane_stride + roff + n;
       if (ncol == 16 && ((reinterpret_cast<uintptr_t>(rp) & 15) == 0)) {
         const uint4 q0 = __ldg(reinterpret_cast<const uint4*>(rp));
         const uint4 q1 = __ldg(reinterpret_cast<const uint4*>(rp) + 1);
         const uint32_t w[8] = {q0.x, q0.y, q0.z, q0.w, q1.x, q1.y, q1.z, q1.w};
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
-          const __nv_bfloat162 b2 = *reinterpret_cast<const __nv_bfloat162*>(&w[j]);
+          const typename Pair2<T>::type b2 = *reinterpret_cast<const typename Pair2<T>::type*>(&w[j]);
           v[2 * j] += p.alpha * __low2float(b2);
           v[2 * j + 1] += p.alpha * __high2float(b2);
         }
       } else {
 #pragma unroll
         for (int j = 0; j < 16; ++j)
-          if (j < ncol) v[j] += p.alpha * __bfloat162float(rp[j]);
+          if (j < ncol) v[j] += p.alpha * to_float(rp[j]);
       }
     }
   }
@@ -316,7 +340,7 @@ __host__ __device__ constexpr int y_box_bytes(int bn, int esz) { return (bn * es
 // TMA-store epilogue: bias + activation on one accumulator half (rows row0 + 8 i, columns 8 j + c0, + 1 of this thread), rounded
 // to the output dtype and written to the staging half as the boxes of the output map: column group g (kCols channels) is a
 // [rows][kBox bytes] block at g * kGroupBytes in the map's swizzle, which XORs the 16-byte unit of a row with address bits 7+.
-template <int BN, bool F32>
+template <typename T, int BN, bool F32>
 __device__ __forceinline__ void stage_out_tile(const ConvKParams& p, float (&acc)[BN / 2], const float* sbias, uint8_t* stage,
                                                int row0, int c0) {
   constexpr int kEsz = F32 ? 4 : 2, kBox = y_box_bytes(BN, kEsz), kCols = kBox / kEsz;
@@ -341,7 +365,7 @@ __device__ __forceinline__ void stage_out_tile(const ConvKParams& p, float (&acc
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
       if (F32) *reinterpret_cast<float2*>(dst + 8 * i * kBox) = make_float2(v[2 * i], v[2 * i + 1]);
-      else *reinterpret_cast<uint32_t*>(dst + 8 * i * kBox) = pack_bf16x2(v[2 * i], v[2 * i + 1]);
+      else *reinterpret_cast<uint32_t*>(dst + 8 * i * kBox) = pack2<T>(v[2 * i], v[2 * i + 1]);
     }
   }
 }
@@ -359,7 +383,7 @@ __device__ __forceinline__ void stmatrix_x4_trans(uint32_t addr, uint32_t r0, ui
 // pixel-major into the same boxes as stage_out_tile, from pixel row px0 of the staging half on.  bf16: the four 8 x 8
 // (channel x pixel) blocks of j = 2 jj, 2 jj + 1 go out in one stmatrix .trans, each as eight 16-byte units (one pixel's 8
 // channels, one swizzled unit per 128-byte row): conflict-free, where 2-byte stores would hit one bank for every pixel.
-template <bool F32>
+template <typename T, bool F32>
 __device__ __forceinline__ void stage_out_tile_t(const ConvKParams& p, float (&acc)[32], const float* sbias, uint8_t* stage, int px0,
                                                  int r0, int c0, int lane) {
   float b[2] = {0.f, 0.f};
@@ -398,8 +422,8 @@ __device__ __forceinline__ void stage_out_tile_t(const ConvKParams& p, float (&a
         for (int m = 0; m < 8; ++m) v[m] += b[(m >> 1) & 1];
       }
       activate(p, v);
-      stmatrix_x4_trans(dst + (uint32_t)jj * 16u * 128u, pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3]), pack_bf16x2(v[4], v[5]),
-                        pack_bf16x2(v[6], v[7]));
+      stmatrix_x4_trans(dst + (uint32_t)jj * 16u * 128u, pack2<T>(v[0], v[1]), pack2<T>(v[2], v[3]), pack2<T>(v[4], v[5]),
+                        pack2<T>(v[6], v[7]));
     }
   }
 }
@@ -408,14 +432,15 @@ __device__ __forceinline__ void stage_out_tile_t(const ConvKParams& p, float (&a
 // B operand), issued back to back as ONE commit group.  KSTEPS must be known at compile time: an MMA under a runtime
 // condition makes ptxas split the group and inject warpgroup.arrive around it (warning C7519).  LO: the same group with the
 // rows 0-63 MMAs only, for a tile whose rows 64-127 all lie outside the output (upper_half_dead); acc[1] is left as it is.
-template <int BN, int KSTEPS, bool LO = false>
+// F16: fp16 operands.
+template <int BN, int KSTEPS, bool LO = false, bool F16 = false>
 __device__ __forceinline__ void mma_kblock(float (&acc)[2][BN / 2], uint64_t ad, uint32_t a_hi, uint64_t bd, uint32_t scale_d) {
   wgmma_fence();
 #pragma unroll
   for (int k = 0; k < KSTEPS; ++k) {
     const uint32_t sd = k == 0 ? scale_d : 1u;
-    Wgmma<BN, 0, 0>::mma(acc[0], ad + (uint64_t)(2 * k), bd + (uint64_t)(2 * k), sd);
-    if constexpr (!LO) Wgmma<BN, 0, 0>::mma(acc[1], ad + (uint64_t)(a_hi + 2 * k), bd + (uint64_t)(2 * k), sd);
+    Wgmma<BN, 0, 0, F16>::mma(acc[0], ad + (uint64_t)(2 * k), bd + (uint64_t)(2 * k), sd);
+    if constexpr (!LO) Wgmma<BN, 0, 0, F16>::mma(acc[1], ad + (uint64_t)(a_hi + 2 * k), bd + (uint64_t)(2 * k), sd);
   }
   wgmma_commit();
 }
@@ -445,23 +470,24 @@ __device__ __forceinline__ bool upper_half_dead(const ConvKParams& p, const Row6
 // A operand and the input box's 128 pixel rows (xd, sixteen 8-row groups) the B operand -- one m64n128k16 per k16 step, half
 // the instructions of mma_kblock<64> for the same FLOPs.  acc[h] holds pixels 64 h .. 64 h + 63 (wgmma fragment columns
 // 8 j + ..., j = 8 h + j' -> acc[h][4 j' + ...]).
-template <int KSTEPS>
+template <int KSTEPS, bool F16 = false>
 __device__ __forceinline__ void mma_kblock_t(float (&acc)[2][32], uint64_t wd, uint64_t xd, uint32_t scale_d) {
   float(&d)[64] = reinterpret_cast<float(&)[64]>(acc);
   wgmma_fence();
 #pragma unroll
-  for (int k = 0; k < KSTEPS; ++k) Wgmma<128, 0, 0>::mma(d, wd + (uint64_t)(2 * k), xd + (uint64_t)(2 * k), k == 0 ? scale_d : 1u);
+  for (int k = 0; k < KSTEPS; ++k) Wgmma<128, 0, 0, F16>::mma(d, wd + (uint64_t)(2 * k), xd + (uint64_t)(2 * k), k == 0 ? scale_d : 1u);
   wgmma_commit();
 }
 
 // MODE: 0 = one TMA box per (tap, channel block); 1 / 3 = halo input tiles (stride 1 / stride-2 column-pair view), weights
 //       streamed through a ring; 2 / 4 = the same with the layer's weights resident in shared memory.  BN = the wgmma N and
 //       the width of the accumulator tile.  CP: CTA-pair variant (launched as clusters of two CTAs, see ConvKParams::cpair).
-//       All are compile-time so that each variant carries only its own loops.
-template <int BN, int MODE, bool CP>
-__global__ void __launch_bounds__(kConvThreads, 1)
-conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                  const __grid_constant__ CUtensorMap tmY, const ConvKParams p) {
+//       All are compile-time so that each variant carries only its own loops.  T: the operand dtype (__nv_bfloat16 or __half).
+//       The body of both kernels below, force-inlined: a call would make ptxas serialize every wgmma.
+template <typename T, int BN, int MODE, bool CP>
+__device__ __forceinline__ void conv_igemm_body(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmY,
+                                                const ConvKParams& p) {
+  constexpr bool F16 = std::is_same_v<T, __half>;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_addr = smem_u32(smem_raw);
   uint8_t* smem = smem_raw + ((1024u - (raw_addr & 1023u)) & 1023u);
@@ -682,8 +708,8 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
               if (!BRES || first) mbar_wait(&b_full[bs], BRES ? 0u : phb);
               const uint64_t ad = desc_a | (uint64_t)(a0 + (uint32_t)((tap / HG::KW) * HG::W + (tap % HG::KW)) * 8u);
               const uint64_t bd = desc_b | (uint64_t)(b_base + (uint32_t)bs * b_step);
-              if constexpr (SWAP) mma_kblock_t<4>(acc, bd, ad, started);
-              else mma_kblock<BN, 4, LO>(acc, ad, a_hi, bd, started);
+              if constexpr (SWAP) mma_kblock_t<4, F16>(acc, bd, ad, started);
+              else mma_kblock<BN, 4, LO, F16>(acc, ad, a_hi, bd, started);
               started = 1u;
               if (!BRES || prev_sa >= 0) {
                 wgmma_wait<1>();
@@ -719,9 +745,9 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             const uint64_t bd = desc | (uint64_t)(b_base + (uint32_t)stage * b_step);
             const uint32_t scale_d = (uint32_t)(kb != 0);
             switch (ksteps) {          // 16-, 32- or 64-channel K blocks
-              case 1: mma_kblock<BN, 1, LO>(acc, ad, a_hi, bd, scale_d); break;
-              case 2: mma_kblock<BN, 2, LO>(acc, ad, a_hi, bd, scale_d); break;
-              default: mma_kblock<BN, 4, LO>(acc, ad, a_hi, bd, scale_d); break;
+              case 1: mma_kblock<BN, 1, LO, F16>(acc, ad, a_hi, bd, scale_d); break;
+              case 2: mma_kblock<BN, 2, LO, F16>(acc, ad, a_hi, bd, scale_d); break;
+              default: mma_kblock<BN, 4, LO, F16>(acc, ad, a_hi, bd, scale_d); break;
             }
             wgmma_wait<1>();
             if (prev >= 0 && arrive_lane) release_b(&empty[prev]);
@@ -759,16 +785,16 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           warpgroup_bar_sync(wg);
           if constexpr (SWAP) {
             if (f32) {
-              stage_out_tile_t<true>(p, acc[h], sbias, stage, 0, r0, c0, lane);
+              stage_out_tile_t<T, true>(p, acc[h], sbias, stage, 0, r0, c0, lane);
             } else {
-              stage_out_tile_t<false>(p, acc[0], sbias, stage, 0, r0, c0, lane);
-              stage_out_tile_t<false>(p, acc[1], sbias, stage, 64, r0, c0, lane);
+              stage_out_tile_t<T, false>(p, acc[0], sbias, stage, 0, r0, c0, lane);
+              stage_out_tile_t<T, false>(p, acc[1], sbias, stage, 64, r0, c0, lane);
             }
           } else if (f32) {
-            stage_out_tile<BN, true>(p, acc[h], sbias, stage, r0, c0);
+            stage_out_tile<T, BN, true>(p, acc[h], sbias, stage, r0, c0);
           } else {
-            stage_out_tile<BN, false>(p, acc[0], sbias, stage, r0, c0);
-            if (!dead_hi) stage_out_tile<BN, false>(p, acc[1], sbias, stage, r0 + 64, c0);
+            stage_out_tile<T, BN, false>(p, acc[0], sbias, stage, r0, c0);
+            if (!dead_hi) stage_out_tile<T, BN, false>(p, acc[1], sbias, stage, r0 + 64, c0);
           }
           fence_proxy_async();
           warpgroup_bar_sync(wg);
@@ -832,14 +858,29 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             r[4 * q + 3] = __float_as_uint(f.w);
           }
           float v[16];
-          epilogue_math(p, r, n, ncol, roff, v);
-          store_chunk(p, off, n, ncol, v);
+          epilogue_math<T>(p, r, n, ncol, roff, v);
+          store_chunk<T>(p, off, n, ncol, v);
         }
       }
     }
   }
   // neither CTA of a pair may exit while its peer can still multicast into it or arrive on its barriers
   if (CP) cluster_sync_all();
+}
+
+template <int BN, int MODE, bool CP>
+__global__ void __launch_bounds__(kConvThreads, 1)
+conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                  const __grid_constant__ CUtensorMap tmY, const ConvKParams p) {
+  conv_igemm_body<__nv_bfloat16, BN, MODE, CP>(tmA, tmB, tmY, p);
+}
+
+// fp16 operands (yv6_conv_desc.reserved0 = YV6_DT_F16): fp16 wgmma, fp16 input / residual / output, fp32 accumulation
+template <int BN, int MODE, bool CP>
+__global__ void __launch_bounds__(kConvThreads, 1)
+conv_f16_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                      const __grid_constant__ CUtensorMap tmY, const ConvKParams p) {
+  conv_igemm_body<__half, BN, MODE, CP>(tmA, tmB, tmY, p);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -850,6 +891,7 @@ struct ConvPlan {
   int grid;
   size_t smem_bytes;
   CUtensorMapSwizzle swz;
+  bool f16;               // fp16 operands (conv_f16_igemm_kernel); the tile plan is the same as for bf16
 };
 
 // wgmma N of the kernel variants (accumulator registers per consumer thread = BN: two m64 halves of BN / 2)
@@ -871,7 +913,11 @@ static int plan_conv(const yv6_handle* h, const yv6_conv_desc* d, ConvPlan* plan
   YV6_REQUIRE(d->nsplit == 1 || d->nsplit == 3, "conv: nsplit must be 1 or 3");
   YV6_REQUIRE((reinterpret_cast<uintptr_t>(d->x) & 15) == 0 && (reinterpret_cast<uintptr_t>(d->w) & 15) == 0,
               "conv: x / w must be 16-byte aligned");
-  YV6_REQUIRE(d->y_dtype == YV6_DT_BF16 || d->y_dtype == YV6_DT_F32, "conv: bad y_dtype");
+  // reserved0 = operand dtype: 0 (bf16) or YV6_DT_F16 (one plane)
+  YV6_REQUIRE(d->reserved0 == 0 || d->reserved0 == YV6_DT_F16, "conv: operand dtype %d must be 0 (bf16) or YV6_DT_F16", d->reserved0);
+  plan->f16 = d->reserved0 == YV6_DT_F16;
+  YV6_REQUIRE(!plan->f16 || d->nsplit == 1, "conv: fp16 operands need nsplit == 1");
+  YV6_REQUIRE(d->y_dtype == (plan->f16 ? YV6_DT_F16 : YV6_DT_BF16) || d->y_dtype == YV6_DT_F32, "conv: bad y_dtype %d", d->y_dtype);
 
   ConvKParams& k = plan->k;
   memset(&k, 0, sizeof(k));
@@ -1056,7 +1102,7 @@ static int plan_conv(const yv6_handle* h, const yv6_conv_desc* d, ConvPlan* plan
 
   k.act = d->act;
   k.y_dtype = d->y_dtype;
-  k.fast_act = (d->y_dtype == YV6_DT_BF16 && d->nsplit != 3) ? 1 : 0;
+  k.fast_act = (d->y_dtype == YV6_DT_BF16 && d->nsplit != 3) ? 1 : 0;   // (not for fp16: 2^-11 is half its ulp)
   k.out_planes = (d->nsplit == 3 && d->y_dtype == YV6_DT_BF16) ? 3 : 1;
   k.res_planes = (d->nsplit == 3) ? 3 : 1;
   k.y = d->y;
@@ -1064,7 +1110,7 @@ static int plan_conv(const yv6_handle* h, const yv6_conv_desc* d, ConvPlan* plan
   k.y_h_stride = d->y_h_stride;
   k.y_w_stride = d->y_w_stride;
   k.y_plane_stride = d->y_plane_stride;
-  k.res = reinterpret_cast<const __nv_bfloat16*>(d->res);
+  k.res = d->res;
   k.alpha = d->alpha;
   k.res_img_stride = d->res_img_stride;
   k.res_h_stride = d->res_h_stride;
@@ -1104,23 +1150,24 @@ static int plan_conv(const yv6_handle* h, const yv6_conv_desc* d, ConvPlan* plan
 using namespace yv6;
 
 using ConvKernelFn = void (*)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const ConvKParams);
-#define YV6_CONV_MODES(BN, CP)                                                                                      \
-  {conv_igemm_kernel<BN, 0, CP>, conv_igemm_kernel<BN, 1, CP>, conv_igemm_kernel<BN, 2, CP>, conv_igemm_kernel<BN, 3, CP>, \
-   conv_igemm_kernel<BN, 4, CP>}
-// [CTA pair][BN index: 32, 64, 96, 128][mode]
-static const ConvKernelFn kConvKernels[2][4][5] = {
-    {YV6_CONV_MODES(32, false), YV6_CONV_MODES(64, false), YV6_CONV_MODES(96, false), YV6_CONV_MODES(128, false)},
-    {YV6_CONV_MODES(32, true), YV6_CONV_MODES(64, true), YV6_CONV_MODES(96, true), YV6_CONV_MODES(128, true)}};
+#define YV6_CONV_MODES(K, BN, CP) {K<BN, 0, CP>, K<BN, 1, CP>, K<BN, 2, CP>, K<BN, 3, CP>, K<BN, 4, CP>}
+#define YV6_CONV_TABLE(K)                                                                                              \
+  {{YV6_CONV_MODES(K, 32, false), YV6_CONV_MODES(K, 64, false), YV6_CONV_MODES(K, 96, false), YV6_CONV_MODES(K, 128, false)}, \
+   {YV6_CONV_MODES(K, 32, true), YV6_CONV_MODES(K, 64, true), YV6_CONV_MODES(K, 96, true), YV6_CONV_MODES(K, 128, true)}}
+// [fp16 operands][CTA pair][BN index: 32, 64, 96, 128][mode]
+static const ConvKernelFn kConvKernels[2][2][4][5] = {YV6_CONV_TABLE(conv_igemm_kernel), YV6_CONV_TABLE(conv_f16_igemm_kernel)};
+#undef YV6_CONV_TABLE
 #undef YV6_CONV_MODES
 
 // Once per device: opt the kernels in to the large dynamic shared memory and ask how many 2-CTA clusters of the conv kernel
 // (one CTA per SM) can be co-resident -- the grid of the pair variants.
 static int conv_configure(yv6_handle* h) {
   if (h->configured & YV6_CFG_CONV) return YV6_OK;
-  for (int c = 0; c < 2; ++c)
-    for (int b = 0; b < 4; ++b)
-      for (int m = 0; m < 5; ++m)
-        YV6_CHECK_CUDA(cudaFuncSetAttribute(kConvKernels[c][b][m], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->max_smem_optin));
+  for (const auto& by_pair : kConvKernels)
+    for (const auto& by_bn : by_pair)
+      for (const auto& by_mode : by_bn)
+        for (ConvKernelFn fn : by_mode)
+          YV6_CHECK_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->max_smem_optin));
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
   cfg.gridDim = dim3((unsigned)(2 * h->num_sms));
@@ -1134,7 +1181,7 @@ static int conv_configure(yv6_handle* h) {
   cfg.attrs = attr;
   cfg.numAttrs = 1;
   int n = 0;
-  if (cudaOccupancyMaxActiveClusters(&n, kConvKernels[1][3][0], &cfg) != cudaSuccess) {
+  if (cudaOccupancyMaxActiveClusters(&n, kConvKernels[0][1][3][0], &cfg) != cudaSuccess) {
     (void)cudaGetLastError();
     n = 0;                                   // pairs unavailable: the single-CTA variants are used
   }
@@ -1205,6 +1252,7 @@ extern "C" int yv6_conv_fwd(yv6_handle* h, const yv6_conv_desc* d, void* stream)
 
   // A: (C, W, H, N, plane) over the input (channel slice of a wider NHWC buffer allowed)
   CUtensorMap tmA, tmB;
+  const CUtensorMapDataType operand_type = plan.f16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
   {
     const uint64_t planes = (d->nsplit == 3) ? 3 : 1;
     cuuint64_t dims[5] = {(cuuint64_t)d->Cin, (cuuint64_t)d->W, (cuuint64_t)d->H, (cuuint64_t)d->N, planes};
@@ -1221,7 +1269,7 @@ extern "C" int yv6_conv_fwd(yv6_handle* h, const yv6_conv_desc* d, void* stream)
       box[2] = (k.halo == 2) ? HaloGeom<true>::H : HaloGeom<false>::H;
       estr[1] = estr[2] = 1;
     }
-    CUresult cr = h->encode_tiled(&tmA, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, const_cast<void*>(d->x), dims,
+    CUresult cr = h->encode_tiled(&tmA, operand_type, 5, const_cast<void*>(d->x), dims,
                                   strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, plan.swz,
                                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (cr != CUDA_SUCCESS) {
@@ -1239,7 +1287,7 @@ extern "C" int yv6_conv_fwd(yv6_handle* h, const yv6_conv_desc* d, void* stream)
     cuuint64_t strides[2] = {ktot * 2, plane_stride};
     cuuint32_t box[3] = {(cuuint32_t)k.kb_elems, (cuuint32_t)k.b_rows, 1};   // pair mode: each CTA loads half of the N tile
     cuuint32_t estr[3] = {1, 1, 1};
-    CUresult cr = h->encode_tiled(&tmB, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(d->w), dims,
+    CUresult cr = h->encode_tiled(&tmB, operand_type, 3, const_cast<void*>(d->w), dims,
                                   strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, plan.swz,
                                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (cr != CUDA_SUCCESS) {
@@ -1258,7 +1306,7 @@ extern "C" int yv6_conv_fwd(yv6_handle* h, const yv6_conv_desc* d, void* stream)
     const int box_bytes = y_box_bytes(k.BN, (int)esz);
     cuuint32_t box[4] = {(cuuint32_t)(box_bytes / esz), (cuuint32_t)k.BW, (cuuint32_t)(f32 ? k.BH / 2 : k.BH), (cuuint32_t)k.BI};
     cuuint32_t estr[4] = {1, 1, 1, 1};
-    CUresult cr = h->encode_tiled(&tmY, f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, d->y, dims,
+    CUresult cr = h->encode_tiled(&tmY, f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : operand_type, 4, d->y, dims,
                                   strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                                   box_bytes == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
                                   CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -1271,7 +1319,7 @@ extern "C" int yv6_conv_fwd(yv6_handle* h, const yv6_conv_desc* d, void* stream)
 
   const int mode = k.halo ? (k.halo == 2 ? 3 : 1) + (k.b_resident ? 1 : 0) : 0;
   const int bn_idx = k.BN == 32 ? 0 : k.BN == 64 ? 1 : k.BN == 96 ? 2 : 3;
-  ConvKernelFn fn = kConvKernels[k.cpair][bn_idx][mode];
+  ConvKernelFn fn = kConvKernels[plan.f16][k.cpair][bn_idx][mode];
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
   cfg.gridDim = dim3((unsigned)plan.grid);

@@ -6,7 +6,10 @@
 //   * yv6_upsample2x     : nn.Upsample(scale_factor=2, mode='nearest') of Lite_EffiNeck (reppan.py:1147-1149)
 // All of them are memory-bound.  Activations are NHWC bf16 channel slices (base pointer + channel pitch), one plane or the
 // three bf16 planes (hi, mid, lo) of the fp32-equivalent mode; in that mode every value is read as the fp32 sum of its
-// planes, computed in fp32 and written back as three planes (the split of ops.split3).
+// planes, computed in fp32 and written back as three planes (the split of ops.split3).  yv6_dwconv_fwd_f16 and yv6_se_fwd with
+// reserved0 = YV6_DT_F16 run the same kernels on one plane of fp16 activations (T = __half below).
+#include <type_traits>
+
 #include "yv6_common.cuh"
 #include "yv6_handle.h"
 
@@ -16,12 +19,17 @@ namespace {
 __device__ __forceinline__ float hardswish(float v) { return v * fminf(fmaxf(v + 3.f, 0.f), 6.f) * (1.f / 6.f); }   // nn.Hardswish
 __device__ __forceinline__ float hardsigmoid(float v) { return fminf(fmaxf(v + 3.f, 0.f), 6.f) * (1.f / 6.f); }    // nn.Hardsigmoid
 
-__device__ __forceinline__ float load_val(const __nv_bfloat16* p, int64_t plane_stride, int planes) {
-  float v = __bfloat162float(p[0]);
-  for (int pl = 1; pl < planes; ++pl) v += __bfloat162float(p[pl * plane_stride]);
+__device__ __forceinline__ float to_float(__nv_bfloat16 v) { return __bfloat162float(v); }
+__device__ __forceinline__ float to_float(__half v) { return __half2float(v); }
+
+template <typename T>
+__device__ __forceinline__ float load_val(const T* p, int64_t plane_stride, int planes) {
+  float v = to_float(p[0]);
+  for (int pl = 1; pl < planes; ++pl) v += to_float(p[pl * plane_stride]);
   return v;
 }
 
+__device__ __forceinline__ void store_val(__half* p, int64_t, int, float v) { p[0] = __float2half_rn(v); }   // one plane
 __device__ __forceinline__ void store_val(__nv_bfloat16* p, int64_t plane_stride, int planes, float v) {
   const __nv_bfloat16 hi = __float2bfloat16(v);
   p[0] = hi;
@@ -43,16 +51,30 @@ __device__ __forceinline__ void store_val(__nv_bfloat16* p, int64_t plane_stride
 constexpr int kDwTH = 8, kDwTW = 16, kDwCV = 8, kDwThreads = kDwTH * kDwTW;
 
 struct DwParams {
-  const __nv_bfloat16* x;
+  const void* x;            // bf16 or fp16 (T)
   const float* w;           // [k*k][C]
   const float* b;           // [C] or null
-  __nv_bfloat16* y;
+  void* y;
   int64_t x_pitch, y_pitch, x_plane, y_plane;
   int32_t N, H, W, C, Ho, Wo, act, planes, x_vec, y_vec, tiles_w;
 };
 
-template <int K, int S>
-__global__ void __launch_bounds__(kDwThreads) dwconv_kernel(const DwParams p) {
+template <typename T>
+__device__ __forceinline__ uint32_t pack2(float a, float b) {
+  if constexpr (std::is_same_v<T, __half>) {
+    const __half2 v = __floats2half2_rn(a, b);
+    return *reinterpret_cast<const uint32_t*>(&v);
+  } else {
+    const __nv_bfloat162 v = __floats2bfloat162_rn(a, b);
+    return *reinterpret_cast<const uint32_t*>(&v);
+  }
+}
+template <typename T> struct Pair2;
+template <> struct Pair2<__nv_bfloat16> { using type = __nv_bfloat162; };
+template <> struct Pair2<__half> { using type = __half2; };
+
+template <int K, int S, typename T>
+__device__ __forceinline__ void dwconv_body(const DwParams& p) {
   constexpr int IH = (kDwTH - 1) * S + K, IW = (kDwTW - 1) * S + K;
   __shared__ float4 tile[IH * IW * 2];
   __shared__ float wsm[K * K * kDwCV];
@@ -73,19 +95,19 @@ __global__ void __launch_bounds__(kDwThreads) dwconv_kernel(const DwParams p) {
 #pragma unroll
     for (int c = 0; c < kDwCV; ++c) v[c] = 0.f;
     if (h >= 0 && h < p.H && w >= 0 && w < p.W) {
-      const __nv_bfloat16* src = p.x + ((int64_t)(n * p.H + h) * p.W + w) * p.x_pitch + c0;
+      const T* src = static_cast<const T*>(p.x) + ((int64_t)(n * p.H + h) * p.W + w) * p.x_pitch + c0;
       for (int pl = 0; pl < p.planes; ++pl, src += p.x_plane) {
         if (vec_x) {
           const uint4 q = __ldg(reinterpret_cast<const uint4*>(src));
           const uint32_t u[4] = {q.x, q.y, q.z, q.w};
 #pragma unroll
           for (int j = 0; j < 4; ++j) {
-            const __nv_bfloat162 b2 = *reinterpret_cast<const __nv_bfloat162*>(&u[j]);
+            const typename Pair2<T>::type b2 = *reinterpret_cast<const typename Pair2<T>::type*>(&u[j]);
             v[2 * j] += __low2float(b2);
             v[2 * j + 1] += __high2float(b2);
           }
         } else {
-          for (int c = 0; c < nc; ++c) v[c] += __bfloat162float(src[c]);
+          for (int c = 0; c < nc; ++c) v[c] += to_float(src[c]);
         }
       }
     }
@@ -115,15 +137,12 @@ __global__ void __launch_bounds__(kDwThreads) dwconv_kernel(const DwParams p) {
 #pragma unroll
     for (int c = 0; c < kDwCV; ++c) acc[c] = hardswish(acc[c]);
   }
-  __nv_bfloat16* dst = p.y + ((int64_t)(n * p.Ho + ho) * p.Wo + wo) * p.y_pitch + c0;
+  T* dst = static_cast<T*>(p.y) + ((int64_t)(n * p.Ho + ho) * p.Wo + wo) * p.y_pitch + c0;
   if (p.planes == 1 && p.y_vec && nc == kDwCV) {
     uint4 q;
     uint32_t* u = reinterpret_cast<uint32_t*>(&q);
 #pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const __nv_bfloat162 b2 = __floats2bfloat162_rn(acc[2 * j], acc[2 * j + 1]);
-      u[j] = *reinterpret_cast<const uint32_t*>(&b2);
-    }
+    for (int j = 0; j < 4; ++j) u[j] = pack2<T>(acc[2 * j], acc[2 * j + 1]);
     *reinterpret_cast<uint4*>(dst) = q;
   } else {
 #pragma unroll
@@ -131,6 +150,11 @@ __global__ void __launch_bounds__(kDwThreads) dwconv_kernel(const DwParams p) {
       if (c < nc) store_val(dst + c, p.y_plane, p.planes, acc[c]);
   }
 }
+
+template <int K, int S>
+__global__ void __launch_bounds__(kDwThreads) dwconv_kernel(const DwParams p) { dwconv_body<K, S, __nv_bfloat16>(p); }
+template <int K, int S>
+__global__ void __launch_bounds__(kDwThreads) dwconv_f16_kernel(const DwParams p) { dwconv_body<K, S, __half>(p); }
 
 // ------------------------------------------------------------------------------------------------
 // squeeze-excite: one CTA per image does the whole block -- the mean, both FCs and the scaling -- so nothing crosses CTAs:
@@ -140,17 +164,18 @@ __global__ void __launch_bounds__(kDwThreads) dwconv_kernel(const DwParams p) {
 constexpr int kSeThreads = 512, kSeMaxC = 512, kSeMaxCr = 128;
 
 struct SeParams {
-  __nv_bfloat16* x;
+  void* x;                  // bf16 or fp16 (T)
   const float *w1, *b1, *w2, *b2;
   int64_t pitch, plane;
   int32_t HW, C, Cr, planes;
 };
 
-__global__ void __launch_bounds__(kSeThreads) se_kernel(const SeParams p) {
+template <typename T>
+__device__ __forceinline__ void se_body(const SeParams& p) {
   __shared__ double part[kSeThreads];
   __shared__ float mean[kSeMaxC], hid[kSeMaxCr], scale[kSeMaxC];
   const int t = threadIdx.x, C = p.C, P = kSeThreads / C;
-  __nv_bfloat16* x = p.x + (int64_t)blockIdx.x * p.HW * p.pitch;
+  T* x = static_cast<T*>(p.x) + (int64_t)blockIdx.x * p.HW * p.pitch;
   const int c = t % C, ph = t / C;
   if (ph < P) {
     double s = 0.0;
@@ -177,10 +202,13 @@ __global__ void __launch_bounds__(kSeThreads) se_kernel(const SeParams p) {
   }
   __syncthreads();
   for (int64_t i = t; i < (int64_t)p.HW * C; i += kSeThreads) {
-    __nv_bfloat16* e = x + (i / C) * p.pitch + i % C;
+    T* e = x + (i / C) * p.pitch + i % C;
     store_val(e, p.plane, p.planes, load_val(e, p.plane, p.planes) * scale[i % C]);
   }
 }
+
+__global__ void __launch_bounds__(kSeThreads) se_kernel(const SeParams p) { se_body<__nv_bfloat16>(p); }
+__global__ void __launch_bounds__(kSeThreads) se_f16_kernel(const SeParams p) { se_body<__half>(p); }
 
 // ------------------------------------------------------------------------------------------------
 // channel shuffle / nearest 2x upsample: one thread per output element (and plane).  These move a few hundred KB per
@@ -220,8 +248,9 @@ __global__ void upsample2x_kernel(const CopyParams p) {
 }
 
 template <int K, int S>
-cudaError_t launch_dw(const DwParams& p, dim3 grid, cudaStream_t st) {
-  dwconv_kernel<K, S><<<grid, kDwThreads, 0, st>>>(p);
+cudaError_t launch_dw(const DwParams& p, dim3 grid, cudaStream_t st, bool f16) {
+  if (f16) dwconv_f16_kernel<K, S><<<grid, kDwThreads, 0, st>>>(p);
+  else dwconv_kernel<K, S><<<grid, kDwThreads, 0, st>>>(p);
   return cudaGetLastError();
 }
 
@@ -232,9 +261,10 @@ bool aligned16(const void* ptr) { return (reinterpret_cast<uintptr_t>(ptr) & 15)
 
 using namespace yv6;
 
-extern "C" int yv6_dwconv_fwd(yv6_handle* h, const yv6_dw_desc* d, void* stream) {
+static int dwconv_fwd(yv6_handle* h, const yv6_dw_desc* d, void* stream, bool f16) {
   yv6_device_guard _dev(h);
   YV6_REQUIRE(h && d && d->x && d->w && d->y, "dwconv: null argument");
+  YV6_REQUIRE(!f16 || d->nsplit == 1, "dwconv_f16: nsplit must be 1");
   YV6_REQUIRE((d->k == 3 || d->k == 5) && (d->stride == 1 || d->stride == 2), "dwconv: k=%d stride=%d (k in {3,5}, stride in {1,2})",
               d->k, d->stride);
   YV6_REQUIRE(d->N > 0 && d->H > 0 && d->W > 0 && d->C > 0 && d->N <= 65535, "dwconv: bad shape %dx%dx%dx%d", d->N, d->H, d->W, d->C);
@@ -242,10 +272,10 @@ extern "C" int yv6_dwconv_fwd(yv6_handle* h, const yv6_dw_desc* d, void* stream)
   YV6_REQUIRE(d->act == YV6_ACT_NONE || d->act == YV6_ACT_HARDSWISH, "dwconv: act %d (none or hardswish)", d->act);
   YV6_REQUIRE(d->nsplit == 1 || d->nsplit == 3, "dwconv: nsplit %d", d->nsplit);
   DwParams p;
-  p.x = static_cast<const __nv_bfloat16*>(d->x);
+  p.x = d->x;
   p.w = d->w;
   p.b = d->bias;
-  p.y = static_cast<__nv_bfloat16*>(d->y);
+  p.y = d->y;
   p.x_pitch = d->x_c_total, p.y_pitch = d->y_c_total, p.x_plane = d->x_plane_stride, p.y_plane = d->y_plane_stride;
   p.N = d->N, p.H = d->H, p.W = d->W, p.C = d->C;
   p.Ho = (d->H - 1) / d->stride + 1, p.Wo = (d->W - 1) / d->stride + 1;   // padding k / 2
@@ -256,11 +286,14 @@ extern "C" int yv6_dwconv_fwd(yv6_handle* h, const yv6_dw_desc* d, void* stream)
   const dim3 grid(p.tiles_w * ((p.Ho + kDwTH - 1) / kDwTH), (d->C + kDwCV - 1) / kDwCV, d->N);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   cudaError_t e;
-  if (d->k == 3) e = d->stride == 1 ? launch_dw<3, 1>(p, grid, st) : launch_dw<3, 2>(p, grid, st);
-  else e = d->stride == 1 ? launch_dw<5, 1>(p, grid, st) : launch_dw<5, 2>(p, grid, st);
+  if (d->k == 3) e = d->stride == 1 ? launch_dw<3, 1>(p, grid, st, f16) : launch_dw<3, 2>(p, grid, st, f16);
+  else e = d->stride == 1 ? launch_dw<5, 1>(p, grid, st, f16) : launch_dw<5, 2>(p, grid, st, f16);
   YV6_CHECK_CUDA(e);
   return YV6_OK;
 }
+
+extern "C" int yv6_dwconv_fwd(yv6_handle* h, const yv6_dw_desc* d, void* stream) { return dwconv_fwd(h, d, stream, false); }
+extern "C" int yv6_dwconv_fwd_f16(yv6_handle* h, const yv6_dw_desc* d, void* stream) { return dwconv_fwd(h, d, stream, true); }
 
 extern "C" int yv6_se_fwd(yv6_handle* h, const yv6_se_desc* d, void* stream) {
   yv6_device_guard _dev(h);
@@ -269,8 +302,11 @@ extern "C" int yv6_se_fwd(yv6_handle* h, const yv6_se_desc* d, void* stream) {
               kSeMaxC, kSeMaxCr);
   YV6_REQUIRE(d->N > 0 && d->HW > 0 && d->c_total >= d->C, "se: bad shape N=%d HW=%d", d->N, d->HW);
   YV6_REQUIRE(d->nsplit == 1 || d->nsplit == 3, "se: nsplit %d", d->nsplit);
-  SeParams p{static_cast<__nv_bfloat16*>(d->x), d->w1, d->b1, d->w2, d->b2, d->c_total, d->plane_stride, d->HW, d->C, d->Cr, d->nsplit};
-  se_kernel<<<d->N, kSeThreads, 0, static_cast<cudaStream_t>(stream)>>>(p);
+  YV6_REQUIRE(d->reserved0 == 0 || (d->reserved0 == YV6_DT_F16 && d->nsplit == 1), "se: operand dtype %d (0 = bf16, or YV6_DT_F16 with nsplit 1)",
+              d->reserved0);
+  SeParams p{d->x, d->w1, d->b1, d->w2, d->b2, d->c_total, d->plane_stride, d->HW, d->C, d->Cr, d->nsplit};
+  if (d->reserved0 == YV6_DT_F16) se_f16_kernel<<<d->N, kSeThreads, 0, static_cast<cudaStream_t>(stream)>>>(p);
+  else se_kernel<<<d->N, kSeThreads, 0, static_cast<cudaStream_t>(stream)>>>(p);
   YV6_CHECK_CUDA(cudaGetLastError());
   return YV6_OK;
 }

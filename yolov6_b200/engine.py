@@ -6,8 +6,9 @@ decode (Model.forward yolo.py:33-41, Detect.forward effidehead.py:93-139), this 
   * pre-allocated NHWC activation buffers (concats are channel slices),
   * a prepared list of C-ABI descriptors per input shape, replayed per batch -- optionally as one
     captured CUDA graph (no Python / launch overhead in steady state).
-Precision modes: "bf16" (bf16 operands, fp32 accumulate) and "fp32" (bf16x3 split operands: fp32-
-equivalent products, used for the 1e-4 parity bar of BASELINE.json).
+Precision modes: "bf16" (bf16 operands, fp32 accumulate), "fp16" (fp16 operands and activations, fp32 accumulate: the same
+launches and tile plans as bf16, 3 more mantissa bits, activations beyond 65504 become inf as under the reference's --half) and
+"fp32" (bf16x3 split operands: fp32-equivalent products, used for the 1e-4 parity bar of BASELINE.json).
 """
 import ctypes as C
 import itertools
@@ -18,7 +19,7 @@ import torch
 
 from . import _lib, ops
 from ._lib import ConvDesc
-from .fold import fold_op, se_weights
+from .fold import fold_op, se_weights, to_f16
 
 
 def siblings(g):
@@ -131,12 +132,12 @@ def _viewer(g, N, H, W, sibling, addr):
     return view
 
 
-def conv_launches(g, N, H, W, nsplit, sibling, addr, plan_fn):
+def conv_launches(g, N, H, W, nsplit, sibling, addr, plan_fn, f16=False):
     """Descriptors of the conv launches of one inference forward of graph g over an [N, 3, H, W] input, in launch order:
     {op index: [ConvDesc, ...]} -- four 1x1 quadrant launches for a transposed conv, one otherwise; the first conv of a sibling pair
     computes both.  Descriptors only: no allocation and no CUDA call, so the planner can be checked on these launches without a GPU.
 
-    nsplit: 1 (bf16) or 3 (bf16x3 planes); sibling: siblings(g) or {}.  addr(kind, key, q=0) resolves device addresses:
+    nsplit: 1 (bf16, or fp16 if f16) or 3 (bf16x3 planes); sibling: siblings(g) or {}.  addr(kind, key, q=0) resolves device addresses:
     ("buf", buffer index) activation buffers, ("fused", first conv of the pair) the [.., 2 x Cout] sibling outputs,
     ("head", "cls" | "reg") the [N, A, ch] fp32 head tensors, ("w", op index, quadrant q of a transposed conv) packed weights,
     ("w_pair" | "w_fused" | "bias" | "bias_fused", op index) the other packed weights and padded biases; ("alpha", op index) is
@@ -160,7 +161,7 @@ def conv_launches(g, N, H, W, nsplit, sibling, addr, plan_fn):
             lo, hi = conv_window(g, op)
             x_off, cin = x_off - op.src.c_off + lo, hi - lo
         ws = (2 * op.cout if fused else op.cout, k, k, cin)
-        kw = dict(x_c_off=x_off, bias=addr("bias_fused" if fused else "bias", i), stride=s, act=op.act, nsplit=nsplit)
+        kw = dict(x_c_off=x_off, bias=addr("bias_fused" if fused else "bias", i), stride=s, act=op.act, nsplit=nsplit, f16=f16)
         if op.res is not None:
             _, r, r_off, (_, rh, rw, rct) = view(op.res)
             kw.update(res=r, res_c_off=r_off, res_strides=(rh * rw * rct, rw * rct, rct), alpha=addr("alpha", i))
@@ -182,16 +183,18 @@ def conv_launches(g, N, H, W, nsplit, sibling, addr, plan_fn):
     return out
 
 
-def forward_launches(g, N, H, W, nsplit, addr, plan_fn, u8=False):
+def forward_launches(g, N, H, W, nsplit, addr, plan_fn, u8=False, f16=False):
     """Every launch of one inference forward of graph g over an [N, 3, H, W] input (uint8 if u8), in launch order, as InferLaunch
     records: stem, the conv launches of conv_launches (the fused head siblings of siblings(g) included), SPPF pool, depthwise
     conv, SE, channel shuffle, upsample (the head decode is not included).  Records only: no allocation and no CUDA call, so the
     launches can be checked without a GPU.  The stem's input address is 0 (set per forward).
 
-    nsplit, addr and plan_fn as for conv_launches; addr also resolves ("w_dev" | "b_dev" | "w1" | "b1" | "w2" | "b2", op index):
+    nsplit, addr, plan_fn and f16 (fp16 activations: the _f16 entry points, fp16 descriptors) as for conv_launches; addr also
+    resolves ("w_dev" | "b_dev" | "w1" | "b1" | "w2" | "b2", op index):
     the stem, depthwise and SE weights and biases."""
     sibling = siblings(g)
-    convs = conv_launches(g, N, H, W, nsplit, sibling, addr, plan_fn)
+    convs = conv_launches(g, N, H, W, nsplit, sibling, addr, plan_fn, f16)
+    sfx = "_f16" if f16 else ""
     view = _viewer(g, N, H, W, sibling, addr)
 
     def span(t):
@@ -211,19 +214,19 @@ def forward_launches(g, N, H, W, nsplit, addr, plan_fn, u8=False):
             assert c0 == 0
             d = ops.stem_desc(0, N, H, W, u8, addr("w_dev", i), addr("b_dev", i), stem_channels(g, op), op.act, y, nsplit,
                               N * h * w * pitch if nsplit == 3 else 0)
-            out.append(InferLaunch("stem", "yv6_stem_fwd", (C.byref(d),), d, writes=[(key, 0, stem_channels(g, op))], **rec))
+            out.append(InferLaunch("stem", "yv6_stem_fwd" + sfx, (C.byref(d),), d, writes=[(key, 0, stem_channels(g, op))], **rec))
         elif op.kind in ("pool", "dw", "se", "shuffle", "up"):
             (x, xp, xpl), (_, _, _, (_, h, w, _)) = at(op.src), view(op.src)
             if op.kind == "pool":      # in place: channels [0, C) -> [C, 4C) of one buffer
                 key, y, _, (_, h, w, ct) = view(op.dst)
-                out.append(InferLaunch("pool", "yv6_sppf_pool", (y, N, h, w, op.cin, ct, nsplit, N * h * w * ct if nsplit == 3 else 0),
+                out.append(InferLaunch("pool", "yv6_sppf_pool" + sfx, (y, N, h, w, op.cin, ct, nsplit, N * h * w * ct if nsplit == 3 else 0),
                                        reads=[(key, 0, op.cin)], writes=[(key, op.cin, 4 * op.cin)], **rec))
             elif op.kind == "dw":
                 y, yp, ypl = at(op.dst)
                 d = ops.dw_desc(x, (N, h, w, xp), xpl, addr("w_dev", i), addr("b_dev", i), op.cin, op.k, op.s, op.act, y, yp, ypl, nsplit)
-                out.append(InferLaunch("dw", "yv6_dwconv_fwd", (C.byref(d),), d, reads=[span(op.src)], writes=[span(op.dst)], **rec))
+                out.append(InferLaunch("dw", "yv6_dwconv_fwd" + sfx, (C.byref(d),), d, reads=[span(op.src)], writes=[span(op.dst)], **rec))
             elif op.kind == "se":      # in place
-                d = ops.se_desc(x, N, h * w, op.cin, op.cout, xp, xpl, *(addr(k, i) for k in ("w1", "b1", "w2", "b2")), nsplit=nsplit)
+                d = ops.se_desc(x, N, h * w, op.cin, op.cout, xp, xpl, *(addr(k, i) for k in ("w1", "b1", "w2", "b2")), nsplit=nsplit, f16=f16)
                 out.append(InferLaunch("se", "yv6_se_fwd", (C.byref(d),), d, reads=[span(op.src)], writes=[span(op.src)], **rec))
             elif op.kind == "shuffle":
                 out.append(InferLaunch("shuffle", "yv6_channel_shuffle", (x, xp, xpl, *at(op.src2), N * h * w, op.cin, *at(op.dst), nsplit),
@@ -260,7 +263,7 @@ class InferEngine:
         if device.type != "cuda":
             raise RuntimeError("yolov6_b200 runs its networks on sm_90a CUDA kernels only (no CPU fallback); "
                                f"got device {device}")
-        assert precision in ("bf16", "fp32")
+        assert precision in ("bf16", "fp16", "fp32")
         self.g = graph
         self.device = device
         self.precision = precision
@@ -275,12 +278,24 @@ class InferEngine:
         self._pinned = set()  # shapes captured into CUDA graphs (their buffers must outlive the graph)
         self._pack(state_dict)
 
+    @property
+    def f16(self):
+        """fp16 operands and activations (precision "fp16")."""
+        return self.precision == "fp16"
+
+    @property
+    def act_dtype(self):
+        """dtype of the activation buffers (bf16 planes in the fp32 mode)."""
+        return torch.float16 if self.f16 else torch.bfloat16
+
     # ------------------------------------------------------------------ weight packing
     def _pack(self, sd):
         sd = {k: v.detach().cpu() for k, v in sd.items()}
         dev = self.device
 
-        def planes(w):       # KRSC weights in the precision's operand layout
+        def planes(w, name):  # KRSC weights in the precision's operand layout (folded in fp64, rounded once)
+            if self.f16:
+                return to_f16(w, name).contiguous().to(dev)
             w = w.float().to(dev)
             return ops.split3(w).contiguous() if self.nsplit == 3 else w.to(torch.bfloat16).contiguous()
 
@@ -296,6 +311,8 @@ class InferEngine:
             if op.kind == "stem":
                 cp = stem_channels(self.g, op)
                 w, b = torch.cat([w, w.new_zeros((cp - op.cout,) + w.shape[1:])]), torch.cat([b, b.new_zeros(cp - op.cout)])
+                if self.f16:                   # the stem kernel rounds its fp32 weights to fp16
+                    to_f16(w, op.name)
                 ent["w_dev"] = w.float().permute(1, 2, 3, 0).contiguous().to(dev)       # [3][3][3][Cout]
                 ent["b_dev"] = b.float().contiguous().to(dev)
             elif op.kind == "dw":
@@ -305,15 +322,15 @@ class InferEngine:
             else:
                 w = w if op.kind == "convT" else window_weights(self.g, op, w)
                 ws = w if isinstance(w, list) else [w]
-                ent["w"] = [planes(wi) for wi in ws]
+                ent["w"] = [planes(wi, op.name) for wi in ws]
                 if pair_view_candidate(op):      # [Cout][3][2][2*Cin] weights of the column-pair view (see pair_view)
-                    ent["w_pair"] = planes(ops.pair_view_weights(ws[0].float()))
+                    ent["w_pair"] = planes(ops.pair_view_weights(ws[0]), op.name)
                 ent["bias"] = ops.pad_bias(b.to(dev), op.cout)
             ent["alpha"] = float(sd[op.alpha]) if (op.alpha and op.res is not None) else 1.0
             self.weights[i] = ent
         for i, j in self.sibling.items():      # one conv with 2 x Cout output channels: [cls branch | reg branch]
             (wa, ba), (wb, bb) = fold_op(sd, self.g.ops[i]), fold_op(sd, self.g.ops[j])
-            self.weights[i]["w_fused"] = planes(torch.cat([wa, wb], 0))
+            self.weights[i]["w_fused"] = planes(torch.cat([wa, wb], 0), self.g.ops[i].name)
             self.weights[i]["bias_fused"] = ops.pad_bias(torch.cat([ba, bb]).to(dev), 2 * self.g.ops[i].cout)
 
     # ------------------------------------------------------------------ per-shape plan
@@ -335,7 +352,7 @@ class InferEngine:
 
         def zeros(level, c):
             shape = (N, H >> level, W >> level, c)
-            return torch.zeros((P,) + shape if P == 3 else shape, dtype=torch.bfloat16, device=dev)
+            return torch.zeros((P,) + shape if P == 3 else shape, dtype=self.act_dtype, device=dev)
 
         plan = _Plan()
         plan.bufs = [zeros(b.level, b.c_total) for b in g.bufs]
@@ -357,7 +374,8 @@ class InferEngine:
             t = self.weights[key][kind]
             return (t[q] if kind == "w" else t).data_ptr()
 
-        plan.launches = forward_launches(g, N, H, W, P, addr, lambda d: ops.plan_of(d, dev.index or 0), in_dtype == torch.uint8)
+        plan.launches = forward_launches(g, N, H, W, P, addr, lambda d: ops.plan_of(d, dev.index or 0), in_dtype == torch.uint8,
+                                         self.f16)
         plan.stem = next(r.desc for r in plan.launches if r.kind == "stem")
         plan.neck_start = next((j for j, r in enumerate(plan.launches) if r.kind == "conv" and r.name.startswith("neck.")), 0)
         lvl = [(C.c_int32 * len(sizes))(*[h for h, _ in sizes]), (C.c_int32 * len(sizes))(*[w for _, w in sizes]),
@@ -500,7 +518,7 @@ class InferEngine:
         return self._heads(self._plan(N, H, W, in_dtype), head_set)
 
     def feature_maps(self, N, H, W, in_dtype=torch.float32):
-        """Neck outputs as NCHW views (reference `featmaps`, yolo.py:37-39); bf16 (hi plane in fp32 mode)."""
+        """Neck outputs as NCHW views (reference `featmaps`, yolo.py:37-39); bf16 (hi plane in fp32 mode), fp16 in fp16 mode."""
         plan = self._plan(N, H, W, in_dtype)
         out = []
         for t in self.g.feat:

@@ -75,6 +75,19 @@ def fold_op(sd, op):
     raise ValueError(op.layout)
 
 
+F16_MAX = 65504.0      # largest finite fp16
+
+
+def to_f16(w, name):
+    """Folded weights rounded to fp16, the fp16 mode's operands.  Folding can scale a weight past fp16's finite range (a BatchNorm
+    with a tiny running variance); such a weight would become inf, so it raises ValueError naming the layer instead."""
+    h = w.to(torch.float16)
+    if not torch.isfinite(h).all():
+        raise ValueError(f"{name}: a folded weight ({float(w.abs().max()):.6g}) is outside fp16's finite range (+-{F16_MAX:g}); "
+                         "run this model in the bf16 or fp32 precision mode")
+    return h
+
+
 def se_weights(sd, op):
     """SEBlock FCs, unfolded (common.py:745-757): (w1 [Cr, C], b1 [Cr], w2 [C, Cr], b2 [C]) in fp64."""
     n = op.name

@@ -233,8 +233,10 @@ class Model(nn.Module):
 
     # ------------------------------------------------------------------ execution
     def set_precision(self, precision):
-        """'bf16' (speed: bf16 operands, fp32 accumulate) or 'fp32' (bf16x3 operands, fp32-equivalent)."""
-        assert precision in ("bf16", "fp32")
+        """Inference precision: 'bf16' (speed: bf16 operands, fp32 accumulate), 'fp16' (fp16 operands and activations, fp32
+        accumulate: the reference's --half path; activations beyond 65504 become inf) or 'fp32' (bf16x3 operands, fp32-equivalent).
+        Training runs the same way whatever the setting."""
+        assert precision in ("bf16", "fp16", "fp32")
         self.precision = precision
         return self
 
