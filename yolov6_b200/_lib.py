@@ -315,6 +315,12 @@ def check(rc):
         raise RuntimeError(f"yolov6_b200 kernel call failed ({rc}): {lib().yv6_last_error().decode()}")
 
 
+def require_cuda(t, what):
+    """RuntimeError unless tensor `t` lives on a CUDA device; `what` names the caller and its verb ("... runs")."""
+    if t.device.type != "cuda":
+        raise RuntimeError(f"{what} on CUDA tensors only (no CPU fallback)")
+
+
 def handle(device_index=0):
     """Per-device `yv6_handle*` (created lazily, cached for the life of the process)."""
     h = _handles.get(device_index)

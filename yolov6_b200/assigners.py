@@ -48,9 +48,8 @@ def _workspace(dev, nbytes):
 
 
 def tal_compact(pd_scores, pd_bboxes, anc_points, gt, mask_gt, topk=13, alpha=1.0, beta=6.0, eps=1e-9, stream=None):
+    _lib.require_cuda(pd_scores, "yolov6_b200 assigners run")
     dev = pd_scores.device
-    if dev.type != "cuda":
-        raise RuntimeError("yolov6_b200 assigners run on CUDA tensors only (no CPU fallback)")
     B, A, nc = pd_scores.shape
     G = gt.shape[1]
     out = _Compact()
@@ -68,9 +67,8 @@ def tal_compact(pd_scores, pd_bboxes, anc_points, gt, mask_gt, topk=13, alpha=1.
 
 
 def atss_compact(anc_bboxes, n_level_bboxes, gt, mask_gt, pd_bboxes, nc, topk=9, stream=None):
+    _lib.require_cuda(anc_bboxes, "yolov6_b200 assigners run")
     dev = anc_bboxes.device
-    if dev.type != "cuda":
-        raise RuntimeError("yolov6_b200 assigners run on CUDA tensors only (no CPU fallback)")
     B, G = gt.shape[:2]
     A = anc_bboxes.shape[0]
     out = _Compact()

@@ -8,6 +8,7 @@ Same constructor and call signature as the reference (yolov6/models/losses/loss.
 produced by the same kernel launch as the forward values); `loss_items` = [iou, dfl, cls] weighted and
 detached (loss.py:179-182).  The whole path (target padding, box decode, TAL or ATSS, VFL + IoU + DFL,
 normalisation) runs on the device with no host synchronisation; failures surface as RuntimeError.
+The anchor-aided (loss_fuseab.py) and self-distillation (loss_distill.py) losses subclass it.
 """
 import ctypes as C
 
@@ -19,20 +20,24 @@ from .assigners import _p, atss_compact, generate_anchors_train, tal_compact
 IOU_TYPES = {"giou": 0, "siou": 1, "ciou": 2, "diou": 3}
 
 
-class _DetLossFn(torch.autograd.Function):
+class LossFn(torch.autograd.Function):
+    """Scalar loss whose gradients w.r.t. its tensor inputs were produced by the kernels already: forward returns state['out'][0],
+    backward hands out `grads` (one per tensor) scaled by the incoming gradient, in each tensor's dtype."""
+
     @staticmethod
-    def forward(ctx, pred_scores, pred_distri, state):
-        ctx.save_for_backward(state["grad_scores"], state["grad_distri"])
-        ctx.shapes = (pred_scores.dtype, pred_distri.dtype)
+    def forward(ctx, state, grads, *tensors):
+        ctx.save_for_backward(*grads)
+        ctx.dtypes = [t.dtype for t in tensors]
         return state["out"][0].clone()
 
     @staticmethod
     def backward(ctx, grad_out):
-        gs, gd = ctx.saved_tensors
-        return (gs * grad_out).to(ctx.shapes[0]), (gd * grad_out).to(ctx.shapes[1]), None
+        return (None, None, *[(g * grad_out).to(dt) for g, dt in zip(ctx.saved_tensors, ctx.dtypes)])
 
 
 class ComputeLoss:
+    _norm_gt_zero = 0       # subclasses: 1 = divide by target_scores_sum whenever it is > 0 (loss_distill.py:190-191, 318-323)
+
     def __init__(self, fpn_strides=[8, 16, 32], grid_cell_size=5.0, grid_cell_offset=0.5, num_classes=80,
                  ori_img_size=640, warmup_epoch=4, use_dfl=True, reg_max=16, iou_type='giou',
                  loss_weight={'class': 1.0, 'iou': 2.5, 'dfl': 0.5}):
@@ -47,21 +52,21 @@ class ComputeLoss:
         self.loss_weight = loss_weight
         self._anchor_key, self._anchors = None, None
         self.last_assignment = None
-        self._norm_gt_zero = 0      # subclasses: 1 = divide by target_scores_sum whenever it is > 0 (loss_distill.py:190-191, 318-323)
+
+    def _build_anchors(self, sizes, device):
+        return generate_anchors_train(sizes, self.fpn_strides, device, self.grid_cell_size, self.grid_cell_offset)
 
     def _get_anchors(self, sizes, device):
         key = (tuple(sizes), str(device))
         if key != self._anchor_key:       # cached like loss.py:63-69
-            self._anchors = generate_anchors_train(sizes, self.fpn_strides, device, self.grid_cell_size, self.grid_cell_offset)
-            self._anchor_key = key
+            self._anchors, self._anchor_key = self._build_anchors(sizes, device), key
         return self._anchors
 
     def __call__(self, outputs, targets, epoch_num, step_num, batch_height, batch_width):
         feats, pred_scores, pred_distri = outputs
         sizes = [tuple(f.shape[2:]) for f in feats]
         state = self.forward_backward(pred_scores, pred_distri, sizes, targets, epoch_num, batch_height, batch_width)
-        loss = _DetLossFn.apply(pred_scores, pred_distri, state)
-        return loss, state["out"][1:4].detach().clone()
+        return LossFn.apply(state, [state["grad_scores"], state["grad_distri"]], pred_scores, pred_distri), state["out"][1:4].detach().clone()
 
     def forward_backward(self, pred_scores, pred_distri, sizes, targets, epoch_num, batch_height, batch_width, max_gt=None,
                          grad_scores=None, grad_distri=None, grad_scale=1.0, reuse=None, weights=None):
@@ -72,60 +77,64 @@ class ComputeLoss:
         host read when `targets` lives on the device).  `grad_*` let the caller provide the output buffers.
         `reuse` = the state of an earlier call: its padded targets and label assignment are used as they are (a second box
         branch scored against the same assignment, loss_distill_ns.py:93,150-160); `weights` overrides the (class, iou, dfl) weights."""
+        _lib.require_cuda(pred_scores, "yolov6_b200.ComputeLoss runs")
         dev = pred_scores.device
-        if dev.type != "cuda":
-            raise RuntimeError("yolov6_b200.ComputeLoss runs on CUDA tensors only (no CPU fallback)")
         anchors, anchor_points, n_list, stride_t = self._get_anchors(sizes, dev)
         B, A, nc = pred_scores.shape
-        R = pred_distri.shape[2]
-        lib, h, sp = _lib.lib(), _lib.handle(dev.index or 0), _lib.stream_ptr()
-        ps = pred_scores.detach().float().contiguous()
-        pd = pred_distri.detach().float().contiguous()
+        ps, pd = (t.detach().float().contiguous() for t in (pred_scores, pred_distri))
         strides = stride_t.reshape(-1).contiguous()
         if reuse is not None:       # second box branch against the first call's padded targets and assignment
-            gt, gt_count, G, c, mask = reuse["gt"], reuse["gt_count"], reuse["G"], reuse["assignment"], reuse["mask"]
-            tg = pboxes = None
+            st, tg, pboxes = {k: reuse[k] for k in ("gt", "gt_count", "G", "mask", "assignment")}, None, None
         else:
-            n = targets.shape[0]
-            if max_gt is not None:
-                G = max(int(max_gt), 1)
-            elif n == 0:
-                G = 1
-            else:   # loss.py:184-192 pads to the largest per-image count
-                img = targets[:, 0].detach()
-                valid = img[(img >= 0) & (img < B)].long()
-                G = max(int(torch.bincount(valid, minlength=1).max()), 1) if valid.numel() else 1
-            tg = targets.detach().float().contiguous().to(dev)
-            gt = torch.empty(B, G, 5, dtype=torch.float64, device=dev)
-            gt_count = torch.empty(B, dtype=torch.int32, device=dev)
-            _lib.check(lib.yv6_targets_pad(h, _p(tg), n, B, G, float(batch_width), float(batch_height), _p(gt), _p(gt_count), sp))
-            mask = (gt[:, :, 1:].sum(-1) > 0).to(torch.uint8).contiguous()          # loss.py:79
-            # predicted boxes in pixels for the assigner (loss.py:82-83, 94/100)
-            pboxes = torch.empty(B, A, 4, dtype=torch.float32, device=dev)
-            _lib.check(lib.yv6_box_decode(h, _p(pd), _p(anchor_points), _p(strides), B, A, R, 1, _p(pboxes), sp))
+            st, tg = self._pad_targets(targets, B, max_gt, batch_height, batch_width, dev)
+            pboxes = torch.empty(B, A, 4, dtype=torch.float32, device=dev)      # in pixels, for the assigner (loss.py:82-83, 94/100)
+            _lib.check(_lib.lib().yv6_box_decode(_lib.handle(dev.index or 0), _p(pd), _p(anchor_points), _p(strides), B, A,
+                                                 pd.shape[2], 1, _p(pboxes), _lib.stream_ptr()))
             if epoch_num < self.warmup_epoch:
-                c = atss_compact(anchors, n_list, gt, mask, pboxes, nc, 9)
+                c = atss_compact(anchors, n_list, st["gt"], st["mask"], pboxes, nc, 9)
             else:
-                c = tal_compact(ps, pboxes, anchor_points, gt, mask, 13, 1.0, 6.0)
-            self.last_assignment = c
-        d = _lib.LossDesc()
-        if grad_scores is None:
-            grad_scores = torch.empty_like(ps)
-        if grad_distri is None:
-            grad_distri = torch.empty_like(pd)
+                c = tal_compact(ps, pboxes, anchor_points, st["gt"], st["mask"], 13, 1.0, 6.0)
+            st["assignment"] = self.last_assignment = c
+        ws = self._det_loss(st, ps, pd, anchor_points, strides, grad_scores, grad_distri, grad_scale, weights)
+        st["keep"] = (ps, pd, st["gt"], st["mask"], pboxes, ws, tg)
+        return st
+
+    def _pad_targets(self, targets, B, max_gt, batch_height, batch_width, dev):
+        """yv6_targets_pad of the [n, 6] (image, class, cx, cy, w, h) rows into a state {"gt": [B, G, 5] float64 (class, xyxy
+        in pixels), "gt_count", "G", "mask": uint8 [B, G] of the real rows (loss.py:79)}; also returns the float32 rows read."""
+        n = targets.shape[0]
+        if max_gt is not None:
+            G = max(int(max_gt), 1)
+        elif n == 0:
+            G = 1
+        else:   # loss.py:184-192 pads to the largest per-image count
+            img = targets[:, 0].detach()
+            valid = img[(img >= 0) & (img < B)].long()
+            G = max(int(torch.bincount(valid, minlength=1).max()), 1) if valid.numel() else 1
+        tg = targets.detach().float().contiguous().to(dev)
+        gt = torch.empty(B, G, 5, dtype=torch.float64, device=dev)
+        gt_count = torch.empty(B, dtype=torch.int32, device=dev)
+        _lib.check(_lib.lib().yv6_targets_pad(_lib.handle(dev.index or 0), _p(tg), n, B, G, float(batch_width), float(batch_height),
+                                              _p(gt), _p(gt_count), _lib.stream_ptr()))
+        mask = (gt[:, :, 1:].sum(-1) > 0).to(torch.uint8).contiguous()
+        return {"gt": gt, "gt_count": gt_count, "G": G, "mask": mask}, tg
+
+    def _det_loss(self, st, ps, pd, anchor_points, strides, grad_scores=None, grad_distri=None, grad_scale=1.0, weights=None):
+        """yv6_det_loss of scores `ps` and box predictions `pd` (reg_ch = pd.shape[2]) against the state's targets and assignment:
+        adds "out" and the gradient buffers "grad_scores" / "grad_distri" (new unless given) to the state; returns the workspace."""
+        B, A, nc = ps.shape
+        dev, lib, c = ps.device, _lib.lib(), st["assignment"]
+        grad_scores = torch.empty_like(ps) if grad_scores is None else grad_scores
+        grad_distri = torch.empty_like(pd) if grad_distri is None else grad_distri
         out = torch.zeros(8, dtype=torch.float64, device=dev)
         ws = torch.empty(int(lib.yv6_det_loss_workspace_bytes(B, A)), dtype=torch.uint8, device=dev)
-        d.pred_scores, d.pred_distri, d.anc_points, d.strides = ps.data_ptr(), pd.data_ptr(), anchor_points.data_ptr(), strides.data_ptr()
-        d.gt, d.gt_idx, d.fg, d.norm = gt.data_ptr(), c.gt_idx.data_ptr(), c.fg.data_ptr(), c.norm.data_ptr()
-        d.B, d.A, d.G, d.nc, d.reg_ch = B, A, G, nc, R
-        d.iou_type = IOU_TYPES[self.iou_type]
-        d.w_cls, d.w_iou, d.w_dfl = float(self.loss_weight['class']), float(self.loss_weight['iou']), float(self.loss_weight['dfl'])
-        if weights is not None:
-            d.w_cls, d.w_iou, d.w_dfl = (float(v) for v in weights)
-        d.grad_scale = float(grad_scale)
-        d.grad_scores, d.grad_distri, d.out = grad_scores.data_ptr(), grad_distri.data_ptr(), out.data_ptr()
-        d.workspace, d.workspace_bytes = ws.data_ptr(), ws.numel()
-        d.norm_gt_zero = self._norm_gt_zero
-        _lib.check(lib.yv6_det_loss(h, C.byref(d), sp))
-        return {"grad_scores": grad_scores, "grad_distri": grad_distri, "out": out, "gt_count": gt_count, "G": G, "gt": gt, "mask": mask,
-                "assignment": c, "keep": (ps, pd, gt, mask, pboxes, ws, tg)}
+        w = [float(v) for v in (weights if weights is not None else [self.loss_weight[k] for k in ("class", "iou", "dfl")])]
+        d = _lib.LossDesc(pred_scores=ps.data_ptr(), pred_distri=pd.data_ptr(), anc_points=anchor_points.data_ptr(), strides=strides.data_ptr(),
+                          gt=st["gt"].data_ptr(), gt_idx=c.gt_idx.data_ptr(), fg=c.fg.data_ptr(), norm=c.norm.data_ptr(),
+                          B=B, A=A, G=st["G"], nc=nc, reg_ch=pd.shape[2], iou_type=IOU_TYPES[self.iou_type],
+                          w_cls=w[0], w_iou=w[1], w_dfl=w[2], grad_scale=float(grad_scale),
+                          grad_scores=grad_scores.data_ptr(), grad_distri=grad_distri.data_ptr(), out=out.data_ptr(),
+                          workspace=ws.data_ptr(), workspace_bytes=ws.numel(), norm_gt_zero=self._norm_gt_zero)
+        _lib.check(lib.yv6_det_loss(_lib.handle(dev.index or 0), C.byref(d), _lib.stream_ptr()))
+        st.update(out=out, grad_scores=grad_scores, grad_distri=grad_distri)
+        return ws

@@ -25,10 +25,12 @@ import torch
 
 from . import _lib
 from .assigners import _p
-from .loss import ComputeLoss as _DetLoss
+from .loss import ComputeLoss as _DetLoss, LossFn
 
 
 class ComputeLoss(_DetLoss):
+    _norm_gt_zero = 1
+
     def __init__(self, fpn_strides=[8, 16, 32], grid_cell_size=5.0, grid_cell_offset=0.5, num_classes=80, ori_img_size=640,
                  warmup_epoch=0, use_dfl=True, reg_max=16, iou_type='giou',
                  loss_weight={'class': 1.0, 'iou': 2.5, 'dfl': 0.5, 'cwd': 10.0},
@@ -37,7 +39,6 @@ class ComputeLoss(_DetLoss):
                          iou_type, loss_weight)
         self.distill_feat = bool(distill_feat)       # needs `model.return_featmaps = True` on student and teacher (real neck outputs)
         self.distill_weight = distill_weight
-        self._norm_gt_zero = 1
 
     def _cw_term(self, s_featmaps, t_featmaps, decay, terms):
         """distill_loss_cw (:223-245), temperature 1: per level KL over the H*W positions of every (image, channel) row, / (N*C).
@@ -107,29 +108,14 @@ class ComputeLoss(_DetLoss):
         sizes = [tuple(f.shape[2:]) for f in feats]
         state = self.distill_forward_backward(pred_scores, pred_distri, t_pred_scores, t_pred_distri, sizes, targets, epoch_num, max_epoch,
                                               temperature, batch_height, batch_width, s_featmaps, t_featmaps)
-        loss = _GradsFn.apply(state, [state["grad_scores"], state["grad_distri"]] + state["feat_grads"], pred_scores, pred_distri,
-                              *list(s_featmaps[:3] if self.distill_feat else []))
+        loss = LossFn.apply(state, [state["grad_scores"], state["grad_distri"]] + state["feat_grads"], pred_scores, pred_distri,
+                            *list(s_featmaps[:3] if self.distill_feat else []))
         return loss, _items(state["out"])
 
 
 def _items(out):
     """(iou, dfl_all, cls_all, cwd): the reference's loss_items."""
     return torch.cat([out[1:4], out[6:7]]).detach()
-
-
-class _GradsFn(torch.autograd.Function):
-    """Scalar loss whose gradients w.r.t. its tensor inputs were produced by the kernels already: forward returns state['out'][0],
-    backward hands out the stored gradients scaled by the incoming one."""
-
-    @staticmethod
-    def forward(ctx, state, grads, *tensors):
-        ctx.save_for_backward(*grads)
-        ctx.dtypes = [t.dtype for t in tensors]
-        return state["out"][0].clone()
-
-    @staticmethod
-    def backward(ctx, grad_out):
-        return (None, None, *[(g * grad_out).to(dt) for g, dt in zip(ctx.saved_tensors, ctx.dtypes)])
 
 
 class ComputeLossNS(ComputeLoss):
@@ -153,8 +139,7 @@ class ComputeLossNS(ComputeLoss):
         st2 = self.forward_backward(pred_scores, pred_lrtb, sizes, targets, epoch_num, batch_height, batch_width, reuse=state,
                                     grad_distri=grad_lrtb, weights=(0.0, float(self.loss_weight['iou']), 0.0))
         total = state["out"].clone()
-        total[0] = total[0] + st2["out"][0]
-        total[1] = total[1] + st2["out"][1]
+        total[:2] += st2["out"][:2]
         # (the class-score gradient of the second call is exactly zero: w_cls = 0)
         return dict(state, out=total, keep_lrtb=st2)
 
@@ -165,5 +150,5 @@ class ComputeLossNS(ComputeLoss):
         state = self.distill_forward_backward(pred_scores, pred_distri, t_outputs[-2], t_outputs[-1], sizes, targets, epoch_num, max_epoch,
                                               temperature, batch_height, batch_width, s_featmaps, t_featmaps, pred_lrtb=pred_lrtb)
         grads = [state["grad_scores"], state["grad_distri"], state["keep_lrtb"]["grad_distri"]] + state["feat_grads"]
-        loss = _GradsFn.apply(state, grads, pred_scores, pred_distri, pred_lrtb, *list(s_featmaps[:3] if self.distill_feat else []))
+        loss = LossFn.apply(state, grads, pred_scores, pred_distri, pred_lrtb, *list(s_featmaps[:3] if self.distill_feat else []))
         return loss, _items(state["out"])

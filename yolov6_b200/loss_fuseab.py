@@ -17,111 +17,57 @@ equivalent (l, t, r, b) distances around the cell centre, so that `yv6_tal_assig
 one launch) are reused unchanged; `yv6_ab_boxes_bwd` maps the gradient back.  Everything runs on the device without host
 synchronisation (except the per-image target count when `max_gt` is not given, as in loss.py).
 """
-import ctypes as C
-
 import torch
 
 from . import _lib
-from .assigners import _p, tal_compact
-from .loss import IOU_TYPES, _DetLossFn
+from .assigners import _p, generate_anchors_train, tal_compact
+from .loss import ComputeLoss as _DetLoss
 
 AB_TOPK = 26        # loss_fuseab.py:40
 
 
 def generate_anchors_ab(sizes, strides, device, grid_cell_offset=0.5, num_anchors=3):
-    """anchor_generator.py:36-63 with mode='ab': cell centres in pixels and strides, each level's block repeated
+    """anchor_generator.py:36-63 with mode='ab': the train-mode cell centres in pixels and strides, each level's block repeated
     `num_anchors` times ((anchor, pixel) order inside a level)."""
-    pts, strs = [], []
-    for (h, w), s in zip(sizes, strides):
-        sx = (torch.arange(w, dtype=torch.float32, device=device) + grid_cell_offset) * s
-        sy = (torch.arange(h, dtype=torch.float32, device=device) + grid_cell_offset) * s
-        yy, xx = torch.meshgrid(sy, sx, indexing="ij")
-        pts.append(torch.stack([xx, yy], -1).reshape(-1, 2).repeat(num_anchors, 1))
-        strs.append(torch.full((h * w * num_anchors, 1), float(s), dtype=torch.float32, device=device))
-    return torch.cat(pts).contiguous(), torch.cat(strs).contiguous()
+    levels = [generate_anchors_train([hw], [s], device, 0.0, grid_cell_offset) for hw, s in zip(sizes, strides)]
+    pts = torch.cat([pt.repeat(num_anchors, 1) for _, pt, _, _ in levels])
+    strs = torch.cat([st.repeat(num_anchors, 1) for _, _, _, st in levels])
+    return pts.contiguous(), strs.contiguous()
 
 
-class ComputeLoss:
+class ComputeLoss(_DetLoss):
+    _norm_gt_zero = 1       # loss_fuseab.py:139, 203-206
+
     def __init__(self, fpn_strides=[8, 16, 32], grid_cell_size=5.0, grid_cell_offset=0.5, num_classes=80,
                  ori_img_size=640, warmup_epoch=0, use_dfl=True, reg_max=16, iou_type='giou',
-                 loss_weight={'class': 1.0, 'iou': 2.5, 'dfl': 0.5}):
-        self.fpn_strides = list(fpn_strides)
-        self.grid_cell_size, self.grid_cell_offset = grid_cell_size, grid_cell_offset
-        self.num_classes, self.ori_img_size = num_classes, ori_img_size
-        self.warmup_epoch = warmup_epoch
-        self.use_dfl, self.reg_max = use_dfl, reg_max      # the ab head predicts four values per anchor: no DFL term either way
-        self.iou_type = iou_type.lower()
-        if self.iou_type not in IOU_TYPES:
-            raise ValueError(f"unknown iou_type {iou_type}")
-        self.loss_weight = loss_weight
-        self._anchor_key, self._anchors = None, None
-        self.last_assignment = None
+                 loss_weight={'class': 1.0, 'iou': 2.5, 'dfl': 0.5}):     # use_dfl: the ab head has no DFL term either way
+        super().__init__(fpn_strides, grid_cell_size, grid_cell_offset, num_classes, ori_img_size, warmup_epoch, use_dfl, reg_max,
+                         iou_type, loss_weight)
 
-    def _get_anchors(self, sizes, device):
-        key = (tuple(sizes), str(device))
-        if key != self._anchor_key:
-            self._anchors = generate_anchors_ab(sizes, self.fpn_strides, device, self.grid_cell_offset)
-            self._anchor_key = key
-        return self._anchors
-
-    def __call__(self, outputs, targets, epoch_num, step_num, batch_height, batch_width):
-        feats, pred_scores, pred_distri = outputs
-        sizes = [tuple(f.shape[2:]) for f in feats]
-        state = self.forward_backward(pred_scores, pred_distri, sizes, targets, epoch_num, batch_height, batch_width)
-        loss = _DetLossFn.apply(pred_scores, pred_distri, state)
-        return loss, state["out"][1:4].detach().clone()
+    def _build_anchors(self, sizes, device):
+        return generate_anchors_ab(sizes, self.fpn_strides, device, self.grid_cell_offset)
 
     def forward_backward(self, pred_scores, pred_distri, sizes, targets, epoch_num, batch_height, batch_width, max_gt=None,
                          grad_scores=None, grad_distri=None, grad_scale=1.0):
         """Loss value and its gradients w.r.t. (cls_ab, reg_ab) in one pass; same contract as loss.ComputeLoss.forward_backward."""
+        _lib.require_cuda(pred_scores, "yolov6_b200.loss_fuseab.ComputeLoss runs")
         dev = pred_scores.device
-        if dev.type != "cuda":
-            raise RuntimeError("yolov6_b200.loss_fuseab.ComputeLoss runs on CUDA tensors only (no CPU fallback)")
         anchor_points, stride_t = self._get_anchors(sizes, dev)
         B, A, nc = pred_scores.shape
         if pred_distri.shape[2] != 4 or anchor_points.shape[0] != A:
             raise RuntimeError(f"fuse_ab loss: expected [B, {anchor_points.shape[0]}, 4] box predictions, got {tuple(pred_distri.shape)}")
         lib, h, sp = _lib.lib(), _lib.handle(dev.index or 0), _lib.stream_ptr()
-        ps = pred_scores.detach().float().contiguous()
-        pd = pred_distri.detach().float().contiguous()
+        ps, pd = (t.detach().float().contiguous() for t in (pred_scores, pred_distri))
         strides = stride_t.reshape(-1).contiguous()
-        n = targets.shape[0]
-        if max_gt is not None:
-            G = max(int(max_gt), 1)
-        elif n == 0:
-            G = 1
-        else:   # loss_fuseab.py:150-158 pads to the largest per-image count
-            img = targets[:, 0].detach()
-            valid = img[(img >= 0) & (img < B)].long()
-            G = max(int(torch.bincount(valid, minlength=1).max()), 1) if valid.numel() else 1
-        tg = targets.detach().float().contiguous().to(dev)
-        gt = torch.empty(B, G, 5, dtype=torch.float64, device=dev)
-        gt_count = torch.empty(B, dtype=torch.int32, device=dev)
-        _lib.check(lib.yv6_targets_pad(h, _p(tg), n, B, G, float(batch_width), float(batch_height), _p(gt), _p(gt_count), sp))
-        mask = (gt[:, :, 1:].sum(-1) > 0).to(torch.uint8).contiguous()          # loss_fuseab.py:69
+        st, tg = self._pad_targets(targets, B, max_gt, batch_height, batch_width, dev)
         ltrb = torch.empty(B, A, 4, dtype=torch.float32, device=dev)
         pboxes = torch.empty(B, A, 4, dtype=torch.float32, device=dev)
         _lib.check(lib.yv6_ab_boxes(h, _p(pd), _p(anchor_points), _p(strides), B, A, _p(ltrb), _p(pboxes), sp))
-        c = tal_compact(ps, pboxes, anchor_points, gt, mask, AB_TOPK, 1.0, 6.0)   # formal_assigner, every epoch (:78-86)
-        self.last_assignment = c
-        d = _lib.LossDesc()
-        if grad_scores is None:
-            grad_scores = torch.empty_like(ps)
-        if grad_distri is None:
-            grad_distri = torch.empty_like(pd)
+        # formal_assigner, every epoch (:78-86)
+        st["assignment"] = self.last_assignment = tal_compact(ps, pboxes, anchor_points, st["gt"], st["mask"], AB_TOPK, 1.0, 6.0)
+        grad_distri = torch.empty_like(pd) if grad_distri is None else grad_distri
         grad_ltrb = torch.empty_like(pd)
-        out = torch.zeros(8, dtype=torch.float64, device=dev)
-        ws = torch.empty(int(lib.yv6_det_loss_workspace_bytes(B, A)), dtype=torch.uint8, device=dev)
-        d.pred_scores, d.pred_distri, d.anc_points, d.strides = ps.data_ptr(), ltrb.data_ptr(), anchor_points.data_ptr(), strides.data_ptr()
-        d.gt, d.gt_idx, d.fg, d.norm = gt.data_ptr(), c.gt_idx.data_ptr(), c.fg.data_ptr(), c.norm.data_ptr()
-        d.B, d.A, d.G, d.nc, d.reg_ch = B, A, G, nc, 4
-        d.iou_type = IOU_TYPES[self.iou_type]
-        d.w_cls, d.w_iou, d.w_dfl = float(self.loss_weight['class']), float(self.loss_weight['iou']), float(self.loss_weight['dfl'])
-        d.grad_scale = float(grad_scale)
-        d.grad_scores, d.grad_distri, d.out = grad_scores.data_ptr(), grad_ltrb.data_ptr(), out.data_ptr()
-        d.workspace, d.workspace_bytes = ws.data_ptr(), ws.numel()
-        d.norm_gt_zero = 1                                                       # loss_fuseab.py:139, 203-206
-        _lib.check(lib.yv6_det_loss(h, C.byref(d), sp))
+        ws = self._det_loss(st, ps, ltrb, anchor_points, strides, grad_scores, grad_ltrb, grad_scale)
         _lib.check(lib.yv6_ab_boxes_bwd(h, _p(grad_ltrb), B * A, _p(grad_distri), sp))
-        return {"grad_scores": grad_scores, "grad_distri": grad_distri, "out": out, "gt_count": gt_count, "G": G,
-                "keep": (ps, pd, gt, mask, pboxes, ltrb, grad_ltrb, ws, tg)}
+        st["grad_distri"], st["keep"] = grad_distri, (ps, pd, st["gt"], st["mask"], pboxes, ltrb, grad_ltrb, ws, tg)
+        return st
