@@ -58,8 +58,9 @@ def host_planner():
 
 
 def dry_engine(case):
-    """An InferEngine over a CPU model with seeded weights whose library, handle and streams are the recorder's stand-ins."""
-    c = CASES[case]
+    """An InferEngine over a CPU model with seeded weights whose library, handle and streams are the recorder's stand-ins.
+    `case` names one of CASES or is a dict of the same form (tests/test_serving_plan.py)."""
+    c = CASES[case] if isinstance(case, str) else case
     cfg = configs.get_config(c["cfg"])
     if c.get("distill_ns"):       # the N / S distillation student needs the DFL head
         cfg["head"]["use_dfl"], cfg["head"]["reg_max"] = True, 16

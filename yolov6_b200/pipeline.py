@@ -24,154 +24,211 @@ locations.
 Device frames are read in stream order: the copy stream waits for the work enqueued on the caller's current stream before
 the call, so frames a kernel wrote there are complete when the graph reads them.  They are read in place, so the caller
 must not write to them until `collect()` has returned their batch (`DetectPipeline.__call__` returns after the batch is
-done); the pipeline keeps a reference to them until then, so dropping them early is safe.
+done); the pipeline keeps a reference to them at least until then, so dropping them early is safe.
+
+Each batch in flight lives in a `BatchSlot` (its input and staging buffers, pinned results and events): `DetectPipeline`
+holds one, `DetectStream` two, used by alternate steps.
 """
+import functools
+import os
+
 import torch
 
 from .nms import nms_batched_head, workspace_bytes
-from .preprocess import GEO, REC, check_frames, letterbox_frames_launch, pack_sources, rescale_launch
+from .preprocess import REC, check_frames, letterbox_frames_launch, pack_sources, rescale_launch
 
 RAW_DEFAULT_BYTES = 1920 * 1080 * 3        # staging bytes per batch slot when max_src_bytes is not given: one 1080p frame each
+OVERFLOW = "non_max_suppression: more than 65536 near-identical candidate scores in one image; raise conf_thres"
 
 
-def raw_buffers(batch, height, width, max_det, max_src_bytes, dev):
-    """Pinned staging + device buffers of one raw-frame slot."""
-    cap = int(max_src_bytes) if max_src_bytes else batch * RAW_DEFAULT_BYTES
-    geo = torch.tensor([[0, height, width, 0, 0, 0, 0, 0]] * batch, dtype=torch.int32)     # all border until frames arrive
-    rec = torch.zeros(batch * REC, dtype=torch.uint8)          # null records: an all-border slot reads no source
-    return dict(src_host=torch.empty(cap, dtype=torch.uint8).pin_memory(), geo_host=geo.pin_memory(), rec_host=rec.pin_memory(),
-                src_dev=torch.zeros(cap, dtype=torch.uint8, device=dev), geo_dev=geo.to(dev), rec_dev=rec.to(dev), res_geo=geo.to(dev),
-                res=torch.zeros(batch, max_det, 6, device=dev), nbytes=0, frames=[])
+class BatchSlot:
+    """The buffers and events of one batch in flight: the device input with its pinned host input or, for raw frames, the
+    staging buffer, record and geometry tables; the pinned results; `ev_copied` (its H2D is complete) and `ev_done` (the
+    step that read it is complete).  `hold_geo`: the letterbox keeps a copy of the geometry (`res_geo`) for a rescale that
+    runs after the copy stream may already have refilled `geo_dev` with the next batch's."""
 
-
-def raw_pack(slot, frames, height, width, layout, dev):
-    """Validate 1..B frames and lay them out in one raw-frame slot's host tables; RuntimeError before anything is written
-    when a frame is unusable.  Returns the device frames (read in place by the slot's next launch)."""
-    srcs = check_frames(frames, slot["geo_host"].shape[0], layout, dev)
-    slot["nbytes"], _, devs = pack_sources(srcs, slot["geo_host"].shape[0], height, width, True, layout, slot["src_host"],
-                                           slot["geo_host"], slot["rec_host"], slot["src_dev"].data_ptr())
-    return devs
-
-
-def raw_h2d(slot):
-    """Copy the used staging bytes, the source records and the geometry of one raw-frame slot to the device (current stream)."""
-    n = slot["nbytes"]
-    if n:
-        slot["src_dev"][:n].copy_(slot["src_host"][:n], non_blocking=True)
-    slot["rec_dev"].copy_(slot["rec_host"], non_blocking=True)
-    slot["geo_dev"].copy_(slot["geo_host"], non_blocking=True)
-
-
-class DetectPipeline:
-    def __init__(self, model, batch, height, width, conf_thres=0.25, iou_thres=0.45, classes=None, agnostic=False,
-                 multi_label=False, max_det=300, host_input=True, overlap_h2d=False, copy_stream=None, raw_input=False,
-                 max_src_bytes=None):
-        self.model = model.eval()
-        self.dev = next(model.parameters()).device
-        if self.dev.type != "cuda":
-            raise RuntimeError("DetectPipeline needs a CUDA model")
-        if raw_input and not host_input:
-            raise RuntimeError("DetectPipeline: raw_input returns detections in host memory (host_input=True)")
-        self.kw = dict(conf_thres=conf_thres, iou_thres=iou_thres, classes=classes, agnostic=agnostic,
-                       multi_label=multi_label, max_det=max_det)
-        self.host_input = host_input
-        self.raw = raw_input and raw_buffers(batch, height, width, max_det, max_src_bytes, self.dev)
-        self.n_frames = batch
-        self.overlap_h2d = bool((overlap_h2d or raw_input) and host_input)
-        if self.overlap_h2d:
-            self.copy_stream = copy_stream or torch.cuda.Stream(device=self.dev)
-            self.ev_copied = torch.cuda.Event()
-            self.ev_done = torch.cuda.Event()
-            self.ev_ready = torch.cuda.Event()
-            self._ready = None       # event the next copy waits for: the caller's stream when device frames were given
-            self._used = False
-        dt = torch.uint8 if host_input else torch.float32
-        self.x_dev = torch.zeros(batch, 3, height, width, dtype=dt, device=self.dev)
-        self.x_host = torch.zeros(batch, 3, height, width, dtype=torch.uint8).pin_memory() if host_input and not self.raw else None
+    def __init__(self, batch, height, width, max_det, host_input, raw_input, max_src_bytes, dev, hold_geo=False):
+        self.dev, self.host_input, self.raw, self.hold_geo = dev, host_input, raw_input, hold_geo
+        self.x_dev = torch.zeros(batch, 3, height, width, dtype=torch.uint8 if host_input else torch.float32, device=dev)
+        self.x_host = torch.zeros(batch, 3, height, width, dtype=torch.uint8).pin_memory() if host_input and not raw_input else None
+        if raw_input:
+            cap = int(max_src_bytes) if max_src_bytes else batch * RAW_DEFAULT_BYTES
+            geo = torch.tensor([[0, height, width, 0, 0, 0, 0, 0]] * batch, dtype=torch.int32)    # all border until frames arrive
+            rec = torch.zeros(batch * REC, dtype=torch.uint8)          # null records: an all-border slot reads no source
+            self.src_host = torch.empty(cap, dtype=torch.uint8).pin_memory()
+            self.geo_host, self.rec_host = geo.pin_memory(), rec.pin_memory()
+            self.src_dev, self.geo_dev, self.rec_dev = torch.zeros(cap, dtype=torch.uint8, device=dev), geo.to(dev), rec.to(dev)
+            self.res_geo = geo.to(dev) if hold_geo else self.geo_dev
+            self.res = torch.zeros(batch, max_det, 6, device=dev)
+            self.nbytes, self.frames = 0, []          # staged host bytes; device frames, read in place by the next launch
         self.out_host = torch.zeros(batch, max_det, 6).pin_memory()
-        self.count_host = torch.zeros(batch + 1, dtype=torch.int32).pin_memory()
-        self.eng = model.engine()
-        self.eng.pin(batch, height, width, dt)          # the graph points at this shape's buffers
-        A = sum((height // int(s)) * (width // int(s)) for s in model.graph.strides)
-        nc = model.graph.num_classes
-        # scratch owned by this pipeline: a shared cache could be replaced (freed) while the graph still references it
-        self.nms_ws = torch.empty(workspace_bytes(batch, A, nc, multi_label), dtype=torch.uint8, device=self.dev)
-        self.graph = None
-        self._warm()
+        self.count_host = torch.zeros(batch + 1, dtype=torch.int32).pin_memory()      # per-image counts, then the overflow flag
+        self.ev_copied, self.ev_done, self.ev_ready = torch.cuda.Event(), torch.cuda.Event(), torch.cuda.Event()
+        self.ready = None          # event the next H2D waits for: the producer of the staged device frames
+        self.used = False          # ev_done has been recorded
 
-    def _body(self):
+    def stage(self, images, layout="bgr_hwc", ready=None):
+        """Put the next batch into the slot: an image batch into x_host (host input) or x_dev, or 1..B raw frames into the
+        staging tables (RuntimeError before anything is written when a frame is unusable).  The H2D of device frames waits
+        for `ready`, by default an event recorded now on the current stream."""
+        if not self.raw:
+            (self.x_host if self.host_input else self.x_dev).copy_(images)
+            return
+        srcs = check_frames(images, self.geo_host.shape[0], layout, self.dev)
+        self.nbytes, _, self.frames = pack_sources(srcs, self.geo_host.shape[0], self.x_dev.shape[2], self.x_dev.shape[3], True,
+                                                   layout, self.src_host, self.geo_host, self.rec_host, self.src_dev.data_ptr())
+        # only device frames need it: the caller's stream usually holds the previous step, and a copy that waited for it
+        # would no longer overlap that step
+        if self.frames:
+            if ready is None:
+                ready = self.ev_ready
+                ready.record(torch.cuda.current_stream(self.dev))
+            self.ready = ready
+
+    def h2d(self, copy_stream, cur):
+        """Copy the staged input to the device on `copy_stream`, after the slot's previous step and the producer of its
+        device frames; `cur` waits for the copy."""
+        if self.used:
+            copy_stream.wait_event(self.ev_done)           # the previous step of this slot is done with x_dev
+        if self.ready is not None:
+            copy_stream.wait_event(self.ready)
+            self.ready = None
+        with torch.cuda.stream(copy_stream):
+            if not self.raw:
+                self.x_dev.copy_(self.x_host, non_blocking=True)
+            else:
+                if self.nbytes:
+                    self.src_dev[:self.nbytes].copy_(self.src_host[:self.nbytes], non_blocking=True)
+                self.rec_dev.copy_(self.rec_host, non_blocking=True)
+                self.geo_dev.copy_(self.geo_host, non_blocking=True)
+            self.ev_copied.record(copy_stream)
+        cur.wait_event(self.ev_copied)
+
+    def done(self, stream):
+        self.ev_done.record(stream)
+        self.used = True
+
+    def letterbox(self):
+        """Raw frames -> x_dev (nothing to do for letterboxed input)."""
         if self.raw:
-            letterbox_frames_launch(self.raw["rec_dev"], self.raw["geo_dev"], self.x_dev)
-        elif self.host_input and not self.overlap_h2d:
-            self.x_dev.copy_(self.x_host, non_blocking=True)
-        # the [B, A, 5+nc] prediction tensor of Detect.forward (effidehead.py:131-139) is never materialised here: the NMS
-        # kernels scan the class scores where the cls_pred convs wrote them and decode boxes for the candidates only
-        cls, reg, sizes = self.eng.forward(self.x_dev, decode=False)
-        out, count, src, overflow = nms_batched_head(cls, reg, sizes, self.model.graph.strides, workspace=self.nms_ws, **self.kw)
+            letterbox_frames_launch(self.rec_dev, self.geo_dev, self.x_dev)
+            if self.hold_geo:
+                self.res_geo.copy_(self.geo_dev)
+
+    def detect(self, nms, cls, reg):
+        """NMS over the head tensors, rescaled to source pixels (raw frames) and copied to the pinned results (host input).
+        Returns the device results (out, count, overflow)."""
+        out, count, _, overflow = nms(cls, reg)
         if self.raw:
-            out = rescale_launch(out, count, self.raw["geo_dev"], self.x_dev.shape[2], self.x_dev.shape[3], res=self.raw["res"])
-        self.out_dev, self.count_dev = out, count
+            out = rescale_launch(out, count, self.res_geo, self.x_dev.shape[2], self.x_dev.shape[3], res=self.res)
         if self.host_input:
             self.out_host.copy_(out, non_blocking=True)
             self.count_host[:-1].copy_(count, non_blocking=True)
             self.count_host[-1:].copy_(overflow, non_blocking=True)
+        return out, count, overflow
 
-    def _warm(self):
+    def rows(self, n, dev=None):
+        """The per-image [k, 6] detections of the first n images of the slot's finished batch, from the pinned results or,
+        when given, from the device results `dev` = (out, count, overflow)."""
+        if dev is None:
+            out, counts = self.out_host, self.count_host.tolist()
+            if counts[-1]:
+                raise RuntimeError(OVERFLOW)
+        else:
+            out, count, overflow = dev
+            if overflow.item():
+                raise RuntimeError(OVERFLOW)
+            counts = count.tolist()
+        return [out[j, :counts[j]].clone() for j in range(n)]
+
+
+class _Served:
+    """What DetectPipeline and DetectStream share: the checks, NMS settings, pinned engine shape, NMS workspace and batch
+    slots, and the warm-up-then-capture of their graphs."""
+
+    def __init__(self, model, batch, height, width, nms_kw, host_input, raw_input, max_src_bytes, slots, engine=None):
+        self.model = model.eval()
+        self.dev = next(model.parameters()).device
+        if self.dev.type != "cuda":
+            raise RuntimeError(f"{type(self).__name__} needs a CUDA model")
+        if raw_input and not host_input:
+            raise RuntimeError(f"{type(self).__name__}: raw_input returns detections in host memory (host_input=True)")
+        self.host_input = bool(host_input)
+        self.slots = [BatchSlot(batch, height, width, nms_kw["max_det"], self.host_input, raw_input, max_src_bytes, self.dev,
+                                hold_geo=slots > 1) for _ in range(slots)]
+        self.shape = (batch, height, width, self.slots[0].x_dev.dtype)
+        self.eng = engine if engine is not None else model.engine()
+        self.eng.pin(*self.shape)          # the graphs point at this shape's buffers
+        self.sizes = [(height // int(s), width // int(s)) for s in model.graph.strides]
+        A = sum(h * w for h, w in self.sizes)
+        # scratch owned by this pipeline: a shared cache could be replaced (freed) while a graph still references it
+        self.nms_ws = torch.empty(workspace_bytes(batch, A, model.graph.num_classes, nms_kw["multi_label"]), dtype=torch.uint8,
+                                  device=self.dev)
+        self.nms = functools.partial(nms_batched_head, sizes=self.sizes, strides=model.graph.strides, workspace=self.nms_ws, **nms_kw)
+
+    def _capture(self, warm, bodies):
+        """Run `warm` on a side stream (plans, tensor maps, cudaFuncSetAttribute, allocator warm-up), then capture one graph
+        per body."""
         s = torch.cuda.Stream(device=self.dev)
         s.wait_stream(torch.cuda.current_stream(self.dev))
         with torch.cuda.stream(s), torch.no_grad():
-            for _ in range(2):     # plans, tensor maps, cudaFuncSetAttribute, allocator warm-up
-                self._body()
+            warm()
         torch.cuda.current_stream(self.dev).wait_stream(s)
         torch.cuda.synchronize(self.dev)
-        self.graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(self.graph), torch.no_grad():
-            self._body()
+        graphs = []
+        for body in bodies:
+            graphs.append(torch.cuda.CUDAGraph())
+            with torch.cuda.graph(graphs[-1]), torch.no_grad():
+                body()
+        return graphs
+
+
+class DetectPipeline(_Served):
+    def __init__(self, model, batch, height, width, conf_thres=0.25, iou_thres=0.45, classes=None, agnostic=False,
+                 multi_label=False, max_det=300, host_input=True, overlap_h2d=False, copy_stream=None, raw_input=False,
+                 max_src_bytes=None):
+        super().__init__(model, batch, height, width, dict(conf_thres=conf_thres, iou_thres=iou_thres, classes=classes,
+                         agnostic=agnostic, multi_label=multi_label, max_det=max_det), host_input, raw_input, max_src_bytes, 1)
+        self.slot = self.slots[0]
+        self.x_dev, self.x_host = self.slot.x_dev, self.slot.x_host
+        self.n_frames = batch
+        self.overlap_h2d = bool((overlap_h2d or raw_input) and host_input)
+        if self.overlap_h2d:
+            self.copy_stream = copy_stream or torch.cuda.Stream(device=self.dev)
+        self.graph, = self._capture(lambda: (self._body(), self._body()), [self._body])
+
+    def _body(self):
+        self.slot.letterbox()
+        if self.host_input and not self.overlap_h2d:
+            self.x_dev.copy_(self.x_host, non_blocking=True)
+        # the [B, A, 5+nc] prediction tensor of Detect.forward (effidehead.py:131-139) is never materialised here: the NMS
+        # kernels scan the class scores where the cls_pred convs wrote them and decode boxes for the candidates only
+        cls, reg, _ = self.eng.forward(self.x_dev, decode=False)
+        self.out_dev, self.count_dev, _ = self.slot.detect(self.nms, cls, reg)
 
     def launch(self):
         """Enqueue one batch (input already in `x_host` / `x_dev`); asynchronous."""
-        if self.overlap_h2d:
-            cur = torch.cuda.current_stream(self.dev)
-            if self._used:
-                self.copy_stream.wait_event(self.ev_done)      # the previous batch of THIS pipeline is done with x_dev
-            if self._ready is not None:
-                self.copy_stream.wait_event(self._ready)       # the producer of the device frames
-                self._ready = None
-            with torch.cuda.stream(self.copy_stream):
-                if self.raw:
-                    raw_h2d(self.raw)
-                else:
-                    self.x_dev.copy_(self.x_host, non_blocking=True)
-                self.ev_copied.record(self.copy_stream)
-            cur.wait_event(self.ev_copied)
+        if not self.overlap_h2d:
             self.graph.replay()
-            self.ev_done.record(cur)
-            self._used = True
             return
+        cur = torch.cuda.current_stream(self.dev)
+        self.slot.h2d(self.copy_stream, cur)
         self.graph.replay()
+        self.slot.done(cur)
 
     def __call__(self, images=None, layout="bgr_hwc"):
         """images: uint8 [B,3,H,W] host tensor (host_input) or fp32 device tensor; with raw_input, a list of 1..B uint8 frames
         in `layout` (see the module docstring), each a numpy array, a CPU tensor or a CUDA tensor on the pipeline's device.
         Returns the list of per-image [k,6] detections (host tensors when host_input) like `non_max_suppression`; with
         raw_input in source pixels, rounded (Inferer.rescale(...).round())."""
-        devs = None          # device frames of this batch, referenced until the batch is done
         if images is not None:
-            if self.raw:
-                devs = raw_pack(self.raw, images, self.x_dev.shape[2], self.x_dev.shape[3], layout, self.dev)
-                if devs:
-                    self.ev_ready.record(torch.cuda.current_stream(self.dev))
-                    self._ready = self.ev_ready
+            self.slot.stage(images, layout)
+            if self.slot.raw:
                 self.n_frames = len(images)
-            else:
-                (self.x_host if self.host_input else self.x_dev).copy_(images)
         self.launch()
         torch.cuda.current_stream(self.dev).synchronize()
         if self.host_input:
-            counts = self.count_host.tolist()
-            if counts[-1]:
-                raise RuntimeError("non_max_suppression: more than 65536 near-identical candidate scores in one image; raise conf_thres")
-            return [self.out_host[i, :counts[i]].clone() for i in range(self.n_frames)]
+            return self.slot.rows(self.n_frames)
         counts = self.count_dev.tolist()
         return [self.out_dev[i, :counts[i]] for i in range(self.out_dev.shape[0])]
 
@@ -202,15 +259,11 @@ class DetectRing:
         assert self.tail < self.head, "nothing in flight"
         i = self.tail % len(self.pipes)
         self.done[i].synchronize()
-        p = self.pipes[i]
-        counts = p.count_host.tolist()
         self.tail += 1
-        if counts[-1]:
-            raise RuntimeError("non_max_suppression: more than 65536 near-identical candidate scores in one image; raise conf_thres")
-        return [p.out_host[j, :counts[j]].clone() for j in range(p.out_host.shape[0])]
+        return self.pipes[i].slot.rows(self.pipes[i].n_frames)
 
 
-class DetectStream:
+class DetectStream(_Served):
     """Software-pipelined serving loop: ONE graph launch per batch in which the network of batch i and the NMS of batch
     i - 1 are parallel branches.
 
@@ -233,60 +286,33 @@ class DetectStream:
 
     def __init__(self, model, batch, height, width, conf_thres=0.25, iou_thres=0.45, classes=None, agnostic=False,
                  multi_label=False, max_det=300, host_input=True, engine=None, raw_input=False, max_src_bytes=None):
-        self.model = model.eval()
-        self.dev = next(model.parameters()).device
-        if self.dev.type != "cuda":
-            raise RuntimeError("DetectStream needs a CUDA model")
-        if raw_input and not host_input:
-            raise RuntimeError("DetectStream: raw_input returns detections in host memory (host_input=True)")
-        self.kw = dict(conf_thres=conf_thres, iou_thres=iou_thres, classes=classes, agnostic=agnostic,
-                       multi_label=multi_label, max_det=max_det)
-        self.host_input = bool(host_input)
+        super().__init__(model, batch, height, width, dict(conf_thres=conf_thres, iou_thres=iou_thres, classes=classes,
+                         agnostic=agnostic, multi_label=multi_label, max_det=max_det), host_input, raw_input, max_src_bytes, 2,
+                         engine)
         self.B = batch
-        dt = torch.uint8 if host_input else torch.float32
-        self.x_dev = [torch.zeros(batch, 3, height, width, dtype=dt, device=self.dev) for _ in range(2)]
-        self.raw = [raw_buffers(batch, height, width, max_det, max_src_bytes, self.dev) for _ in range(2)] if raw_input else None
+        self.x_dev = [s.x_dev for s in self.slots]
+        self.x_host = [s.x_host for s in self.slots] if self.slots[0].x_host is not None else None
         self.n_frames = {}        # batch number -> frames in it (raw_input)
-        self.x_host = ([torch.zeros(batch, 3, height, width, dtype=torch.uint8).pin_memory() for _ in range(2)]
-                       if host_input and not raw_input else None)
-        self.out_host = [torch.zeros(batch, max_det, 6).pin_memory() for _ in range(2)]
-        self.count_host = [torch.zeros(batch + 1, dtype=torch.int32).pin_memory() for _ in range(2)]
         self.dev_step, self.dev_drain = {}, {}      # head set -> (out, count, overflow) device tensors of the step / drain graphs
-        import os
         self.fork_at_neck = os.environ.get("YV6_NMS_FORK", "neck") == "neck"
         self._drained = False
-        self.eng = engine if engine is not None else model.engine()
-        self.eng.pin(batch, height, width, dt)
-        self.shape = (batch, height, width, dt)
-        self.sizes = [(height // int(s), width // int(s)) for s in model.graph.strides]
-        A = sum(h * w for h, w in self.sizes)
-        self.nms_ws = torch.empty(workspace_bytes(batch, A, model.graph.num_classes, multi_label), dtype=torch.uint8, device=self.dev)
         self.side = torch.cuda.Stream(device=self.dev)
         self.copy_stream = torch.cuda.Stream(device=self.dev)
         self.ev_fork, self.ev_join = torch.cuda.Event(), torch.cuda.Event()
-        self.ev_copied = [torch.cuda.Event(), torch.cuda.Event()]
-        self.ev_done = [torch.cuda.Event(), torch.cuda.Event()]
-        self.ev_ready = torch.cuda.Event()
-        self._ready = None        # event the next copy waits for: the producer of the submitted device frames
         self.steps = 0            # submitted batches
         self.collected = 0
-        self.graphs = [None, None]
-        self.drain_graphs = [None, None]
-        self._build()
+
+        def warm():
+            for k in (0, 1, 0, 1):     # both head sets exist and hold valid scores before anything is captured
+                self.slots[k].letterbox()
+                self.eng.forward(self.x_dev[k], decode=False, head_set=k)
+                self._nms(k, {})
+        g = self._capture(warm, [f for k in (0, 1) for f in (lambda k=k: self._body(k), lambda k=k: self._nms(k, self.dev_drain))])
+        self.graphs, self.drain_graphs = g[0::2], g[1::2]
 
     def _nms(self, k, store):
         """NMS over head set k -> result slot k (pinned host when host_input; the device tensors go to `store[k]`)."""
-        cls, reg = self.eng.head_outputs(*self.shape, head_set=k)
-        out, count, src, overflow = nms_batched_head(cls, reg, self.sizes, self.model.graph.strides, workspace=self.nms_ws, **self.kw)
-        if self.raw:
-            # res_geo[k] is the geometry of the batch whose network wrote head set k: the copy stream may already be refilling
-            # geo_dev[k] with the batch after next
-            out = rescale_launch(out, count, self.raw[k]["res_geo"], self.x_dev[k].shape[2], self.x_dev[k].shape[3], res=self.raw[k]["res"])
-        store[k] = (out, count, overflow)
-        if self.host_input:
-            self.out_host[k].copy_(out, non_blocking=True)
-            self.count_host[k][:-1].copy_(count, non_blocking=True)
-            self.count_host[k][-1:].copy_(overflow, non_blocking=True)
+        store[k] = self.slots[k].detect(self.nms, *self.eng.head_outputs(*self.shape, head_set=k))
 
     def _body(self, k):
         cur = torch.cuda.current_stream(self.dev)
@@ -302,52 +328,18 @@ class DetectStream:
         # idle, whereas next to the backbone's persistent one-CTA-per-SM kernels the one-CTA-per-image NMS kernels just take SMs away
         # (forking at the start of the step gains 2 %, measured).
         at = self.eng.neck_start(*self.shape) if self.fork_at_neck else 0
-        self._letterbox(k)
+        self.slots[k].letterbox()
         self.eng.forward(self.x_dev[k], decode=False, head_set=k, hook=(at, fork))
         cur.wait_event(self.ev_join)
 
-    def _letterbox(self, k):
-        if self.raw:
-            letterbox_frames_launch(self.raw[k]["rec_dev"], self.raw[k]["geo_dev"], self.x_dev[k])
-            self.raw[k]["res_geo"].copy_(self.raw[k]["geo_dev"])
-
-    def _build(self):
-        s = torch.cuda.Stream(device=self.dev)
-        s.wait_stream(torch.cuda.current_stream(self.dev))
-        with torch.cuda.stream(s), torch.no_grad():
-            for k in (0, 1, 0, 1):     # both head sets exist and hold valid scores before anything is captured
-                self._letterbox(k)
-                self.eng.forward(self.x_dev[k], decode=False, head_set=k)
-                self._nms(k, {})
-        torch.cuda.current_stream(self.dev).wait_stream(s)
-        torch.cuda.synchronize(self.dev)
-        for k in (0, 1):
-            self.graphs[k] = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(self.graphs[k]), torch.no_grad():
-                self._body(k)
-            self.drain_graphs[k] = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(self.drain_graphs[k]), torch.no_grad():
-                self._nms(k, self.dev_drain)
-
     def launch(self):
         """Enqueue one step on the current stream (input of slot steps & 1 already in x_host / x_dev); asynchronous."""
-        k = self.steps & 1
+        slot = self.slots[self.steps & 1]
         cur = torch.cuda.current_stream(self.dev)
         if self.host_input:
-            if self.steps >= 2:
-                self.copy_stream.wait_event(self.ev_done[k])   # the step that last read x_dev[k] has finished
-            if self._ready is not None:
-                self.copy_stream.wait_event(self._ready)
-                self._ready = None
-            with torch.cuda.stream(self.copy_stream):
-                if self.raw:
-                    raw_h2d(self.raw[k])
-                else:
-                    self.x_dev[k].copy_(self.x_host[k], non_blocking=True)
-                self.ev_copied[k].record(self.copy_stream)
-            cur.wait_event(self.ev_copied[k])
-        self.graphs[k].replay()
-        self.ev_done[k].record(cur)
+            slot.h2d(self.copy_stream, cur)
+        self.graphs[self.steps & 1].replay()
+        slot.done(cur)
         self.steps += 1
 
     def submit(self, images, layout="bgr_hwc", ready=None):
@@ -356,40 +348,14 @@ class DetectStream:
         the work enqueued before this call on the current stream, or after the event `ready` when one is given."""
         if self.steps - self.collected > 2:
             raise RuntimeError("DetectStream: collect() the oldest batch before submitting another (result slots would be overwritten)")
-        k = self.steps & 1
-        if self.host_input:
-            if self.steps >= 2:
-                self.ev_done[k].synchronize()                  # x_host[k] was copied by the step two submissions ago
-            if self.raw:
-                devs = raw_pack(self.raw[k], images, self.x_dev[k].shape[2], self.x_dev[k].shape[3], layout, self.dev)
-                # the step that read the slot's previous device frames is complete (ev_done[k] above): release them now
-                self.raw[k]["frames"] = devs
-                # only device frames need it: the caller's stream usually holds the previous step, and a copy that waited for
-                # it would no longer overlap that step
-                if devs:
-                    if ready is None:
-                        ready = self.ev_ready
-                        ready.record(torch.cuda.current_stream(self.dev))
-                    self._ready = ready
-                self.n_frames[self.steps] = len(images)
-            else:
-                self.x_host[k].copy_(images)
-        else:
-            self.x_dev[k].copy_(images)
+        slot = self.slots[self.steps & 1]
+        if self.host_input and slot.used:
+            slot.ev_done.synchronize()          # the step two submissions ago has copied x_host and read the frames
+        slot.stage(images, layout, ready)
+        if slot.raw:
+            self.n_frames[self.steps] = len(images)
         self._drained = False
         self.launch()
-
-    def _results(self, k, store, n):
-        if self.host_input:
-            counts = self.count_host[k].tolist()
-            if counts[-1]:
-                raise RuntimeError("non_max_suppression: more than 65536 near-identical candidate scores in one image; raise conf_thres")
-            return [self.out_host[k][j, :counts[j]].clone() for j in range(n)]
-        out, count, overflow = store[k]
-        if int(overflow.item()):
-            raise RuntimeError("non_max_suppression: more than 65536 near-identical candidate scores in one image; raise conf_thres")
-        counts = count.tolist()
-        return [out[j, :counts[j]].clone() for j in range(self.B)]
 
     def collect(self):
         """Detections of the oldest uncollected batch: batch t is post-processed by step t + 1 (or by `drain()` when it is
@@ -398,7 +364,7 @@ class DetectStream:
         if t >= self.steps:
             return None
         if t + 1 < self.steps:
-            self.ev_done[(t + 1) & 1].synchronize()
+            self.slots[(t + 1) & 1].ev_done.synchronize()
             store = self.dev_step
         elif self._drained:
             torch.cuda.current_stream(self.dev).synchronize()
@@ -406,7 +372,7 @@ class DetectStream:
         else:
             return None
         self.collected += 1
-        return self._results(t & 1, store, self.n_frames.pop(t, self.B))
+        return self.slots[t & 1].rows(self.n_frames.pop(t, self.B), None if self.host_input else store[t & 1])
 
     def drain(self):
         """NMS of the last submitted batch (nothing follows it in the pipeline)."""
