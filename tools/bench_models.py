@@ -42,7 +42,9 @@ def native(name):
 
 
 def conv_gflop_per_image(g, size):
-    """2 x multiply-accumulates of every conv of graph g (inference forward, eval head) on one size x size image."""
+    """2 x multiply-accumulates of every conv of graph g (inference forward, eval head) on one size x size image (or one
+    H x W image when size is (H, W))."""
+    H, W = (size, size) if isinstance(size, int) else size
     flop = 0
     for op in g.ops:
         if op.kind in ("pool", "se", "shuffle", "up") or (op.kind == "pred" and op.head[0] not in ("cls", "reg")):
@@ -53,7 +55,7 @@ def conv_gflop_per_image(g, size):
             lvl = g.bufs[op.src.buf].level
         else:
             lvl = g.bufs[op.dst.buf].level
-        hw = (size >> lvl) ** 2
+        hw = (H >> lvl) * (W >> lvl)
         k = 2 if op.kind == "convT" else op.k        # a 2x2 stride-2 transposed conv: 4 taps per input pixel = 1 per output pixel
         flop += 2 * hw * op.cout * (1 if op.kind == "dw" else op.cin) * (1 if op.kind == "convT" else k * k)
     return flop / 1e9

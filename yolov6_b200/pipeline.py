@@ -26,6 +26,14 @@ the call, so frames a kernel wrote there are complete when the graph reads them.
 must not write to them until `collect()` has returned their batch (`DetectPipeline.__call__` returns after the batch is
 done); the pipeline keeps a reference to them at least until then, so dropping them early is safe.
 
+`auto=True` (with raw_input) serves the way `tools/infer.py` letterboxes: `Inferer.process_image` pads a frame only up to the
+next multiple of the stride (letterbox auto=True), so a 1920 x 1080 frame at img_size 640 runs on a 384 x 640 canvas, 0.6
+of the square one's conv work.  `height, width` are then Inferer's img_size and `source_shape=(h0, w0)` names the frames
+served: the pipeline is built, pinned and captured at `rect_canvas(h0, w0, (height, width), stride)`, exposed as `.canvas`
+(one fixed shape, so slots, graphs and lanes are those of the full canvas).  A frame of any size is accepted when its own
+rect canvas is that one (1080p and 720p both give 384 x 640 at 640); any other frame raises RuntimeError before anything is
+written.  `stride` defaults to Inferer's `max(model stride, 32)`.
+
 Each batch in flight lives in a `BatchSlot` (its input and staging buffers, pinned results and events): `DetectPipeline`
 holds one, `DetectStream` two, used by alternate steps.
 """
@@ -35,7 +43,8 @@ import os
 import torch
 
 from .nms import nms_batched_head, workspace_bytes
-from .preprocess import REC, check_frames, letterbox_frames_launch, pack_sources, rescale_launch
+from .preprocess import (REC, check_frames, inferer_size, inferer_stride, letterbox_frames_launch, pack_sources, rect_canvas,
+                         rescale_launch)
 
 RAW_DEFAULT_BYTES = 1920 * 1080 * 3        # staging bytes per batch slot when max_src_bytes is not given: one 1080p frame each
 OVERFLOW = "non_max_suppression: more than 65536 near-identical candidate scores in one image; raise conf_thres"
@@ -45,10 +54,13 @@ class BatchSlot:
     """The buffers and events of one batch in flight: the device input with its pinned host input or, for raw frames, the
     staging buffer, record and geometry tables; the pinned results; `ev_copied` (its H2D is complete) and `ev_done` (the
     step that read it is complete).  `hold_geo`: the letterbox keeps a copy of the geometry (`res_geo`) for a rescale that
-    runs after the copy stream may already have refilled `geo_dev` with the next batch's."""
+    runs after the copy stream may already have refilled `geo_dev` with the next batch's.  The input is `height x width`;
+    with `auto`, raw frames are letterboxed at img_size `size` with padding to a multiple of `stride` and must land on it."""
 
-    def __init__(self, batch, height, width, max_det, host_input, raw_input, max_src_bytes, dev, hold_geo=False):
+    def __init__(self, batch, height, width, max_det, host_input, raw_input, max_src_bytes, dev, hold_geo=False, auto=False,
+                 stride=32, size=None):
         self.dev, self.host_input, self.raw, self.hold_geo = dev, host_input, raw_input, hold_geo
+        self.auto, self.stride, self.size = auto, stride, tuple(size or (height, width))
         self.x_dev = torch.zeros(batch, 3, height, width, dtype=torch.uint8 if host_input else torch.float32, device=dev)
         self.x_host = torch.zeros(batch, 3, height, width, dtype=torch.uint8).pin_memory() if host_input and not raw_input else None
         if raw_input:
@@ -75,8 +87,9 @@ class BatchSlot:
             (self.x_host if self.host_input else self.x_dev).copy_(images)
             return
         srcs = check_frames(images, self.geo_host.shape[0], layout, self.dev)
-        self.nbytes, _, self.frames = pack_sources(srcs, self.geo_host.shape[0], self.x_dev.shape[2], self.x_dev.shape[3], True,
-                                                   layout, self.src_host, self.geo_host, self.rec_host, self.src_dev.data_ptr())
+        self.nbytes, _, self.frames = pack_sources(srcs, self.geo_host.shape[0], *self.size, True, layout, self.src_host,
+                                                   self.geo_host, self.rec_host, self.src_dev.data_ptr(), self.auto, self.stride,
+                                                   tuple(self.x_dev.shape[2:]))
         # only device frames need it: the caller's stream usually holds the previous step, and a copy that waited for it
         # would no longer overlap that step
         if self.frames:
@@ -144,18 +157,29 @@ class BatchSlot:
 
 class _Served:
     """What DetectPipeline and DetectStream share: the checks, NMS settings, pinned engine shape, NMS workspace and batch
-    slots, and the warm-up-then-capture of their graphs."""
+    slots, and the warm-up-then-capture of their graphs.  `canvas` is the (H, W) everything is built at: (height, width),
+    or with auto=True the rect canvas of `source_shape` at img_size (height, width)."""
 
-    def __init__(self, model, batch, height, width, nms_kw, host_input, raw_input, max_src_bytes, slots, engine=None):
+    def __init__(self, model, batch, height, width, nms_kw, host_input, raw_input, max_src_bytes, slots, engine=None, auto=False,
+                 source_shape=None, stride=None):
         self.model = model.eval()
         self.dev = next(model.parameters()).device
         if self.dev.type != "cuda":
             raise RuntimeError(f"{type(self).__name__} needs a CUDA model")
         if raw_input and not host_input:
             raise RuntimeError(f"{type(self).__name__}: raw_input returns detections in host memory (host_input=True)")
+        size = (height, width)
+        if auto:
+            if not raw_input or source_shape is None:
+                raise RuntimeError(f"{type(self).__name__}: auto=True letterboxes decoded frames: it needs raw_input=True and "
+                                   f"source_shape=(h0, w0)")
+            stride = int(stride or inferer_stride(model.graph.strides))
+            size = inferer_size(size, stride)
+            height, width = rect_canvas(*source_shape, size, stride)
+        self.canvas = (height, width)
         self.host_input = bool(host_input)
         self.slots = [BatchSlot(batch, height, width, nms_kw["max_det"], self.host_input, raw_input, max_src_bytes, self.dev,
-                                hold_geo=slots > 1) for _ in range(slots)]
+                                hold_geo=slots > 1, auto=bool(auto), stride=stride or 32, size=size) for _ in range(slots)]
         self.shape = (batch, height, width, self.slots[0].x_dev.dtype)
         self.eng = engine if engine is not None else model.engine()
         self.eng.pin(*self.shape)          # the graphs point at this shape's buffers
@@ -186,9 +210,10 @@ class _Served:
 class DetectPipeline(_Served):
     def __init__(self, model, batch, height, width, conf_thres=0.25, iou_thres=0.45, classes=None, agnostic=False,
                  multi_label=False, max_det=300, host_input=True, overlap_h2d=False, copy_stream=None, raw_input=False,
-                 max_src_bytes=None):
+                 max_src_bytes=None, auto=False, source_shape=None, stride=None):
         super().__init__(model, batch, height, width, dict(conf_thres=conf_thres, iou_thres=iou_thres, classes=classes,
-                         agnostic=agnostic, multi_label=multi_label, max_det=max_det), host_input, raw_input, max_src_bytes, 1)
+                         agnostic=agnostic, multi_label=multi_label, max_det=max_det), host_input, raw_input, max_src_bytes, 1,
+                         auto=auto, source_shape=source_shape, stride=stride)
         self.slot = self.slots[0]
         self.x_dev, self.x_host = self.slot.x_dev, self.slot.x_host
         self.n_frames = batch
@@ -285,10 +310,11 @@ class DetectStream(_Served):
     """
 
     def __init__(self, model, batch, height, width, conf_thres=0.25, iou_thres=0.45, classes=None, agnostic=False,
-                 multi_label=False, max_det=300, host_input=True, engine=None, raw_input=False, max_src_bytes=None):
+                 multi_label=False, max_det=300, host_input=True, engine=None, raw_input=False, max_src_bytes=None, auto=False,
+                 source_shape=None, stride=None):
         super().__init__(model, batch, height, width, dict(conf_thres=conf_thres, iou_thres=iou_thres, classes=classes,
                          agnostic=agnostic, multi_label=multi_label, max_det=max_det), host_input, raw_input, max_src_bytes, 2,
-                         engine)
+                         engine, auto, source_shape, stride)
         self.B = batch
         self.x_dev = [s.x_dev for s in self.slots]
         self.x_host = [s.x_host for s in self.slots] if self.slots[0].x_host is not None else None
@@ -389,7 +415,8 @@ class DetectFarm:
     before the next dependent kernel) next to the head of the other lane's kernel: the persistent conv kernels hold one CTA
     per SM, so the lanes interleave kernel by kernel rather than share SMs, and what one lane leaves idle the other fills.
     Costs `lanes` x the activation memory (YOLOv6-S bs32: ~2.3 GB per lane).  Per-lane results are those of DetectStream
-    (bit-identical to the serial path); batch order across lanes is the submission order."""
+    (bit-identical to the serial path); batch order across lanes is the submission order.  `.canvas` is the lanes' input
+    shape (with auto=True, the rect canvas of `source_shape`)."""
 
     def __init__(self, model, batch, height, width, lanes=2, **kw):
         from .engine import InferEngine
@@ -400,6 +427,7 @@ class DetectFarm:
         for i in range(lanes):
             eng = model.engine() if i == 0 else InferEngine(model.graph, model.state_dict(), self.dev, model.precision)
             self.lanes.append(DetectStream(model, batch, height, width, engine=eng, **kw))
+        self.canvas = self.lanes[0].canvas
         self.n = 0
         self._ev = [torch.cuda.Event() for _ in range(lanes)]
         self._go = torch.cuda.Event()

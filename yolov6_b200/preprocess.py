@@ -8,11 +8,15 @@ tensors in place.  A per-image record table says where each image is and in whic
 carries the geometry the host computed with the reference's Python expressions.  Because both are data, a CUDA graph that
 contains these kernels serves any mix of image sizes, layouts and locations.
 
-Only letterbox(..., auto=False) is provided: it pads every image to the full H x W canvas, so a batch has one shape.
-Inferer's own default, auto=True, pads to a stride multiple and gives each image its own shape; that does not fit a
-fixed-shape batch.  Decoding (JPEG / PNG -> pixels) stays with the caller.
+Both of the reference's padding modes are provided.  auto=False pads every image to the full H x W canvas (the Evaler's
+and a fixed-shape server's choice).  auto=True is Inferer's own default: the image is padded only up to the next multiple
+of the stride, so a 1920 x 1080 frame at img_size 640 reaches the network as a 384 x 640 canvas.  Each source shape then
+has its own canvas (`rect_canvas`); a batch takes one canvas, so frames whose canvases differ are refused before anything
+is staged, and a caller serving mixed sources keeps one batch per canvas.  Decoding (JPEG / PNG -> pixels) stays with the
+caller.
 """
 import ctypes as C
+import math
 
 import numpy as np
 import torch
@@ -22,15 +26,59 @@ from . import _lib
 GEO = 8      # int32 per image in the geometry table: src_off, h0, w0, nh, nw, top, left, 0 (YV6_LB_GEO)
 
 
-def letterbox_geometry(h0, w0, H, W, scaleup=True):
-    """The reference's letterbox numbers for an h0 x w0 image on an H x W canvas (data_augment.py:38-55, auto=False):
-    (r, (nw, nh), top, left), new_unpad = (nw, nh) rounded half to even as Python's round() does."""
+def inferer_stride(strides):
+    """The stride Inferer pads and rounds img_size to: DetectBackend's max(model stride, 32) -- 32 for the P5 detectors,
+    64 for the P6 and Lite ones."""
+    return max(max(int(s) for s in strides), 32)
+
+
+def inferer_size(img_size, stride):
+    """Inferer.check_img_size: img_size (an int or (H, W)) with each side rounded up to a multiple of `stride`, as (H, W)."""
+    H, W = (img_size, img_size) if isinstance(img_size, int) else img_size
+    return math.ceil(H / stride) * stride, math.ceil(W / stride) * stride
+
+
+def _resize_and_pad(h0, w0, H, W, scaleup, auto, stride):
+    """data_augment.py:38-49: (r, (nw, nh), (dw, dh)), the total padding before it is split between the two sides."""
     r = min(H / h0, W / w0)
     if not scaleup:
         r = min(r, 1.0)
     nw, nh = int(round(w0 * r)), int(round(h0 * r))
-    dw, dh = (W - nw) / 2, (H - nh) / 2
-    return r, (nw, nh), int(round(dh - 0.1)), int(round(dw - 0.1))
+    dw, dh = W - nw, H - nh
+    if auto:                     # minimum rectangle: np.mod(dw, stride); dw >= 0, so Python's % is the same
+        dw, dh = dw % stride, dh % stride
+    return r, (nw, nh), (dw, dh)
+
+
+def letterbox_geometry(h0, w0, H, W, scaleup=True, auto=False, stride=32):
+    """The reference's letterbox numbers for an h0 x w0 image and new_shape (H, W) (data_augment.py:38-55):
+    (r, (nw, nh), top, left), new_unpad = (nw, nh) rounded half to even as Python's round() does.  auto=False pads to the
+    full H x W canvas, auto=True only up to the next multiple of `stride` (the canvas is `rect_canvas`)."""
+    r, (nw, nh), (dw, dh) = _resize_and_pad(h0, w0, H, W, scaleup, auto, stride)
+    return r, (nw, nh), int(round(dh / 2 - 0.1)), int(round(dw / 2 - 0.1))
+
+
+def rect_canvas(h0, w0, img_size, stride, scaleup=True):
+    """The canvas (H, W) Inferer.process_image(im, img_size, stride, half) gives an h0 x w0 image: letterbox with auto=True
+    on img_size rounded up to the stride (`inferer_size`), i.e. (nh + dh, nw + dw) -- a multiple of `stride` on both sides.
+    1080 x 1920 at 640 / stride 32 -> (384, 640); at 320 / stride 64 -> (192, 320)."""
+    H, W = inferer_size(img_size, stride)
+    _, (nw, nh), (dw, dh) = _resize_and_pad(h0, w0, H, W, scaleup, True, stride)
+    return nh + dh, nw + dw
+
+
+def common_canvas(srcs, H, W, scaleup, stride):
+    """The rect canvas (`rect_canvas`) shared by checked frames (`check_frames`) at img_size (H, W); RuntimeError naming
+    both shapes when two frames' canvases differ (one batch has one canvas)."""
+    canvas = first = None
+    for _, _, h0, w0, *_ in srcs:
+        c = rect_canvas(h0, w0, (H, W), stride, scaleup)
+        if canvas is None:
+            canvas, first = c, (h0, w0)
+        elif c != canvas:
+            raise RuntimeError(f"letterbox: a {h0} x {w0} frame letterboxes to a {c[0]} x {c[1]} canvas, a {first[0]} x {first[1]} "
+                               f"frame of the same batch to {canvas[0]} x {canvas[1]} (auto=True: one canvas per batch)")
+    return canvas
 
 
 def as_frame(im):
@@ -100,19 +148,28 @@ def check_frames(frames, B, layout, dev):
     return out
 
 
-def pack_sources(srcs, B, H, W, scaleup, layout, src_host, geo_host, rec_host, src_dev_ptr):
+def pack_sources(srcs, B, H, W, scaleup, layout, src_host, geo_host, rec_host, src_dev_ptr, auto=False, stride=32, canvas=None):
     """Lay out checked frames (`check_frames`) for yv6_letterbox_frames: copy the host frames back to back into `src_host`
     (the device buffer at `src_dev_ptr` receives these bytes before the launch), fill the geometry table `geo_host` [B, GEO]
-    and the record table `rec_host` (B * REC bytes).  A device frame's record points at the frame itself.  Raises
-    RuntimeError before anything is written when the host frames exceed `src_host`.
+    and the record table `rec_host` (B * REC bytes).  A device frame's record points at the frame itself.  (H, W) is the
+    letterbox's new_shape; `canvas`, the shape of the device canvas, is (H, W) when not given.  With auto=True every frame's
+    `rect_canvas` must equal `canvas`.  Raises RuntimeError before anything is written when a frame's canvas differs or
+    the host frames exceed `src_host`.
     Returns (host bytes used, shapes, the device frames)."""
+    canvas = tuple(canvas or (H, W))
+    if auto:
+        got = common_canvas(srcs, H, W, scaleup, stride)
+        if got != canvas:
+            h0, w0 = srcs[0][2:4]
+            raise RuntimeError(f"letterbox: a {h0} x {w0} frame letterboxes to a {got[0]} x {got[1]} canvas at img_size {H} x {W}, "
+                               f"stride {stride}; this batch's canvas is {canvas[0]} x {canvas[1]}")
     used = sum(t.numel() for t, on_dev, *_ in srcs if not on_dev)
     if used > src_host.numel():
         raise RuntimeError(f"letterbox: the host frames hold {used} bytes, the staging buffer {src_host.numel()} (raise max_src_bytes)")
     recs = (_lib.LbSrc * B)()
     rows, shapes, devs, off = [], [], [], 0
     for i, (t, on_dev, h0, w0, row_pitch, plane_pitch) in enumerate(srcs):
-        r, (nw, nh), top, left = letterbox_geometry(h0, w0, H, W, scaleup)
+        r, (nw, nh), top, left = letterbox_geometry(h0, w0, H, W, scaleup, auto, stride)
         if on_dev:
             base, src_off = t.data_ptr(), 0
             devs.append(t)
@@ -123,7 +180,7 @@ def pack_sources(srcs, B, H, W, scaleup, layout, src_host, geo_host, rec_host, s
         recs[i] = _lib.LbSrc(base, row_pitch, plane_pitch, LAYOUTS[layout], 0)
         rows.append([src_off, h0, w0, nh, nw, top, left, 0])
         shapes.append(((h0, w0), ((h0 * r / h0, w0 * r / w0), (left, top))))
-    rows += [[0, H, W, 0, 0, 0, 0, 0]] * (B - len(srcs))         # unused slots: all border, rescale well defined
+    rows += [[0, canvas[0], canvas[1], 0, 0, 0, 0, 0]] * (B - len(srcs))     # unused slots: all border, rescale well defined
     geo_host.copy_(torch.tensor(rows, dtype=torch.int32))
     C.memmove(rec_host.data_ptr(), recs, C.sizeof(recs))
     return used, shapes, devs
@@ -157,33 +214,40 @@ def rescale_launch(out, count, geo_dev, H, W, res=None, stream=None):
     return res
 
 
-def letterbox_batch(images, H, W, scaleup=True, out=None, device=None, layout="bgr_hwc"):
+def letterbox_batch(images, H, W, scaleup=True, out=None, device=None, layout="bgr_hwc", auto=False, stride=32):
     """Letterbox a list of uint8 frames of any sizes onto the uint8 NCHW RGB canvas [B, 3, H, W] on the device --
     letterbox(im, (H, W), auto=False, scaleup) + HWC->CHW + BGR->RGB of Inferer.process_image, bit-exact against cv2.
     Each frame is a host numpy array or CPU tensor (staged through pinned memory) or a CUDA tensor on the canvas's device
     (read in place, in stream order after the work already on the current stream).  `layout` applies to every frame:
     "bgr_hwc" is cv2 imread's [h0, w0, 3] (rows may be padded, e.g. a crop view), "rgb_chw" torchvision's decoders'
     [3, h0, w0]; both give the canvas of the equivalent BGR HWC image.  `scaleup=True` is Inferer's setting, False the
-    Evaler dataset's.  Returns (canvas, LetterboxMeta).  `out` (uint8 [B, 3, H, W] CUDA tensor, B >= len(images)) is
-    filled in place."""
+    Evaler dataset's.  auto=True is Inferer.process_image(im, (H, W), stride, half) itself: (H, W) is img_size (rounded up
+    to the stride) and the canvas is the frames' common `rect_canvas`; frames with different canvases raise RuntimeError
+    before anything is staged.  Returns (canvas, LetterboxMeta).  `out` (uint8 [B, 3, h, w] CUDA tensor on that canvas,
+    B >= len(images)) is filled in place."""
+    dev = out.device if out is not None else device or torch.device("cuda", torch.cuda.current_device())
+    if auto:
+        H, W = inferer_size((H, W), stride)
+    srcs = check_frames(images, out.shape[0] if out is not None else len(images), layout, dev)
+    canvas = common_canvas(srcs, H, W, scaleup, stride) if auto else (H, W)
     if out is None:
-        out = torch.empty(len(images), 3, H, W, dtype=torch.uint8, device=device or torch.device("cuda", torch.cuda.current_device()))
-    if out.device.type != "cuda" or out.dtype != torch.uint8 or tuple(out.shape[1:]) != (3, H, W):
+        out = torch.empty(len(images), 3, *canvas, dtype=torch.uint8, device=dev)
+    if out.device.type != "cuda" or out.dtype != torch.uint8 or tuple(out.shape[1:]) != (3, *canvas):
         raise RuntimeError("letterbox_batch: out must be a uint8 CUDA tensor [B, 3, H, W]")
     B = out.shape[0]
-    srcs = check_frames(images, B, layout, out.device)
     nbytes = max(1, sum(t.numel() for t, on_dev, *_ in srcs if not on_dev))
     src_host = torch.empty(nbytes, dtype=torch.uint8).pin_memory()
     geo_host = torch.empty(B, GEO, dtype=torch.int32).pin_memory()
     rec_host = torch.empty(B * REC, dtype=torch.uint8).pin_memory()
     src_dev = torch.empty(nbytes, dtype=torch.uint8, device=out.device)
-    _, shapes, _ = pack_sources(srcs, B, H, W, scaleup, layout, src_host, geo_host, rec_host, src_dev.data_ptr())
+    _, shapes, _ = pack_sources(srcs, B, H, W, scaleup, layout, src_host, geo_host, rec_host, src_dev.data_ptr(), auto, stride,
+                                canvas)
     src_dev.copy_(src_host, non_blocking=True)
     geo_dev = geo_host.to(out.device, non_blocking=True)
     rec_dev = rec_host.to(out.device, non_blocking=True)
     letterbox_frames_launch(rec_dev, geo_dev, out)
     torch.cuda.current_stream(out.device).synchronize()      # the pinned staging buffers die with this call
-    return out, LetterboxMeta(geo_host.clone(), len(images), H, W, shapes, geo_dev)
+    return out, LetterboxMeta(geo_host.clone(), len(images), canvas[0], canvas[1], shapes, geo_dev)
 
 
 def rescale_boxes(out, count, meta):
