@@ -373,6 +373,21 @@ int yv6_letterbox_frames(yv6_handle* h, const yv6_lb_src* srcs, const int32_t* g
 int yv6_rescale_boxes(yv6_handle* h, const float* det, const int32_t* count, const int32_t* geo, int32_t B, int32_t max_det,
                       int32_t H, int32_t W, float* out, void* stream);
 
+/* yv6_letterbox_val: the Evaler's validation images, TrainValDataset.__getitem__ with augment=False
+ *   (yolov6/data/datasets.py:189-198, 281-296): load_image's resize of the source to (nh, nw), then letterbox onto the batch
+ *   canvas with scaleup=False -- which, the canvas being at least nh x nw, only pads -- + HWC->CHW + BGR->RGB, into dst
+ *   uint8 NCHW [B,3,H,W].  Sources as for yv6_letterbox_frames (srcs, layouts, pitches); geo as above, with geo[7] the
+ *   image's mode, chosen by the caller the way cv::resize chooses its path:
+ *     YV6_VAL_COPY       (nh, nw) == (h0, w0): load_image's ratio is 1, the image is copied;
+ *     YV6_VAL_LINEAR     cv2.INTER_LINEAR enlargement (ratio > 1), as yv6_letterbox;
+ *     YV6_VAL_AREA       cv2.INTER_AREA shrink (ratio < 1), OpenCV's generic resizeArea_ path, bit-exact;
+ *     YV6_VAL_AREA_FAST  cv2.INTER_AREA shrink whose scales h0 / nh and w0 / nw are both integers (resizeAreaFast_), bit-exact.
+ *   Canvas outside [top, top+nh) x [left, left+nw) = 114; a slot with nh = 0 is all border and reads nothing.  The caller
+ *   guarantees top + nh <= H and left + nw <= W.  W % 16 == 0, dst 16-byte aligned. */
+enum { YV6_VAL_COPY = 0, YV6_VAL_LINEAR = 1, YV6_VAL_AREA = 2, YV6_VAL_AREA_FAST = 3 };
+int yv6_letterbox_val(yv6_handle* h, const yv6_lb_src* srcs, const int32_t* geo, int32_t B, int32_t H, int32_t W, uint8_t* dst,
+                      void* stream);
+
 /* ------------------------------------------------------------------------------------------------
  * Training augmentation from decoded frames: TrainValDataset.__getitem__ (yolov6/data/datasets.py:166-255) with
  * augment=True for a whole batch, bit-exact against the cv2 calls it makes.  All images live in one device byte arena

@@ -175,6 +175,7 @@ class LbSrc(C.Structure):
 
 
 LB_BGR_HWC, LB_RGB_CHW = 0, 1
+VAL_COPY, VAL_LINEAR, VAL_AREA, VAL_AREA_FAST = 0, 1, 2, 3      # yv6_letterbox_val's per-image modes (geo[7])
 XF_F32, XF_F64, XF_BF16 = 0, 1, 2
 XFORM_CHUNK = 4096
 
@@ -244,6 +245,7 @@ _SIGNATURES = {
     "yv6_eval_boxes": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
     "yv6_letterbox": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
     "yv6_letterbox_frames": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
+    "yv6_letterbox_val": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
     "yv6_rescale_boxes": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                     C.c_void_p, C.c_void_p]),
     "yv6_aug_resize": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int64, C.c_void_p]),
