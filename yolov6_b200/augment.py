@@ -17,7 +17,9 @@ The reference builds every training sample on the host in `TrainValDataset.__get
 side streams while batch i's graphs run, and writes the augmented images straight into the step's static uint8 input,
 ordered by events rather than host synchronisation.  Decoding (JPEG / PNG -> pixels) stays with the caller.
 
-Not provided: `rect` batches, `specific_shape` / `shrink_size` datasets and the dataloader's worker processes.
+Off the square: `Sampler(..., target="specific")` is `--specific-shape` (every sample on one H x W, load_image at
+min(W / w0, H / h0)); `target="rect"` with `rect_batches` is `--rect` (each batch on its own aspect-ratio canvas, which
+`Sampler.draw` / `AugmentFeed.draw` take per batch).  Not provided: `shrink_size` datasets and the dataloader's workers.
 """
 import ctypes as C
 import math
@@ -85,33 +87,48 @@ def transform_matrix(img_shape, new_shape, degrees, scale, shear, translate):
     return M, s
 
 
+TARGETS = (None, "specific", "rect")
+
+
 class Sampler:
     """The random draws of TrainValDataset.__getitem__ with augment=True, for a dataset of `n_images` images, training
-    images of H x W and `load_image` size `img_size` (default max(H, W))."""
+    images of H x W and `load_image` size `img_size` (default max(H, W)).
 
-    def __init__(self, n_images, H, W, hyp, img_size=None):
+    `target` says where __getitem__'s target_shape comes from, which decides load_image's size and the letterbox branch's
+    label arithmetic (`sample_labels`):
+      - None: the original rule of this class (an img_size load; float64 box arithmetic when H != W);
+      - "specific": --specific-shape, (height, width) as a Python tuple: load at min(W / w0, H / h0) (datasets.py:279-281),
+        box arithmetic in float32 at every shape;
+      - "rect": a numpy row of --rect's batch_shapes: an img_size load, box arithmetic in float64 at every shape, square
+        canvases included.  Each batch names its canvas in `draw(indices, canvas)`."""
+
+    def __init__(self, n_images, H, W, hyp, img_size=None, target=None):
+        if target not in TARGETS:
+            raise ValueError(f"augment: target must be one of {TARGETS}, got {target!r}")
         self.n, self.H, self.W, self.hyp = int(n_images), int(H), int(W), dict(hyp)
         self.img_size = int(img_size or max(H, W))
+        self.target = target
 
-    def _mosaic(self, index):
+    def _mosaic(self, index, H, W):
         """get_mosaic (datasets.py:452-467) + the draws of mosaic_augmentation (data_augment.py:156, 201)."""
         indices = [index] + random.choices(range(0, self.n), k=3)
         random.shuffle(indices)
-        yc, xc = (int(random.uniform(x // 2, 3 * x // 2)) for x in (self.H, self.W))
+        yc, xc = (int(random.uniform(x // 2, 3 * x // 2)) for x in (H, W))
         h = self.hyp
-        M, s = transform_matrix((2 * self.H, 2 * self.W), (self.H, self.W), h["degrees"], h["scale"], h["shear"], h["translate"])
+        M, s = transform_matrix((2 * H, 2 * W), (H, W), h["degrees"], h["scale"], h["shear"], h["translate"])
         return Canvas(indices, yc, xc, M, s)
 
-    def draw_one(self, index):
+    def draw_one(self, index, canvas=None):
         h = self.hyp
+        H, W = canvas or (self.H, self.W)
         rec = Sample(int(index), random.random() < h["mosaic"])
         if rec.mosaic:
-            rec.canvases.append(self._mosaic(index))
+            rec.canvases.append(self._mosaic(index, H, W))
             if random.random() < h["mixup"]:
-                rec.canvases.append(self._mosaic(random.randint(0, self.n - 1)))
+                rec.canvases.append(self._mosaic(random.randint(0, self.n - 1), H, W))
                 rec.mix_r = float(np.random.beta(32.0, 32.0))
         else:
-            M, s = transform_matrix((self.H, self.W), (self.H, self.W), h["degrees"], h["scale"], h["shear"], h["translate"])
+            M, s = transform_matrix((H, W), (H, W), h["degrees"], h["scale"], h["shear"], h["translate"])
             rec.canvases.append(Canvas([int(index)], None, None, M, s))
         if h["hsv_h"] or h["hsv_s"] or h["hsv_v"]:
             rec.gains = np.random.uniform(-1, 1, 3) * [h["hsv_h"], h["hsv_s"], h["hsv_v"]] + 1
@@ -119,22 +136,50 @@ class Sampler:
         rec.fliplr = random.random() < h["fliplr"]
         return rec
 
-    def draw(self, indices):
-        """One Sample per dataset index, in order.  `Plan.sources` lists the distinct source images the batch needs."""
-        return Plan([self.draw_one(i) for i in indices])
+    def draw(self, indices, canvas=None):
+        """One Sample per dataset index, in order, on `canvas` (H, W) (a --rect batch's; default the sampler's H x W).
+        `Plan.sources` lists the distinct source images the batch needs."""
+        H, W = (int(canvas[0]), int(canvas[1])) if canvas is not None else (self.H, self.W)
+        return Plan([self.draw_one(i, (H, W)) for i in indices], H, W)
+
+    def load_shape(self, h0, w0, H, W):
+        """load_image's size for a source of h0 x w0 drawn on an H x W canvas."""
+        if self.target == "specific":
+            return resized_shape(h0, w0, None, (H, W))
+        return resized_shape(h0, w0, self.img_size)
+
+
+def rect_batches(shapes_hw, img_size, batch, stride, world=1, rank=0):
+    """--rect's training batches of one rank: [(dataset indices, (H, W) canvas)], as the reference's train loader yields them
+    (create_dataloader(rect=True, pad=0.0, shuffle=False), data_load.py:40-92; core/engine.py:385-391) for sources of
+    (h0, w0) `shapes_hw` in dataset order.  Batch canvases come from `sort_files_shapes` over batch * world images
+    (datasets.py:89-100, 497-520; valdata.val_batches with pad 0); under DDP, DistributedSampler(shuffle=False,
+    drop_last=True) gives rank r the sorted positions r::world of the first floor(n / world) * world.  `stride` is
+    max(max(model strides), 32).  The last batch may be short, as the DataLoader's."""
+    from .valdata import val_batches
+    order, batch_index, canvases = val_batches(shapes_hw, img_size, batch * world, stride, pad=0.0)
+    n = len(order)
+    pos = range(n) if world == 1 else range(rank, n // world * world, world)
+    per_rank = min(batch, n)                 # create_dataloader's batch_size = min(batch_size, len(dataset))
+    out = []
+    for k in range(0, len(pos), per_rank):
+        p = pos[k:k + per_rank]
+        out.append(([int(order[i]) for i in p], tuple(int(v) for v in canvases[batch_index[p[0]]])))
+    return out
 
 
 class Plan:
-    """The records of one batch and the distinct source indices they read, in first-use order."""
+    """The records of one batch, its canvas H x W and the distinct source indices they read, in first-use order."""
 
-    def __init__(self, samples):
-        self.samples = samples
+    def __init__(self, samples, H=None, W=None):
+        self.samples, self.H, self.W = samples, H, W
         self.sources = list(dict.fromkeys(i for s in samples for i in s.sources()))
 
 
-def resized_shape(h0, w0, img_size):
-    """load_image's size (datasets.py:287-295): (int(h0 * r), int(w0 * r)) with r = img_size / max(h0, w0), or (h0, w0)."""
-    ratio = img_size / max(h0, w0)
+def resized_shape(h0, w0, img_size, specific=None):
+    """load_image's size (datasets.py:279-295): (int(h0 * r), int(w0 * r)) with r = img_size / max(h0, w0), or with
+    `specific` = (H, W) r = min(W / w0, H / h0); (h0, w0) when r == 1."""
+    ratio = min(specific[1] / w0, specific[0] / h0) if specific is not None else img_size / max(h0, w0)
     if ratio == 1:
         return h0, w0
     return int(h0 * ratio), int(w0 * ratio)
@@ -175,9 +220,9 @@ def _affine_labels(labels, M, s, height, width):
     return labels
 
 
-def _canvas_labels(rec, cv, hw, labels, H, W):
+def _canvas_labels(rec, cv, hw, labels, H, W, target=None):
     """Pixel-space labels of one canvas after its affine: mosaic_augmentation (data_augment.py:158-206) or the letterbox
-    branch of __getitem__ (datasets.py:196-229)."""
+    branch of __getitem__ (datasets.py:196-229).  `target`: Sampler's."""
     if rec.mosaic:
         tiles = _tiles(hw, cv.yc, cv.xc, H, W)
         labels4 = []
@@ -198,9 +243,10 @@ def _canvas_labels(rec, cv, hw, labels, H, W):
         return _affine_labels(labels4, cv.M, cv.s, H, W)
     (h, w), lab = hw[0], labels[0].copy()
     ratio, _, pad = letterbox_fit(h, w, H, W)
-    if H != W:
-        # a non-square shape reaches __getitem__ only as a numpy row of batch_shapes, which makes the ratio a numpy
-        # float64 and so the box arithmetic below float64 instead of float32
+    if target == "rect" or (target is None and H != W):
+        # a numpy row of batch_shapes makes the ratio a numpy float64 and so the box arithmetic below float64 instead of
+        # float32; --specific-shape's (height, width) tuple keeps it a Python float.  target=None assumes a non-square
+        # shape came from batch_shapes.
         ratio = np.float64(ratio)
     if lab.size:
         w *= ratio
@@ -214,13 +260,14 @@ def _canvas_labels(rec, cv, hw, labels, H, W):
     return _affine_labels(lab, cv.M, cv.s, H, W)
 
 
-def sample_labels(rec, shapes, labels, H, W, img_size):
+def sample_labels(rec, shapes, labels, H, W, img_size, target=None):
     """labels_out of __getitem__ (float32 [n, 6], column 0 zero) for a Sample, from the decoded sources' (h0, w0) and
-    their YOLO-format labels (float32 [k, 5]: cls, cx, cy, w, h normalised), both keyed by source index."""
+    their YOLO-format labels (float32 [k, 5]: cls, cx, cy, w, h normalised), both keyed by source index.  `target`:
+    Sampler's."""
     out = []
     for cv in rec.canvases:
-        hw = [resized_shape(*shapes[i], img_size) for i in cv.indices]
-        out.append(_canvas_labels(rec, cv, hw, [labels[i] for i in cv.indices], H, W))
+        hw = [resized_shape(*shapes[i], img_size, (H, W) if target == "specific" else None) for i in cv.indices]
+        out.append(_canvas_labels(rec, cv, hw, [labels[i] for i in cv.indices], H, W, target))
     lab = np.concatenate(out, 0) if len(out) > 1 else out[0]
     if len(lab):
         h, w = H, W
@@ -324,26 +371,39 @@ class AugmentFeed:
         feed.wait()                                  # the current stream waits; step.images / step.targets hold the batch
         out = train_step.run(epoch)
 
+    Off the square: `target` is Sampler's.  With target="rect", H x W is the largest canvas (img_size x img_size), which
+    sizes the staging, and each batch brings its own: `feed.draw(indices, canvas)` (`rect_batches` gives both); a step
+    built with `shapes` is switched to that canvas by `submit`.  With target="specific", H and W must be multiples of
+    `stride` (the model's largest stride when a step is given, else 32).
+
     `submit` validates every frame (uint8 HWC, 3 channels) and label array ([k, 5] normalised) and raises RuntimeError
     before anything is enqueued.  It then stages the sources in pinned memory, copies them on a copy stream, resizes them
     on an augmentation stream, and writes the batch into `images` / `targets` once everything enqueued on the caller's
     stream before the call (the previous step) is done.  The host waits only before reusing a staging slot, for the batch
     submitted two calls earlier.  Without `step`, the feed owns `images` and `targets`."""
 
-    def __init__(self, batch, H, W, hyp, n_images, max_src_bytes, img_size=None, step=None, max_targets=None, device=None):
+    def __init__(self, batch, H, W, hyp, n_images, max_src_bytes, img_size=None, step=None, max_targets=None, device=None,
+                 target=None, stride=None):
         if W % 32:
             raise RuntimeError(f"augment: W ({W}) must be a multiple of 32")
+        if target == "specific":
+            stride = int(stride or (max(step.eng.g.strides) if step is not None else 32))
+            if H % stride or W % stride:
+                raise ValueError(f"augment: a specific shape of {H} x {W} is not a multiple of the model's largest stride {stride}")
         self.B, self.H, self.W = int(batch), int(H), int(W)
-        self.sampler = Sampler(n_images, H, W, hyp, img_size)
+        self.sampler = Sampler(n_images, H, W, hyp, img_size, target)
         self.img_size = self.sampler.img_size
         self.max_src = int(max_src_bytes)
+        self.step = step
         if step is not None:
-            if (step.B, step.H, step.W) != (self.B, self.H, self.W) or step.images.dtype != torch.uint8:
+            full = step.shapes[0] if step.shapes is not None else (step.H, step.W)
+            if (step.B, *full) != (self.B, self.H, self.W) or step.images.dtype != torch.uint8:
                 raise RuntimeError("augment: the TrainStep must take uint8 [batch, 3, H, W] images")
             self.dev, self.images, self.targets = step.dev, step.images, step.targets
         else:
             self.dev = device or torch.device("cuda", torch.cuda.current_device())
-            self.images = torch.empty(self.B, 3, H, W, dtype=torch.uint8, device=self.dev)
+            self._store = torch.empty(self.B * 3 * H * W, dtype=torch.uint8, device=self.dev)
+            self.images = self._store.view(self.B, 3, H, W)
             self.targets = torch.full((int(max_targets or self.B * 64), 6), -1.0, device=self.dev)
         self.max_targets = self.targets.shape[0]
         self.copy_stream = torch.cuda.Stream(device=self.dev)
@@ -357,13 +417,19 @@ class AugmentFeed:
         self.turn = 0
         self.ready = None
 
-    def draw(self, indices):
+    def draw(self, indices, canvas=None):
         if len(indices) != self.B:
             raise RuntimeError(f"augment: {len(indices)} indices for a batch of {self.B}")
-        return self.sampler.draw(indices)
+        if canvas is not None:
+            h, w = int(canvas[0]), int(canvas[1])
+            if h > self.H or w > self.W or w % 32:
+                raise RuntimeError(f"augment: canvas {h} x {w} must fit inside {self.H} x {self.W} with a width that is a "
+                                   f"multiple of 32")
+        return self.sampler.draw(indices, canvas)
 
     def _layout(self, plan, frames):
         """Arena offsets, resize jobs and sample tables of one batch (host only)."""
+        H, W = plan.H, plan.W
         off, loc, shapes = 0, {}, {}
         for i in plan.sources:
             loc[i] = off
@@ -373,7 +439,7 @@ class AugmentFeed:
         jobs1, jobs2, res, lb = [], [], {}, {}
         for i in plan.sources:
             h0, w0 = shapes[i]
-            h, w = resized_shape(h0, w0, self.img_size)
+            h, w = self.sampler.load_shape(h0, w0, H, W)
             if h < 1 or w < 1:
                 raise RuntimeError(f"augment: source {i} of {h0}x{w0} resizes to {h}x{w}")
             if (h, w) == (h0, w0):
@@ -389,21 +455,21 @@ class AugmentFeed:
                 s.minv[j][:] = invert_affine(cv.M)
                 if rec.mosaic:
                     hw = [res[i][1:] for i in cv.indices]
-                    s.ch[j], s.cw[j], s.ntile[j] = 2 * self.H, 2 * self.W, 4
-                    for t, (i, (y1a, y2a, x1a, x2a, y1b, x1b)) in enumerate(zip(cv.indices, _tiles(hw, cv.yc, cv.xc, self.H, self.W))):
+                    s.ch[j], s.cw[j], s.ntile[j] = 2 * H, 2 * W, 4
+                    for t, (i, (y1a, y2a, x1a, x2a, y1b, x1b)) in enumerate(zip(cv.indices, _tiles(hw, cv.yc, cv.xc, H, W))):
                         o, _, w = res[i]
                         s.tile[j][t] = AugTile(o + ((y1b - y1a) * w + (x1b - x1a)) * 3, w, y1a, y2a, x1a, x2a, 0)
                 else:
                     i = cv.indices[0]
                     o, h, w = res[i]
-                    _, (nw, nh), (left, top) = letterbox_fit(h, w, self.H, self.W)
+                    _, (nw, nh), (left, top) = letterbox_fit(h, w, H, W)
                     if (nh, nw) != (h, w):
                         if i not in lb:
                             jobs2.append([o, h, w, off, nh, nw, 0, 0])
                             lb[i] = off
                             off += nh * nw * 3
                         o = lb[i]
-                    s.ch[j], s.cw[j], s.ntile[j] = self.H, self.W, 1
+                    s.ch[j], s.cw[j], s.ntile[j] = H, W, 1
                     s.tile[j][0] = AugTile(o - (top * nw + left) * 3, nw, top, top + nh, left, left + nw, 0)
             s.mixup = int(rec.mix_r is not None)
             s.mix_r = rec.mix_r or 0.0
@@ -426,7 +492,8 @@ class AugmentFeed:
         if used > self.max_src:
             raise RuntimeError(f"augment: the sources hold {used} bytes, the staging buffer {self.max_src} (raise max_src_bytes)")
         used, total, shapes, loc, jobs1, jobs2, smp = self._layout(plan, fr)
-        tg = [sample_labels(rec, shapes, lab, self.H, self.W, self.img_size) for rec in plan.samples]
+        H, W = plan.H, plan.W
+        tg = [sample_labels(rec, shapes, lab, H, W, self.img_size, self.sampler.target) for rec in plan.samples]
         for k, t in enumerate(tg):
             t[:, 0] = k
         targets = torch.cat(tg, 0)
@@ -449,6 +516,13 @@ class AugmentFeed:
         n = targets.shape[0]
         slot["tgt"][:n].copy_(targets)
 
+        if self.step is None:                             # the feed's own buffer, viewed at this batch's canvas
+            self.images = self._store[:self.B * 3 * H * W].view(self.B, 3, H, W)
+        elif self.step.shapes is not None:
+            self.step.use_shape(H, W)
+            self.images = self.step.images
+        elif (H, W) != (self.step.H, self.step.W):
+            raise RuntimeError(f"augment: a {H} x {W} batch for a TrainStep of {self.step.H} x {self.step.W} (build it with shapes=)")
         released = torch.cuda.Event()
         released.record(torch.cuda.current_stream(self.dev))       # the consumer's previous step has read images / targets
         arena = slot["arena"]
@@ -468,7 +542,7 @@ class AugmentFeed:
                     _lib.check(L.yv6_aug_resize(h, C.c_void_p(arena.data_ptr()), C.c_void_p(slot["jobs_dev"][r].data_ptr()), nj[r],
                                                 max_pix, sp))
             self.aug_stream.wait_event(released)
-            _lib.check(L.yv6_augment(h, C.c_void_p(arena.data_ptr()), C.c_void_p(slot["samples_dev"].data_ptr()), self.B, self.H, self.W,
+            _lib.check(L.yv6_augment(h, C.c_void_p(arena.data_ptr()), C.c_void_p(slot["samples_dev"].data_ptr()), self.B, H, W,
                                      C.c_void_p(self.images.data_ptr()), sp))
             self.targets[:n].copy_(slot["tgt"][:n], non_blocking=True)
             if n < self.max_targets:

@@ -22,6 +22,13 @@ running statistics untouched, as get_teacher_model's `track_running_stats = Fals
 own next to the student's forward -- both read the same input buffer -- joins it, and computes the detection loss, the two
 KL terms (and the lrtb IoU term of ComputeLossNS, the channel-wise term with `distill_feat`) into the student's gradient
 buffers.  The KL weights decay with the epoch (loss_distill.py:196), so the graphs are captured once per epoch.
+
+Several canvases (`--rect` batches, core/engine.py:151): `shapes=[(H, W), ...]`, each inside the step's height x width, plans
+every shape over one set of activation, gradient and head-output buffers sized for the largest (`TrainEngine.plan_shapes`)
+and keeps the graphs of every (shape, assigner branch) once captured.  `use_shape` / `load` pick the next batch's shape; the
+loss normalises its targets with that H and W.  Weights, the flat gradient buckets, the optimizer and the all-reduce are
+shared.  The shared buffers are cleared when the shape changes, so a shape's step computes what a step built for it alone
+computes.  Distillation takes one shape only.
 """
 import torch
 import torch.distributed as dist
@@ -33,7 +40,7 @@ from .dist import GradSync
 class TrainStep:
     def __init__(self, model, compute_loss, batch, height, width, in_dtype=torch.float32, max_targets=None, max_gt=64,
                  optimizer=None, n_buckets=None, graph=True, group=None, compute_loss_ab=None, teacher=None, temperature=20.0,
-                 max_epoch=None):
+                 max_epoch=None, shapes=None):
         self.fuse_ab = bool(getattr(model, "fuse_ab", False))
         self.distill = isinstance(compute_loss, loss_distill.ComputeLoss)
         if self.distill or teacher is not None:
@@ -49,13 +56,24 @@ class TrainStep:
         if n_buckets is None:
             n_buckets = 3 if self.world > 1 else 1
         self.eng = model.train_engine(n_buckets=n_buckets)
-        self.B, self.H, self.W = batch, height, width
+        self.B, self.H, self.W, self.in_dtype = batch, height, width, in_dtype
         self.max_gt = int(max_gt)
         self.max_targets = int(max_targets or batch * max_gt)
         self.targets = torch.full((self.max_targets, 6), -1.0, dtype=torch.float32, device=self.dev)
         if self.distill and self.loss.distill_feat != self.eng.external_feat_grads:
             self.eng.external_feat_grads = self.loss.distill_feat     # the neck outputs' gradients come from the channel-wise term
             self.eng._shape = None
+        self.shapes = None
+        if shapes is not None:      # several (H, W) canvases (--rect): one arena sized for the largest, graphs per shape
+            self.shapes = list(dict.fromkeys([(int(height), int(width))] + [(int(h), int(w)) for h, w in shapes]))
+            for h, w in self.shapes:
+                if h > height or w > width:
+                    raise ValueError(f"shape {h}x{w} does not fit inside the step's {height}x{width}: every rect canvas "
+                                     f"(pad 0) fits inside img_size x img_size")
+            if teacher is not None and len(self.shapes) > 1:
+                raise ValueError(f"distillation over several shapes ({self.shapes}) is not supported: build one TrainStep "
+                                 f"per shape")
+            self.eng.plan_shapes(batch, self.shapes, in_dtype)
         self.eng._plan(batch, height, width, in_dtype)
         self.images = self.eng.x_static
         self.teacher = teacher
@@ -67,7 +85,9 @@ class TrainStep:
         self.opt = optimizer
         self.sync = GradSync(self.eng.flat.gflat, self.eng.bucket_range, group) if self.world > 1 else None
         self.use_graph = bool(graph)
-        self.graphs = {}           # (assigner branch (True = ATSS warm-up), epoch when distilling) -> list of graph segments
+        self.graphs = {}           # (assigner branch (True = ATSS warm-up), epoch when distilling[, (H, W)]) -> list of graph segments
+        self.states = {}           # with shapes: the same key -> the loss state its graphs write, and the anchors they read
+        self.captures = 0
         self.state = None
         self.accumulate = False
         self.sizes = self.eng.sizes
@@ -155,12 +175,29 @@ class TrainStep:
                 self._segment(j, epoch_num)
             pool = gph.pool()
             graphs.append(gph)
+        self.captures += 1
         return graphs
 
+    def _planned_here(self):
+        """With shapes: the engine planned at the current shape, its arena holding that shape's tensors."""
+        self.eng._plan(self.B, self.H, self.W, self.in_dtype)
+        self.eng.make_live(self.H, self.W)
+        self.sizes = self.eng.sizes
+
     # ------------------------------------------------------------------ public
+    def use_shape(self, height, width):
+        """A step built with `shapes`: makes (height, width) the shape of the next `load` / `run`; `images` becomes that
+        shape's input view (an AugmentFeed writes the batch there)."""
+        if self.shapes is None or (int(height), int(width)) not in self.shapes:
+            raise ValueError(f"shape {height}x{width} is not one of this step's shapes {self.shapes}")
+        self.H, self.W = int(height), int(width)
+        self.images = self.eng.x_store[:self.B * 3 * self.H * self.W].view(self.B, 3, self.H, self.W)
+
     def load(self, images, targets):
         """images: [B,3,H,W] (host or device; pinned host memory makes the copy asynchronous); targets: [n,6] fp32
-        (img, cls, cx, cy, w, h normalised), n <= max_targets."""
+        (img, cls, cx, cy, w, h normalised), n <= max_targets.  A step built with `shapes` takes any of them."""
+        if self.shapes is not None:
+            self.use_shape(*images.shape[2:])
         self.images.copy_(images, non_blocking=True)
         n = int(targets.shape[0])
         if n > self.max_targets:
@@ -178,11 +215,25 @@ class TrainStep:
             raise RuntimeError("the teacher's tensors were replaced after the step was built (model.to / .half / a train_engine "
                                "of its own); build the TrainStep again")
         key = (epoch_num < self.loss.warmup_epoch, epoch_num if self.distill else None)
+        if self.shapes is not None:   # graphs of every shape are kept; the arena is cleared when the shape changes
+            key += ((self.H, self.W),)
+            if not self.use_graph or accumulate != self.accumulate or key not in self.graphs:
+                if accumulate != self.accumulate:
+                    self.graphs, self.states = {}, {}
+                self._planned_here()
+            else:
+                self.eng.make_live(self.H, self.W)
         nseg = len(self._segments()[0])
         if self.use_graph:
             if accumulate != self.accumulate or key not in self.graphs:
                 self.accumulate = accumulate
-                self.graphs = {key: self._capture(epoch_num)}
+                if self.shapes is None:
+                    self.graphs = {key: self._capture(epoch_num)}
+                else:
+                    self.graphs[key] = self._capture(epoch_num)
+                    self.states[key] = (self.state, self.loss._anchors, getattr(self.loss_ab, "_anchors", None))
+            if self.shapes is not None:
+                self.state = self.states[key][0]
             graphs = self.graphs[key]
         for j in range(nseg):
             if self.use_graph:

@@ -172,9 +172,9 @@ class _Scratch:
     backward refills the other pair.  Also the max-pool backward scratch, the ConvTranspose quadrant gradients and the head
     gradients dl; a buffer that grows keeps its smaller predecessors, which earlier launches still use."""
 
-    def __init__(self, dev, dc_elems):
-        self.dev = dev
-        self.dc = [torch.zeros(dc_elems, dtype=torch.bfloat16, device=dev) for _ in range(4)]
+    def __init__(self, new, dc_elems):
+        self.new = new
+        self.dc = [new((dc_elems,), torch.bfloat16) for _ in range(4)]
         self.bn_ops = 0
         self.pool, self.quad, self.dl = [], [], []
 
@@ -184,8 +184,27 @@ class _Scratch:
     def grown(self, pools, numel, count, dtype):
         """The last set of `count` buffers in `pools`, after appending a new set when it holds fewer than numel elements."""
         if not pools or pools[-1][0].numel() < numel:
-            pools.append([torch.zeros(numel, dtype=dtype, device=self.dev) for _ in range(count)])
+            pools.append([self.new((numel,), dtype) for _ in range(count)])
         return pools[-1]
+
+
+class _Arena:
+    """The per-shape tensors of a multi-shape plan (`TrainEngine.plan_shapes`): every shape's plan carves its activations,
+    gradients, head outputs and scratch from offset 0 of one byte buffer, in planning order, so the buffer is as large as the
+    largest single plan and the shapes' plans overlap.  Only one shape is live at a time: the buffer is cleared whenever the
+    live shape changes (`TrainEngine.make_live`), which leaves it as a fresh plan's torch.zeros would.  Over a meta tensor
+    it only measures a plan."""
+    ALIGN = 512                         # the caching allocator's granularity: a single plan's tensors start 512-aligned too
+
+    def __init__(self, store):
+        self.store, self.off, self.live = store, 0, None
+
+    def take(self, shape, dtype):
+        n = int(np.prod(shape)) * torch.empty(0, dtype=dtype).element_size()
+        o, self.off = self.off, self.off + (n + self.ALIGN - 1) // self.ALIGN * self.ALIGN
+        if self.off > self.store.numel():
+            raise RuntimeError(f"multi-shape plan: {self.off} bytes exceed the shared buffer's {self.store.numel()}")
+        return self.store[o:o + n].view(dtype).view(shape)
 
 
 FWD_ARENA_KEYS = ("fsum", "fcnt", "qsum", "qcnt")     # the zero-arena slots the forward pass uses (batch-statistics sums)
@@ -197,6 +216,7 @@ class TrainEngine:
     no gradient buffers, scratch or backward launches, and no anchor-aided pred convs of a fuse_ab model (the distillation loss
     reads the anchor-free head, loss_distill.py:76).  step.TrainStep runs it next to the student's step."""
     teacher = False
+    arena = None            # plan_shapes: the _Arena every planned shape's tensors are views into
 
     def __init__(self, model, n_buckets=1, teacher=False):
         self.teacher = bool(teacher)
@@ -505,6 +525,12 @@ class TrainEngine:
     def _bf(self, *shape):
         return torch.zeros(*shape, dtype=torch.bfloat16, device=self.dev)
 
+    def _new(self, shape, dtype=torch.bfloat16, zero=True):
+        """A per-shape tensor of the plan: a view into the multi-shape arena, or a tensor of its own."""
+        if self.arena is not None:
+            return self.arena.take(tuple(shape), dtype)
+        return (torch.zeros if zero else torch.empty)(*shape, dtype=dtype, device=self.dev)
+
     def _planned(self, op):
         """False for the pred convs a teacher leaves out: every head but the anchor-free cls / reg pair."""
         return not (self.teacher and op.kind == "pred" and op.head[0] not in ("cls", "reg"))
@@ -519,6 +545,27 @@ class TrainEngine:
                 d.res, d.alpha = 0, 0.0
         return _desc_launch("conv", "yv6_conv_fwd", d, writes=[Write(op.src.buf, op.src.c_off, op.cin, full, assign, group)])
 
+    def plan_shapes(self, N, shapes, in_dtype):
+        """Multi-shape mode: one input buffer for the largest image and one arena for the per-shape tensors (activations,
+        gradients, head outputs, scratch) sized for the largest single plan among `shapes` [(H, W)].  `_plan` then plans any
+        of those shapes as views into the two buffers, at the same addresses every time."""
+        if self.teacher:
+            raise ValueError("a teacher's forward plan reads its student's input: it takes no shape list")
+        shapes = [(int(h), int(w)) for h, w in shapes]
+        self.x_store = torch.zeros(N * 3 * max(h * w for h, w in shapes), dtype=in_dtype, device=self.dev)
+        need = 0
+        for H, W in shapes:                   # measure each plan on a meta buffer: sizes only, no device memory
+            self.arena, self._shape = _Arena(torch.empty(1 << 62, dtype=torch.uint8, device="meta")), None
+            self._plan(N, H, W, in_dtype)
+            need = max(need, self.arena.off)
+        self.arena, self._shape = _Arena(torch.zeros(need, dtype=torch.uint8, device=self.dev)), None
+
+    def make_live(self, H, W):
+        """Multi-shape mode: clears the arena when (H, W) is not the shape whose tensors it holds (the input buffer is kept)."""
+        if self.arena.live != (H, W):
+            self.arena.store.zero_()
+            self.arena.live = (H, W)
+
     def _plan(self, N, H, W, in_dtype, x_static=None):
         """Plans the step for one input shape.  x_static: an existing [N,3,H,W] input buffer for the stem to read (a teacher reads
         its student's), instead of one of the engine's own."""
@@ -527,15 +574,19 @@ class TrainEngine:
             return
         self._shape = key
         g, dev = self.g, self.dev
-        self.bufs = [self._bf(N, H >> b.level, W >> b.level, b.c_total) for b in g.bufs]
-        self.gbufs = [None] * len(self.bufs) if self.teacher else [torch.zeros_like(t) for t in self.bufs]
+        if self.arena is not None:
+            self.arena.off = 0
+        self.bufs = [self._new((N, H >> b.level, W >> b.level, b.c_total)) for b in g.bufs]
+        self.gbufs = [None] * len(self.bufs) if self.teacher else [self._new(t.shape) for t in self.bufs]
         self.sizes = [(H // s, W // s) for s in g.strides]
         self.offs = [0]
         for h, w in self.sizes:
             self.offs.append(self.offs[-1] + h * w)
         A = self.offs[-1]
-        self.cls = torch.empty(N, A, g.num_classes, dtype=torch.float32, device=dev)
-        self.reg = torch.empty(N, A, 4 * (g.reg_max + 1), dtype=torch.float32, device=dev)
+        self.cls = self._new((N, A, g.num_classes), torch.float32, zero=False)
+        self.reg = self._new((N, A, 4 * (g.reg_max + 1)), torch.float32, zero=False)
+        if x_static is None and self.arena is not None:       # the largest shape's input buffer, outside the arena
+            x_static = self.x_store[:N * 3 * H * W].view(N, 3, H, W)
         self.x_static = x_static if x_static is not None else torch.zeros(N, 3, H, W, dtype=in_dtype, device=dev)   # graph-stable address
         self.fwd_calls = []
         planners = {"pool": self._plan_pool, "pred": self._plan_pred, "convT": self._plan_convT}
@@ -545,19 +596,19 @@ class TrainEngine:
                     planners.get(op.kind, self._plan_bn_block)(i, op)
             self.bwd_calls, self.zero_gbufs = [], []
             return
-        self.grad_cls = torch.zeros_like(self.cls)
-        self.grad_reg = torch.zeros_like(self.reg)
+        self.grad_cls = self._new(self.cls.shape, torch.float32)
+        self.grad_reg = self._new(self.reg.shape, torch.float32)
         if getattr(g, "distill_ns", False):   # N / S distillation student: DFL logits next to the 4 lrtb distances
-            self.reg_dist = torch.empty(N, A, g.dist_reg_ch, dtype=torch.float32, device=dev)
-            self.grad_reg_dist = torch.zeros_like(self.reg_dist)
+            self.reg_dist = self._new((N, A, g.dist_reg_ch), torch.float32, zero=False)
+            self.grad_reg_dist = self._new(self.reg_dist.shape, torch.float32)
         if getattr(g, "fuse_ab", False):      # anchor-aided branch (effidehead_fuseab.py:94-140): 3 anchors per pixel, rows (level, anchor, pixel)
             from .arch import AB_ANCHORS
-            self.cls_ab = torch.empty(N, AB_ANCHORS * A, g.num_classes, dtype=torch.float32, device=dev)
-            self.reg_ab = torch.empty(N, AB_ANCHORS * A, 4, dtype=torch.float32, device=dev)
-            self.grad_cls_ab = torch.zeros_like(self.cls_ab)
-            self.grad_reg_ab = torch.zeros_like(self.reg_ab)
+            self.cls_ab = self._new((N, AB_ANCHORS * A, g.num_classes), torch.float32, zero=False)
+            self.reg_ab = self._new((N, AB_ANCHORS * A, 4), torch.float32, zero=False)
+            self.grad_cls_ab = self._new(self.cls_ab.shape, torch.float32)
+            self.grad_reg_ab = self._new(self.reg_ab.shape, torch.float32)
             self._ab = {}                     # level -> {"cls_ab" / "reg_ab": (fp32 conv output, bf16 gradient)}
-        self.scratch = _Scratch(dev, max([N * (H >> g.bufs[op.dst.buf].level) * (W >> g.bufs[op.dst.buf].level) * op.cout
+        self.scratch = _Scratch(self._new, max([N * (H >> g.bufs[op.dst.buf].level) * (W >> g.bufs[op.dst.buf].level) * op.cout
                                           for op in g.ops if op.kind in ("conv", "stem")] + [1]))
         bwd_of_op = [planners.get(op.kind, self._plan_bn_block)(i, op) for i, op in enumerate(g.ops)]
         self.bwd_calls = []
@@ -567,6 +618,9 @@ class TrainEngine:
             if k is not None and self.last_op_of_bucket[k] == i:
                 self.bwd_calls.append(Launch("bucket", None, kernels=0, parity=ALL, bucket=k))
         self._resolve_first_writers()
+        if self.arena is not None and self.arena.store.device.type != "meta":
+            self.arena.live = None            # a new plan starts from cleared tensors, as a single plan's torch.zeros
+            self.make_live(H, W)
 
     # ------------------------------------------------------------------ one planner per op kind: each appends the op's forward
     # launches to self.fwd_calls and returns its backward launches
@@ -605,13 +659,13 @@ class TrainEngine:
                                                                                       y_elem_off=self.offs[lvl] * ch)))
             if self.teacher:
                 return []
-        dl = self._bf(N, lh, lw, chp)               # bf16 gradient of the conv's output, zero padded to chp channels
+        dl = self._new((N, lh, lw, chp))               # bf16 gradient of the conv's output, zero padded to chp channels
         self.scratch.dl.append(dl)
         bwd = []
         if which.endswith("_ab"):
             # fuse_ab pred conv: natural NHWC output [N, hw, na * ch] (fp32, sigmoid fused on the class branch); the pack /
             # grad kernels (csrc/yv6_fuseab.cu) move between it and the reference's (level, anchor, pixel) row order
-            raw = torch.empty(N, lh * lw, ch, dtype=torch.float32, device=self.dev)
+            raw = self._new((N, lh * lw, ch), torch.float32, zero=False)
             st = self._ab.setdefault(lvl, {})
             st[which] = (raw, dl)
             self.fwd_calls.append(_desc_launch("conv", "yv6_conv_fwd", self._conv_desc(src, op.src.c_off, Wt["w"], raw, bias=Wt["bias"],
@@ -679,7 +733,7 @@ class TrainEngine:
             if ent["k"] == 0:
                 xs.append((src, op.src.c_off))
             else:
-                raw = self._bf(n, ho, wo, op.cout)
+                raw = self._new((n, ho, wo, op.cout))
                 if op.kind == "stem":
                     N, H, W, in_dtype = self._shape
                     self.fwd_calls.append(_desc_launch("stem", "yv6_stem_fwd", ops.stem_desc(
@@ -746,7 +800,7 @@ class TrainEngine:
         (u, _), (v, _) = xs
         self.fwd_calls.append(_desc_launch("stats", "yv6_bn_stats_finalize", self._stats_desc(
             [xs[0]], op.cout, count, z(i, "fsum"), z(i, "fcnt"), [(op.name + ".rbr_dense.bn", st[0])])))
-        tq = self._bf(*u.shape)
+        tq = self._new(u.shape)
         q = self._qa_desc(op, u, v, st, tq, z(i, "qsum"), z(i, "qcnt"))
         if op.identity:
             src = self.bufs[op.src.buf]
@@ -787,7 +841,7 @@ class TrainEngine:
         bwd = []
         if op.kind == "stem":       # im2col once, then one tensor-core wgrad GEMM per branch
             N, H, W, in_dtype = self._shape
-            patches, patches_lo = self._bf(*dcs[0].shape[:3], 32), self._bf(*dcs[0].shape[:3], 32)     # image = hi + lo (bf16 planes)
+            patches, patches_lo = self._new((*dcs[0].shape[:3], 32)), self._new((*dcs[0].shape[:3], 32))     # image = hi + lo (bf16 planes)
             self._stem_patches = (patches, patches_lo)
             bwd.append(Launch("im2col", "yv6_stem_im2col", (self.x_static.data_ptr(), DT_U8 if in_dtype == torch.uint8 else DT_F32,
                                                             1.0 / 255.0, N, H, W, patches.data_ptr(), patches_lo.data_ptr())))

@@ -12,6 +12,10 @@ Trainer's per-epoch loader (core/engine.py:396-398) is built the same way with r
    (`sort_files_shapes`, datasets.py:498-520) make at least as large as every loaded image, so this step never resizes.
 3. `shapes` and the labels (datasets.py:197-246) follow from the truncated loaded size.
 
+With --specific-shape (`Evaler(specific_shape=True, height, width)`, the Trainer's loader with `--specific-shape`) every
+canvas is (height, width), load_image's r is min(width / w0, height / h0) whatever shrink_size says, and the batch order is
+still rect's when rect is on: `ValFeed(..., specific_shape=(height, width))`.
+
 `val_batches`, `val_geometry` and `val_labels` restate those expressions on the host; `ValFeed` runs steps 1-2 for a whole
 batch in one `yv6_letterbox_val` launch, bit-exact against cv2 (OpenCV's INTER_AREA has two paths: the integer-factor
 box mean and the generic weighted one; the host picks the one cv::resize would).  Decoding stays with the caller.
@@ -76,13 +80,18 @@ def area_fast(h0, w0, h, w):
     return abs(sx - round(sx)) < DBL_EPSILON and abs(sy - round(sy)) < DBL_EPSILON
 
 
-def val_geometry(h0, w0, canvas, img_size, shrink_size=None):
+def val_geometry(h0, w0, canvas, img_size, shrink_size=None, specific_shape=False):
     """load_image + letterbox(auto=False, scaleup=False) of an h0 x w0 source onto its batch canvas (H, W), with the
-    reference's own expressions (datasets.py:189-198, 281-296).  RuntimeError when the loaded size truncates to 0 (cv2.resize
-    raises there) or when the canvas is smaller than the loaded image (the letterbox would resize a second time)."""
+    reference's own expressions (datasets.py:189-198, 279-296).  With `specific_shape` (--specific-shape: the canvas is the
+    (height, width) of every batch) load_image's ratio is min(W / w0, H / h0) and shrink_size is not read.  RuntimeError
+    when the loaded size truncates to 0 (cv2.resize raises there) or when the canvas is smaller than the loaded image (the
+    letterbox would resize a second time)."""
     h0, w0 = int(h0), int(w0)
     H, W = int(canvas[0]), int(canvas[1])
-    ratio = (img_size - shrink_size) / max(h0, w0) if shrink_size else img_size / max(h0, w0)
+    if specific_shape:
+        ratio = min(W / w0, H / h0)
+    else:
+        ratio = (img_size - shrink_size) / max(h0, w0) if shrink_size else img_size / max(h0, w0)
     h, w = h0, w0
     if ratio != 1:
         w, h = int(w0 * ratio), int(h0 * ratio)
@@ -165,10 +174,15 @@ class ValFeed:
     `feed` never waits for the device.
     """
 
-    def __init__(self, batch, img_size, stride, shapes_hw, pad=0.5, rect=True, shrink_size=None, max_src_bytes=None, device=None):
+    def __init__(self, batch, img_size, stride, shapes_hw, pad=0.5, rect=True, shrink_size=None, max_src_bytes=None, device=None,
+                 specific_shape=None):
         self.batch, self.img_size, self.stride, self.shrink_size = int(batch), int(img_size), int(stride), shrink_size
         self.shapes_hw = np.array(shapes_hw, dtype=np.int64).reshape(-1, 2)
         self.order, self.batch_index, self.canvases = val_batches(self.shapes_hw, img_size, batch, stride, pad, rect)
+        self.specific_shape = specific_shape is not None
+        if self.specific_shape:      # --specific-shape: the order stays as rect sorts it, every canvas is (height, width)
+            self.canvases = np.empty_like(self.canvases)
+            self.canvases[:] = [int(specific_shape[0]), int(specific_shape[1])]
         self.position = np.empty(len(self.order), dtype=np.int64)
         self.position[self.order] = np.arange(len(self.order))
         self.dev = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
@@ -184,7 +198,7 @@ class ValFeed:
         """val_geometry of source `index` on its batch's canvas."""
         h0, w0 = self.shapes_hw[index]
         canvas = self.canvases[self.batch_index[self.position[index]]]
-        return val_geometry(h0, w0, canvas, self.img_size, self.shrink_size)
+        return val_geometry(h0, w0, canvas, self.img_size, self.shrink_size, self.specific_shape)
 
     def plan(self, indices, srcs):
         """Checks and numbers of one call (nothing written): the batch's canvas and each image's ValGeometry."""
