@@ -396,6 +396,10 @@ int yv6_letterbox_val(yv6_handle* h, const yv6_lb_src* srcs, const int32_t* geo,
  * yv6_aug_resize: jobs [J][YV6_AUG_JOB] int64 = (src_off, h0, w0, dst_off, nh, nw, 0, 0): cv2.resize(INTER_LINEAR) of
  *   each source to nh x nw (a plain copy when the sizes are equal).  One launch serves load_image's resize of every source
  *   of a batch; a second launch over its results serves the letterbox branch's resize.  max_pix >= every nh * nw.
+ * yv6_aug_resize_frames: the same resize (same jobs, same bytes) with job j's source read through srcs[j] (device [J]
+ *   yv6_lb_src, layouts and pitches as for yv6_letterbox_frames) instead of base + src_off, which is ignored: a frame
+ *   anywhere in device memory -- a decoder's output, a crop view, a frame cache.  The output is always packed BGR HWC at
+ *   base + dst_off, so a job with (nh, nw) == (h0, w0) copies the frame into the arena in the layout yv6_augment reads.
  * yv6_augment: samples [B] (yv6_aug_sample, device) -> dst uint8 NCHW RGB [B,3,H,W].  Per output pixel: the flips as an
  *   index remap, then for each canvas cv2.warpAffine's INTER_LINEAR / BORDER_CONSTANT 114 sample of a virtual canvas --
  *   a 114 background of ch x cw with ntile placed rectangles, later tiles over earlier ones -- the fp64 mixup blend, and
@@ -419,6 +423,8 @@ typedef struct {
   uint8_t lut[3][256];         /* augment_hsv's hue, saturation and value tables */
 } yv6_aug_sample;
 int yv6_aug_resize(yv6_handle* h, uint8_t* base, const int64_t* jobs, int32_t J, int64_t max_pix, void* stream);
+int yv6_aug_resize_frames(yv6_handle* h, const yv6_lb_src* srcs, const int64_t* jobs, int32_t J, int64_t max_pix,
+                          uint8_t* base, void* stream);
 int yv6_augment(yv6_handle* h, const uint8_t* base, const yv6_aug_sample* samples, int32_t B, int32_t H, int32_t W, uint8_t* dst,
                 void* stream);
 

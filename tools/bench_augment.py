@@ -42,9 +42,10 @@ def card():
 def gpu(args):
     import torch
     from oracle import fabricate as fab
-    from yolov6_b200.augment import HYP_YOLOV6L6, HYP_YOLOV6S, AugmentFeed, resized_shape
+    from yolov6_b200.augment import HYP_YOLOV6L6, HYP_YOLOV6S, AugmentFeed, as_source, batch_tables, resize_frames_launch
     from yolov6_b200.loss import ComputeLoss
     from yolov6_b200.model import build_model
+    from yolov6_b200.preprocess import check_frame
     from yolov6_b200.step import TrainStep
     dev = torch.device("cuda:0")
     B, S = args.batch, args.size
@@ -64,7 +65,8 @@ def gpu(args):
                 feed.submit(plan, src, labels)
                 torch.cuda.synchronize()
             for plan in plans[3:]:
-                used, total, shapes, loc, jobs1, jobs2, smp = feed._layout(plan, {i: torch.from_numpy(src[i]) for i in plan.sources})
+                srcs = {i: as_source(check_frame(src[i], "bgr_hwc", dev), "bgr_hwc") for i in plan.sources}
+                used, total, shapes, loc, jobs1, recs1, jobs2, smp = batch_tables(feed.sampler, B, plan, srcs)
                 feed.submit(plan, src, labels)
                 torch.cuda.synchronize()
                 e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -73,10 +75,12 @@ def gpu(args):
                 import ctypes as C
                 h, L, sp = _lib.handle(0), _lib.lib(), _lib.stream_ptr()
                 e0.record()
-                for r, jobs in enumerate((jobs1, jobs2)):
-                    if jobs:
-                        _lib.check(L.yv6_aug_resize(h, C.c_void_p(slot["arena"].data_ptr()), C.c_void_p(slot["jobs_dev"][r].data_ptr()), len(jobs),
-                                                    max(j[4] * j[5] for j in jobs), sp))
+                if jobs1:
+                    resize_frames_launch(dev, slot["recs_dev"].data_ptr(), slot["jobs_dev"][0].data_ptr(), len(jobs1),
+                                         max(j[4] * j[5] for j in jobs1), slot["arena"].data_ptr(), None)
+                if jobs2:
+                    _lib.check(L.yv6_aug_resize(h, C.c_void_p(slot["arena"].data_ptr()), C.c_void_p(slot["jobs_dev"][1].data_ptr()), len(jobs2),
+                                                max(j[4] * j[5] for j in jobs2), sp))
                 _lib.check(L.yv6_augment(h, C.c_void_p(slot["arena"].data_ptr()), C.c_void_p(slot["samples_dev"].data_ptr()), B, S, S,
                                          C.c_void_p(feed.images.data_ptr()), sp))
                 e1.record()

@@ -249,6 +249,7 @@ _SIGNATURES = {
     "yv6_rescale_boxes": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                     C.c_void_p, C.c_void_p]),
     "yv6_aug_resize": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int64, C.c_void_p]),
+    "yv6_aug_resize_frames": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int64, C.c_void_p, C.c_void_p]),
     "yv6_augment": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
     "yv6_bn_stats_finalize": (C.c_int, [C.c_void_p, C.POINTER(BnStatsDesc), C.c_void_p]),
     "yv6_stem_wgrad2": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_float, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64,

@@ -9,13 +9,16 @@ The reference builds every training sample on the host in `TrainValDataset.__get
     seeds those generators as the reference does gets the reference's augmentation sequence.
   - `sample_labels` moves the labels with the reference's own float64 / float32 numpy expressions: about seven boxes per
     image are not worth a kernel, and the same arithmetic gives the same rows.
-  - Two kernels per batch (`yv6_aug_resize`, `yv6_augment`, csrc/yv6_augment.cu) produce the pixels, bit-exact against
-    the cv2 calls above.  The canvas is never materialised: a per-sample table describes it as a 114 background with up
-    to four placed rectangles of resized sources, and the augment kernel samples it where warpAffine would.
+  - Two kernels per batch (`yv6_aug_resize_frames` / `yv6_aug_resize`, `yv6_augment`, csrc/yv6_augment.cu) produce the
+    pixels, bit-exact against the cv2 calls above.  The canvas is never materialised: a per-sample table describes it as
+    a 114 background with up to four placed rectangles of resized sources, and the augment kernel samples it where
+    warpAffine would.
 
 `AugmentFeed` ties them to a `TrainStep`: it stages the sources of batch i+1 in pinned memory, copies and resizes them on
 side streams while batch i's graphs run, and writes the augmented images straight into the step's static uint8 input,
-ordered by events rather than host synchronisation.  Decoding (JPEG / PNG -> pixels) stays with the caller.
+ordered by events rather than host synchronisation.  Frames may also be CUDA tensors (a GPU decoder's output, read in
+place), and `FrameCache` is the reference's --cache-ram in device memory.  Decoding (JPEG / PNG -> pixels) stays with the
+caller.
 
 Off the square: `Sampler(..., target="specific")` is `--specific-shape` (every sample on one H x W, load_image at
 min(W / w0, H / h0)); `target="rect"` with `rect_batches` is `--rect` (each batch on its own aspect-ratio canvas, which
@@ -30,7 +33,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from .preprocess import as_frame
+from .preprocess import LAYOUTS, REC, check_frame
 
 # yolov6/configs/*.py data_aug of the two flagship configurations
 HYP_YOLOV6S = dict(hsv_h=0.015, hsv_s=0.7, hsv_v=0.4, degrees=0.0, translate=0.1, scale=0.5, shear=0.0, flipud=0.0,
@@ -141,6 +144,10 @@ class Sampler:
         `Plan.sources` lists the distinct source images the batch needs."""
         H, W = (int(canvas[0]), int(canvas[1])) if canvas is not None else (self.H, self.W)
         return Plan([self.draw_one(i, (H, W)) for i in indices], H, W)
+
+    def geometry(self):
+        """What decides load_image's size: (n_images, target, img_size, and H x W for target="specific")."""
+        return self.n, self.target, self.img_size, (self.H, self.W) if self.target == "specific" else None
 
     def load_shape(self, h0, w0, H, W):
         """load_image's size for a source of h0 x w0 drawn on an H x W canvas."""
@@ -362,6 +369,107 @@ def hsv_luts(gains):
             np.clip(x * gains[2], 0, 255).astype(np.uint8))
 
 
+@dataclass
+class Source:
+    """Where the pixels of one source of a batch come from.  `staged`: a host frame copied into the batch arena (tensor
+    `t`); otherwise `base` is its device address (a CUDA frame, or a FrameCache entry).  (h0, w0) is the decoded size the
+    labels and load_image use, (ph, pw) the size of the pixels the record addresses (the load size for a cache entry)."""
+    t: torch.Tensor
+    staged: bool
+    h0: int
+    w0: int
+    ph: int
+    pw: int
+    base: int
+    row_pitch: int
+    plane_pitch: int
+    layout: int
+
+
+def as_source(checked, layout):
+    """A Source from `preprocess.check_frame`'s result for a frame in `layout`."""
+    t, on_dev, h0, w0, row_pitch, plane_pitch = checked
+    return Source(t, not on_dev, h0, w0, h0, w0, t.data_ptr() if on_dev else 0, row_pitch, plane_pitch, LAYOUTS[layout])
+
+
+def batch_tables(sampler, B, plan, srcs):
+    """Arena layout, resize jobs and sample tables of one batch (host only), from a Source per plan.sources entry.
+    The arena holds the staged host frames back to back, then the first pass's outputs, then the letterbox pass's.  A
+    staged BGR HWC frame already at its load size is read in place; every other source gets a first-pass job whose
+    record (in_arena, address or arena offset, row_pitch, plane_pitch, layout) says where it lies -- a copy job when it
+    is at its load size, so every source reaches the arena as packed BGR HWC.
+    Returns (staged bytes, arena bytes, {i: (h0, w0)}, {i: arena offset of a staged frame}, jobs1, recs1, jobs2, samples)."""
+    H, W = plan.H, plan.W
+    off, loc = 0, {}
+    for i in plan.sources:
+        if srcs[i].staged:
+            loc[i] = off
+            off += srcs[i].t.numel()
+    used = off
+    shapes = {i: (srcs[i].h0, srcs[i].w0) for i in plan.sources}
+    jobs1, recs1, jobs2, res, lb = [], [], [], {}, {}
+    for i in plan.sources:
+        s = srcs[i]
+        h, w = sampler.load_shape(s.h0, s.w0, H, W)
+        if h < 1 or w < 1:
+            raise RuntimeError(f"augment: source {i} of {s.h0}x{s.w0} resizes to {h}x{w}")
+        if s.staged and s.layout == _lib.LB_BGR_HWC and (h, w) == (s.h0, s.w0):
+            res[i] = (loc[i], h, w)
+        else:
+            jobs1.append([loc.get(i, 0), s.ph, s.pw, off, h, w, 0, 0])
+            recs1.append((s.staged, loc[i] if s.staged else s.base, s.row_pitch, s.plane_pitch, s.layout))
+            res[i] = (off, h, w)
+            off += h * w * 3
+    smp = (AugSample * B)()
+    for k, rec in enumerate(plan.samples):
+        s = smp[k]
+        for j, cv in enumerate(rec.canvases):
+            s.minv[j][:] = invert_affine(cv.M)
+            if rec.mosaic:
+                hw = [res[i][1:] for i in cv.indices]
+                s.ch[j], s.cw[j], s.ntile[j] = 2 * H, 2 * W, 4
+                for t, (i, (y1a, y2a, x1a, x2a, y1b, x1b)) in enumerate(zip(cv.indices, _tiles(hw, cv.yc, cv.xc, H, W))):
+                    o, _, w = res[i]
+                    s.tile[j][t] = AugTile(o + ((y1b - y1a) * w + (x1b - x1a)) * 3, w, y1a, y2a, x1a, x2a, 0)
+            else:
+                i = cv.indices[0]
+                o, h, w = res[i]
+                _, (nw, nh), (left, top) = letterbox_fit(h, w, H, W)
+                if (nh, nw) != (h, w):
+                    if i not in lb:
+                        jobs2.append([o, h, w, off, nh, nw, 0, 0])
+                        lb[i] = off
+                        off += nh * nw * 3
+                    o = lb[i]
+                s.ch[j], s.cw[j], s.ntile[j] = H, W, 1
+                s.tile[j][0] = AugTile(o - (top * nw + left) * 3, nw, top, top + nh, left, left + nw, 0)
+        s.mixup = int(rec.mix_r is not None)
+        s.mix_r = rec.mix_r or 0.0
+        s.hsv = int(rec.gains is not None)
+        if rec.gains is not None:
+            for c, lut in enumerate(hsv_luts(rec.gains)):
+                s.lut[c][:] = lut.tolist()
+        s.flipud, s.fliplr = int(rec.flipud), int(rec.fliplr)
+    return used, off, shapes, loc, jobs1, recs1, jobs2, smp
+
+
+def frame_records(recs, arena_ptr):
+    """The yv6_lb_src table of first-pass records (`batch_tables`) for an arena at device address `arena_ptr`."""
+    out = (_lib.LbSrc * max(len(recs), 1))()
+    for k, (in_arena, addr, row_pitch, plane_pitch, layout) in enumerate(recs):
+        out[k] = _lib.LbSrc(arena_ptr + addr if in_arena else addr, row_pitch, plane_pitch, layout, 0)
+    return out
+
+
+def resize_frames_launch(dev, recs_ptr, jobs_ptr, J, max_pix, base_ptr, stream):
+    """yv6_aug_resize_frames on device tables at `recs_ptr` / `jobs_ptr`, in launches of at most 65535 jobs."""
+    L, h = _lib.lib(), _lib.handle(dev.index or 0)
+    for k in range(0, J, 65535):
+        n = min(65535, J - k)
+        _lib.check(L.yv6_aug_resize_frames(h, C.c_void_p(recs_ptr + k * REC), C.c_void_p(jobs_ptr + k * JOB * 8), n, max_pix,
+                                           C.c_void_p(base_ptr), _lib.stream_ptr(stream)))
+
+
 class AugmentFeed:
     """Double-buffered device augmentation for batches of `batch` H x W training images.
 
@@ -376,14 +484,16 @@ class AugmentFeed:
     built with `shapes` is switched to that canvas by `submit`.  With target="specific", H and W must be multiples of
     `stride` (the model's largest stride when a step is given, else 32).
 
-    `submit` validates every frame (uint8 HWC, 3 channels) and label array ([k, 5] normalised) and raises RuntimeError
-    before anything is enqueued.  It then stages the sources in pinned memory, copies them on a copy stream, resizes them
-    on an augmentation stream, and writes the batch into `images` / `targets` once everything enqueued on the caller's
-    stream before the call (the previous step) is done.  The host waits only before reusing a staging slot, for the batch
-    submitted two calls earlier.  Without `step`, the feed owns `images` and `targets`."""
+    `submit` validates every frame and label array ([k, 5] normalised) and raises RuntimeError before anything is
+    enqueued.  It then stages the host frames in pinned memory, copies them on a copy stream, resizes every source on an
+    augmentation stream -- host frames from the arena, CUDA frames in place, `cache` entries from the FrameCache -- and
+    writes the batch into `images` / `targets` once everything enqueued on the caller's stream before the call (the
+    previous step) is done.  The host waits only before reusing a staging slot, for the batch submitted two calls
+    earlier.  Without `step`, the feed owns `images` and `targets`.  With `cache` (a FrameCache built on this feed's
+    `sampler` geometry), sources the cache holds need no frame."""
 
     def __init__(self, batch, H, W, hyp, n_images, max_src_bytes, img_size=None, step=None, max_targets=None, device=None,
-                 target=None, stride=None):
+                 target=None, stride=None, cache=None):
         if W % 32:
             raise RuntimeError(f"augment: W ({W}) must be a multiple of 32")
         if target == "specific":
@@ -401,11 +511,15 @@ class AugmentFeed:
                 raise RuntimeError("augment: the TrainStep must take uint8 [batch, 3, H, W] images")
             self.dev, self.images, self.targets = step.dev, step.images, step.targets
         else:
-            self.dev = device or torch.device("cuda", torch.cuda.current_device())
+            self.dev = _cuda_device(device)
             self._store = torch.empty(self.B * 3 * H * W, dtype=torch.uint8, device=self.dev)
             self.images = self._store.view(self.B, 3, H, W)
             self.targets = torch.full((int(max_targets or self.B * 64), 6), -1.0, device=self.dev)
         self.max_targets = self.targets.shape[0]
+        if cache is not None and (cache.geometry != self.sampler.geometry() or cache.dev != self.dev):
+            raise RuntimeError(f"augment: the FrameCache holds images loaded for {cache.geometry} on {cache.dev}, this feed loads "
+                               f"them for {self.sampler.geometry()} on {self.dev}")
+        self.cache = cache
         self.copy_stream = torch.cuda.Stream(device=self.dev)
         self.aug_stream = torch.cuda.Stream(device=self.dev)
         self.slots = [dict(staged=torch.empty(self.max_src, dtype=torch.uint8).pin_memory(), arena=None,
@@ -413,7 +527,9 @@ class AugmentFeed:
                            samples_dev=torch.empty(self.B * C.sizeof(AugSample), dtype=torch.uint8, device=self.dev),
                            jobs=torch.empty(2, 2 * 8 * self.B * JOB, dtype=torch.int64).pin_memory(),
                            jobs_dev=torch.empty(2, 2 * 8 * self.B * JOB, dtype=torch.int64, device=self.dev),
-                           tgt=torch.empty(self.max_targets, 6).pin_memory(), done=None) for _ in range(2)]
+                           recs=torch.empty(8 * self.B * REC, dtype=torch.uint8).pin_memory(),
+                           recs_dev=torch.empty(8 * self.B * REC, dtype=torch.uint8, device=self.dev),
+                           tgt=torch.empty(self.max_targets, 6).pin_memory(), frames=[], done=None) for _ in range(2)]
         self.turn = 0
         self.ready = None
 
@@ -427,71 +543,38 @@ class AugmentFeed:
                                    f"multiple of 32")
         return self.sampler.draw(indices, canvas)
 
-    def _layout(self, plan, frames):
-        """Arena offsets, resize jobs and sample tables of one batch (host only)."""
-        H, W = plan.H, plan.W
-        off, loc, shapes = 0, {}, {}
-        for i in plan.sources:
-            loc[i] = off
-            shapes[i] = tuple(frames[i].shape[:2])
-            off += frames[i].numel()
-        used = off
-        jobs1, jobs2, res, lb = [], [], {}, {}
-        for i in plan.sources:
-            h0, w0 = shapes[i]
-            h, w = self.sampler.load_shape(h0, w0, H, W)
-            if h < 1 or w < 1:
-                raise RuntimeError(f"augment: source {i} of {h0}x{w0} resizes to {h}x{w}")
-            if (h, w) == (h0, w0):
-                res[i] = (loc[i], h, w)
-            else:
-                jobs1.append([loc[i], h0, w0, off, h, w, 0, 0])
-                res[i] = (off, h, w)
-                off += h * w * 3
-        smp = (AugSample * self.B)()
-        for k, rec in enumerate(plan.samples):
-            s = smp[k]
-            for j, cv in enumerate(rec.canvases):
-                s.minv[j][:] = invert_affine(cv.M)
-                if rec.mosaic:
-                    hw = [res[i][1:] for i in cv.indices]
-                    s.ch[j], s.cw[j], s.ntile[j] = 2 * H, 2 * W, 4
-                    for t, (i, (y1a, y2a, x1a, x2a, y1b, x1b)) in enumerate(zip(cv.indices, _tiles(hw, cv.yc, cv.xc, H, W))):
-                        o, _, w = res[i]
-                        s.tile[j][t] = AugTile(o + ((y1b - y1a) * w + (x1b - x1a)) * 3, w, y1a, y2a, x1a, x2a, 0)
-                else:
-                    i = cv.indices[0]
-                    o, h, w = res[i]
-                    _, (nw, nh), (left, top) = letterbox_fit(h, w, H, W)
-                    if (nh, nw) != (h, w):
-                        if i not in lb:
-                            jobs2.append([o, h, w, off, nh, nw, 0, 0])
-                            lb[i] = off
-                            off += nh * nw * 3
-                        o = lb[i]
-                    s.ch[j], s.cw[j], s.ntile[j] = H, W, 1
-                    s.tile[j][0] = AugTile(o - (top * nw + left) * 3, nw, top, top + nh, left, left + nw, 0)
-            s.mixup = int(rec.mix_r is not None)
-            s.mix_r = rec.mix_r or 0.0
-            s.hsv = int(rec.gains is not None)
-            if rec.gains is not None:
-                for c, lut in enumerate(hsv_luts(rec.gains)):
-                    s.lut[c][:] = lut.tolist()
-            s.flipud, s.fliplr = int(rec.flipud), int(rec.fliplr)
-        return used, off, shapes, loc, jobs1, jobs2, smp
+    def submit(self, plan, frames, labels, layout="bgr_hwc", ready=None):
+        """Enqueue one batch.  frames: {source index: frame} covering the plan.sources the cache does not hold; labels:
+        {source index: float32 [k, 5] YOLO rows}.  Returns the host targets [n, 6] (collate_fn's rows).
 
-    def submit(self, plan, frames, labels):
-        """Enqueue one batch.  frames: {source index: uint8 HWC BGR image (numpy or CPU tensor)} covering plan.sources;
-        labels: {source index: float32 [k, 5] YOLO rows}.  Returns the host targets [n, 6] (collate_fn's rows)."""
+        A frame is a host image (numpy array or CPU tensor, staged through pinned memory) or a uint8 CUDA tensor on the
+        feed's device (read in place); both kinds may be mixed.  `layout` applies to every frame of the call: "bgr_hwc"
+        is cv2 imread's [h0, w0, 3] (rows may be padded, e.g. a crop view), "rgb_chw" torchvision's decoders' [3, h0, w0].
+        Device frames are read after the work enqueued on the current stream before this call, or after the event
+        `ready` when one is given.  Pass `ready` when the frames come from a side stream (a GPU decoder's): the current
+        stream usually holds the running step, and waiting for it would serialise this batch's augmentation behind that
+        step.  The feed keeps a reference to each device frame until its slot is reused, which waits for this batch, so a
+        frame may be dropped right after the call; work enqueued on the current stream after `wait()` for this batch may
+        overwrite the frames."""
+        srcs = {}
+        for i in plan.sources:
+            if self.cache is not None and self.cache.cached[i]:
+                srcs[i] = self.cache.source(i)
+                continue
+            if i not in frames:
+                raise RuntimeError(f"augment: no frame for source {i}" + (" and the cache does not hold it" if self.cache else ""))
+            try:
+                srcs[i] = as_source(check_frame(frames[i], layout, self.dev), layout)
+            except RuntimeError as e:
+                raise RuntimeError(f"augment: source {i}: {e}") from None
         try:
-            fr = {i: as_frame(frames[i]) for i in plan.sources}
             lab = {i: check_labels(labels[i], f"source {i}") for i in plan.sources}
         except KeyError as e:
-            raise RuntimeError(f"augment: no frame or labels for source {e.args[0]}") from None
-        used = sum(f.numel() for f in fr.values())
+            raise RuntimeError(f"augment: no labels for source {e.args[0]}") from None
+        used = sum(s.t.numel() for s in srcs.values() if s.staged)
         if used > self.max_src:
-            raise RuntimeError(f"augment: the sources hold {used} bytes, the staging buffer {self.max_src} (raise max_src_bytes)")
-        used, total, shapes, loc, jobs1, jobs2, smp = self._layout(plan, fr)
+            raise RuntimeError(f"augment: the host frames hold {used} bytes, the staging buffer {self.max_src} (raise max_src_bytes)")
+        used, total, shapes, loc, jobs1, recs1, jobs2, smp = batch_tables(self.sampler, self.B, plan, srcs)
         H, W = plan.H, plan.W
         tg = [sample_labels(rec, shapes, lab, H, W, self.img_size, self.sampler.target) for rec in plan.samples]
         for k, t in enumerate(tg):
@@ -499,17 +582,23 @@ class AugmentFeed:
         targets = torch.cat(tg, 0)
         if targets.shape[0] > self.max_targets:
             raise RuntimeError(f"augment: {targets.shape[0]} target rows exceed max_targets={self.max_targets}")
+        if self.step is not None and self.step.shapes is None and (H, W) != (self.step.H, self.step.W):
+            raise RuntimeError(f"augment: a {H} x {W} batch for a TrainStep of {self.step.H} x {self.step.W} (build it with shapes=)")
 
         slot = self.slots[self.turn]
         self.turn ^= 1
         if slot["done"] is not None:
             slot["done"].synchronize()              # the batch submitted two calls ago has left this slot
+        slot["frames"] = [s.t for s in srcs.values() if not s.staged and s.t is not None]
         if slot["arena"] is None or slot["arena"].numel() < total:
             slot["arena"] = torch.empty(max(total, 1), dtype=torch.uint8, device=self.dev)
+        arena = slot["arena"]
         for i in plan.sources:
-            slot["staged"][loc[i]:loc[i] + fr[i].numel()].copy_(fr[i].view(-1))
+            if srcs[i].staged:
+                slot["staged"][loc[i]:loc[i] + srcs[i].t.numel()].copy_(srcs[i].t.view(-1))
         C.memmove(slot["samples"].data_ptr(), C.addressof(smp), C.sizeof(smp))
-        nj = (len(jobs1), len(jobs2))
+        recs = frame_records(recs1, arena.data_ptr())
+        C.memmove(slot["recs"].data_ptr(), recs, C.sizeof(recs))
         for r, jobs in enumerate((jobs1, jobs2)):
             if jobs:
                 slot["jobs"][r, :len(jobs) * JOB].copy_(torch.tensor(jobs, dtype=torch.int64).view(-1))
@@ -521,26 +610,29 @@ class AugmentFeed:
         elif self.step.shapes is not None:
             self.step.use_shape(H, W)
             self.images = self.step.images
-        elif (H, W) != (self.step.H, self.step.W):
-            raise RuntimeError(f"augment: a {H} x {W} batch for a TrainStep of {self.step.H} x {self.step.W} (build it with shapes=)")
         released = torch.cuda.Event()
         released.record(torch.cuda.current_stream(self.dev))       # the consumer's previous step has read images / targets
-        arena = slot["arena"]
         with torch.cuda.stream(self.copy_stream):
             self.copy_stream.wait_stream(self.aug_stream)          # the previous batch is done with this slot's arena
             arena[:used].copy_(slot["staged"][:used], non_blocking=True)
             slot["samples_dev"].copy_(slot["samples"], non_blocking=True)
             slot["jobs_dev"].copy_(slot["jobs"], non_blocking=True)
+            slot["recs_dev"][:len(recs1) * REC].copy_(slot["recs"][:len(recs1) * REC], non_blocking=True)
         h = _lib.handle(self.dev.index or 0)
         L = _lib.lib()
         with torch.cuda.stream(self.aug_stream):
             self.aug_stream.wait_stream(self.copy_stream)
+            if slot["frames"]:
+                self.aug_stream.wait_event(ready if ready is not None else released)
+            if any(s.t is None for s in srcs.values()):
+                self.aug_stream.wait_event(self.cache.filled)     # the fills that wrote the cached sources
             sp = _lib.stream_ptr(self.aug_stream)
-            for r, jobs in enumerate((jobs1, jobs2)):
-                if jobs:
-                    max_pix = max(j[4] * j[5] for j in jobs)
-                    _lib.check(L.yv6_aug_resize(h, C.c_void_p(arena.data_ptr()), C.c_void_p(slot["jobs_dev"][r].data_ptr()), nj[r],
-                                                max_pix, sp))
+            if jobs1:
+                resize_frames_launch(self.dev, slot["recs_dev"].data_ptr(), slot["jobs_dev"][0].data_ptr(), len(jobs1),
+                                     max(j[4] * j[5] for j in jobs1), arena.data_ptr(), self.aug_stream)
+            if jobs2:
+                _lib.check(L.yv6_aug_resize(h, C.c_void_p(arena.data_ptr()), C.c_void_p(slot["jobs_dev"][1].data_ptr()), len(jobs2),
+                                            max(j[4] * j[5] for j in jobs2), sp))
             self.aug_stream.wait_event(released)
             _lib.check(L.yv6_augment(h, C.c_void_p(arena.data_ptr()), C.c_void_p(slot["samples_dev"].data_ptr()), self.B, H, W,
                                      C.c_void_p(self.images.data_ptr()), sp))
@@ -557,3 +649,124 @@ class AugmentFeed:
         if self.ready is None:
             raise RuntimeError("augment: no batch was submitted")
         torch.cuda.current_stream(self.dev).wait_event(self.ready)
+
+
+def _cuda_device(dev):
+    """`dev` (a torch.device, a string or None for the current device) with its CUDA index filled in."""
+    dev = torch.device(dev) if dev is not None else torch.device("cuda", torch.cuda.current_device())
+    if dev.type != "cuda":
+        raise RuntimeError(f"augment: runs on a CUDA device only (no CPU fallback), got {dev}")
+    return dev if dev.index is not None else torch.device("cuda", torch.cuda.current_device())
+
+
+def cache_layout(shapes_hw, sampler):
+    """FrameCache's arena for sources of (h0, w0) `shapes_hw`: each image at load_image's size for `sampler`'s target,
+    img_size and H x W, packed BGR HWC back to back.  Returns (load sizes int64 [n, 2], byte offsets int64 [n], total
+    bytes) -- the exact count, not cal_cache_occupy's estimate from 32 images."""
+    shapes = np.asarray(shapes_hw, dtype=np.int64).reshape(-1, 2)
+    loaded = np.array([sampler.load_shape(int(h0), int(w0), sampler.H, sampler.W) for h0, w0 in shapes],
+                      dtype=np.int64).reshape(-1, 2)
+    bad = np.flatnonzero((shapes < 1).any(1) | (loaded < 1).any(1))
+    if len(bad):
+        i = int(bad[0])
+        raise RuntimeError(f"FrameCache: image {i} of {shapes[i][0]} x {shapes[i][1]} loads at {loaded[i][0]} x {loaded[i][1]}")
+    size = loaded[:, 0] * loaded[:, 1] * 3
+    offsets = np.zeros(len(shapes), dtype=np.int64)
+    offsets[1:] = np.cumsum(size)[:-1]
+    return loaded, offsets, int(size.sum())
+
+
+class FrameCache:
+    """--cache-ram on the device: every training image as load_image returns it with augment=True (datasets.py:106-160,
+    257-269), so later epochs neither decode nor resize again.
+
+        cache = FrameCache(shapes_hw, feed.sampler, max_bytes)     # RuntimeError when the images need more than max_bytes
+        feed = AugmentFeed(..., cache=cache)
+        for each batch of the first epoch:
+            plan = feed.draw(indices)
+            new = {i: decode(i) for i in plan.sources if not cache.cached[i]}
+            cache.put(new)                                         # resized into the cache on its own stream
+            feed.submit(plan, {}, labels)                          # every source now comes from the cache
+
+    `shapes_hw` are the (h0, w0) of the decoded images in dataset order; `sampler` (the feed's) fixes the target, img_size
+    and H x W, and so each image's load size (`cache_layout`).  The images live packed BGR HWC in one device arena of
+    exactly `nbytes`.  A feed built with another geometry refuses the cache.  Every rank of a DDP job holds the whole
+    dataset, as the reference's does: a mosaic draws any index.  The cache never draws from `random` / `np.random`."""
+
+    def __init__(self, shapes_hw, sampler, max_bytes, device=None):
+        self.shapes_hw = np.asarray(shapes_hw, dtype=np.int64).reshape(-1, 2)
+        if len(self.shapes_hw) != sampler.n:
+            raise RuntimeError(f"FrameCache: {len(self.shapes_hw)} shapes for a sampler of {sampler.n} images")
+        self.geometry = sampler.geometry()
+        self.loaded, self.offsets, self.nbytes = cache_layout(self.shapes_hw, sampler)
+        if self.nbytes > max_bytes:
+            raise RuntimeError(f"FrameCache: the {len(self.shapes_hw)} images need {self.nbytes} bytes at their load sizes, "
+                               f"max_bytes is {int(max_bytes)}; train from frames instead")
+        self.dev = _cuda_device(device)
+        self.arena = torch.empty(max(self.nbytes, 1), dtype=torch.uint8, device=self.dev)
+        self.cached = np.zeros(len(self.shapes_hw), dtype=bool)
+        self.stream = torch.cuda.Stream(device=self.dev)
+        self.filled = None                 # event recorded after the last fill
+        self._held = []                    # (fill event, device frames it reads)
+
+    def source(self, i):
+        """Source of cached image i: a BGR HWC record at its load size, labelled with its decoded (h0, w0)."""
+        (h0, w0), (h, w) = self.shapes_hw[i], self.loaded[i]
+        return Source(None, False, int(h0), int(w0), int(h), int(w), self.arena.data_ptr() + int(self.offsets[i]), int(w) * 3, 0,
+                      _lib.LB_BGR_HWC)
+
+    def put(self, frames, layout="bgr_hwc", ready=None):
+        """Resize {index: frame} into the cache (host frames or uint8 CUDA tensors on the cache's device, `layout` as for
+        AugmentFeed.submit) on the cache's own stream.  Device frames are read after the work enqueued on the current
+        stream before the call, or after the event `ready`; they may be dropped right after the call.  RuntimeError
+        before anything is written or enqueued when an index is out of range or already cached, or a frame is unusable
+        or differs in size from its shapes_hw entry."""
+        srcs = {}
+        for i, im in frames.items():
+            i = int(i)
+            if not 0 <= i < len(self.shapes_hw):
+                raise RuntimeError(f"FrameCache: index {i} outside the {len(self.shapes_hw)} images")
+            if self.cached[i] or i in srcs:
+                raise RuntimeError(f"FrameCache: image {i} is already cached")
+            try:
+                s = as_source(check_frame(im, layout, self.dev), layout)
+            except RuntimeError as e:
+                raise RuntimeError(f"FrameCache: image {i}: {e}") from None
+            if (s.h0, s.w0) != tuple(int(v) for v in self.shapes_hw[i]):
+                raise RuntimeError(f"FrameCache: image {i} is {s.h0} x {s.w0}, its entry in shapes_hw says "
+                                   f"{self.shapes_hw[i][0]} x {self.shapes_hw[i][1]}")
+            srcs[i] = s
+        if not srcs:
+            return
+        J = len(srcs)
+        head = J * (REC + JOB * 8)
+        used = sum(s.t.numel() for s in srcs.values() if s.staged)
+        host = torch.empty(head + used, dtype=torch.uint8, pin_memory=True)
+        jobs, recs, off = [], [], head
+        for i, s in srcs.items():
+            if s.staged:
+                host[off:off + s.t.numel()].copy_(s.t.view(-1))
+            jobs.append([0, s.ph, s.pw, int(self.offsets[i]), int(self.loaded[i][0]), int(self.loaded[i][1]), 0, 0])
+            recs.append((s.staged, off if s.staged else s.base, s.row_pitch, s.plane_pitch, s.layout))
+            off += s.t.numel() if s.staged else 0
+        devs = [s.t for s in srcs.values() if not s.staged]
+        cur = torch.cuda.current_stream(self.dev)
+        with torch.cuda.stream(self.stream):
+            buf = torch.empty(head + used, dtype=torch.uint8, device=self.dev)     # freed in this stream's order
+            table = frame_records(recs, buf.data_ptr())
+            C.memmove(host.data_ptr(), table, C.sizeof(table))
+            host[J * REC:head].view(torch.int64).copy_(torch.tensor(jobs, dtype=torch.int64).view(-1))
+            buf.copy_(host, non_blocking=True)     # the pinned block is reused only after this copy (torch's host allocator)
+            if devs:
+                if ready is not None:
+                    self.stream.wait_event(ready)
+                else:
+                    self.stream.wait_stream(cur)
+            resize_frames_launch(self.dev, buf.data_ptr(), buf.data_ptr() + J * REC, J, max(j[4] * j[5] for j in jobs),
+                                 self.arena.data_ptr(), self.stream)
+            filled = torch.cuda.Event()
+            filled.record(self.stream)
+        self.cached[list(srcs)] = True
+        self.filled = filled
+        # the caller may drop its device frames: hold them until the fill that reads them is done
+        self._held = [(e, t) for e, t in self._held if not e.query()] + ([(filled, devs)] if devs else [])

@@ -2,6 +2,8 @@
 // whole batch in two launches:
 //   yv6_aug_resize: load_image's cv2.resize INTER_LINEAR (datasets.py:287-295) of every source, and (second launch) the
 //                   letterbox branch's resize of those results (data_augment.py:52-53);
+//   yv6_aug_resize_frames: the same resize from frames anywhere in device memory (yv6_lb_src records: a decoder's
+//                   output, a crop view, the device frame cache), into packed BGR HWC in the arena;
 //   yv6_augment:    mosaic / letterbox canvas + random_affine's cv2.warpAffine, mixup, augment_hsv, flips, HWC BGR ->
 //                   CHW RGB, written straight into the training input.
 //
@@ -16,6 +18,7 @@
 // 1), times 255, truncated.  Every float / double operation is an explicit intrinsic, so ptxas cannot contract it
 // (the two fmas are OpenCV's own).
 #include "yv6_common.cuh"
+#include "yv6_frame_src.cuh"
 #include "yv6_handle.h"
 #include "yv6_resize.cuh"
 
@@ -23,27 +26,34 @@ namespace yv6 {
 
 constexpr int kAugPix = 16;     // output pixels per thread: one 16-byte store into each channel plane
 
-__global__ void __launch_bounds__(256) aug_resize_kernel(uint8_t* __restrict__ base, const int64_t* __restrict__ jobs) {
+// Job j resizes its source to nh x nw packed BGR HWC at base + dst_off.  The source is read through srcs[j]
+// (yv6_aug_resize_frames: any frame in device memory, either layout) or, when srcs is null, as packed BGR HWC at
+// base + src_off (yv6_aug_resize): only the address of a tap depends on the record.
+__global__ void __launch_bounds__(256) aug_resize_kernel(const yv6_lb_src* __restrict__ srcs, uint8_t* __restrict__ base,
+                                                         const int64_t* __restrict__ jobs) {
   const int64_t* j = jobs + (int64_t)blockIdx.y * YV6_AUG_JOB;
   const int64_t src_off = j[0], dst_off = j[3];
   const int h0 = (int)j[1], w0 = (int)j[2], nh = (int)j[4], nw = (int)j[5];
-  const uint8_t* im = base + src_off;
+  int64_t row_pitch, ch[3];
+  int px;
+  const uint8_t* im = frame_source(srcs, blockIdx.y, srcs ? nullptr : base + src_off, w0, row_pitch, px, ch);
   uint8_t* out = base + dst_off;
   const double sy = lin_scale(nh, h0), sx = lin_scale(nw, w0);
   for (int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; p < (int64_t)nh * nw; p += (int64_t)gridDim.x * blockDim.x) {
     const int y = (int)(p / nw), x = (int)(p - (int64_t)y * nw);
     uint8_t* o = out + p * 3;
-    if (nh == h0 && nw == w0) {                // cv2.resize to the same size copies
-      const uint8_t* s = im + p * 3;
-      o[0] = s[0], o[1] = s[1], o[2] = s[2];
+    if (nh == h0 && nw == w0) {                // cv2.resize to the same size copies (and here converts the layout)
+      const uint8_t* s = im + (int64_t)y * row_pitch + (int64_t)x * px;
+#pragma unroll
+      for (int c = 0; c < 3; ++c) o[c] = __ldg(s + ch[2 - c]);     // output channel c (B, G, R) is canvas channel 2 - c
       continue;
     }
     const LinTap v = lin_tap(y, sy, h0, false);
     const LinTap hz = lin_tap(x, sx, w0, true);
-    const uint8_t* r0 = im + (int64_t)v.s0 * w0 * 3;
-    const uint8_t* r1 = im + (int64_t)v.s1 * w0 * 3;
+    const uint8_t* r0 = im + (int64_t)v.s0 * row_pitch;
+    const uint8_t* r1 = im + (int64_t)v.s1 * row_pitch;
 #pragma unroll
-    for (int c = 0; c < 3; ++c) o[c] = lin_pixel(r0, r1, v, hz, c);
+    for (int c = 0; c < 3; ++c) o[c] = lin_pixel(r0 + ch[2 - c], r1 + ch[2 - c], v, hz, 0, px);
   }
 }
 
@@ -150,15 +160,26 @@ __global__ void __launch_bounds__(128) augment_kernel(const uint8_t* __restrict_
 
 using namespace yv6;
 
-extern "C" int yv6_aug_resize(yv6_handle* h, uint8_t* base, const int64_t* jobs, int32_t J, int64_t max_pix, void* stream) {
-  yv6_device_guard _dev(h);
-  YV6_REQUIRE(h && base && jobs && J >= 0 && max_pix >= 0, "aug_resize: bad argument");
+static int launch_aug_resize(const yv6_lb_src* srcs, uint8_t* base, const int64_t* jobs, int32_t J, int64_t max_pix, void* stream) {
   YV6_REQUIRE(J <= 65535, "aug_resize: %d jobs exceed one launch", J);
   if (J == 0 || max_pix == 0) return YV6_OK;
   const int64_t blocks = (max_pix + 255) / 256;
-  aug_resize_kernel<<<dim3((unsigned)(blocks < 1024 ? blocks : 1024), J), 256, 0, (cudaStream_t)stream>>>(base, jobs);
+  aug_resize_kernel<<<dim3((unsigned)(blocks < 1024 ? blocks : 1024), J), 256, 0, (cudaStream_t)stream>>>(srcs, base, jobs);
   YV6_CHECK_CUDA(cudaGetLastError());
   return YV6_OK;
+}
+
+extern "C" int yv6_aug_resize(yv6_handle* h, uint8_t* base, const int64_t* jobs, int32_t J, int64_t max_pix, void* stream) {
+  yv6_device_guard _dev(h);
+  YV6_REQUIRE(h && base && jobs && J >= 0 && max_pix >= 0, "aug_resize: bad argument");
+  return launch_aug_resize(nullptr, base, jobs, J, max_pix, stream);
+}
+
+extern "C" int yv6_aug_resize_frames(yv6_handle* h, const yv6_lb_src* srcs, const int64_t* jobs, int32_t J, int64_t max_pix,
+                                     uint8_t* base, void* stream) {
+  yv6_device_guard _dev(h);
+  YV6_REQUIRE(h && srcs && base && jobs && J >= 0 && max_pix >= 0, "aug_resize_frames: bad argument");
+  return launch_aug_resize(srcs, base, jobs, J, max_pix, stream);
 }
 
 extern "C" int yv6_augment(yv6_handle* h, const uint8_t* base, const yv6_aug_sample* samples, int32_t B, int32_t H, int32_t W, uint8_t* dst,

@@ -21,33 +21,13 @@
 // wrong on upscaling shapes.  Every float / double operation is an explicit round-to-nearest intrinsic, so ptxas cannot
 // contract it into an FMA.
 #include "yv6_common.cuh"
+#include "yv6_frame_src.cuh"
 #include "yv6_handle.h"
 #include "yv6_resize.cuh"
 
 namespace yv6 {
 
 constexpr int kLbPix = 16;     // output pixels per thread: one 16-byte store into each channel plane
-
-// Where image b lies: srcs[b] (yv6_letterbox_frames, yv6_letterbox_val) or, when srcs is null, packed BGR HWC at
-// packed + src_off (yv6_letterbox).  Canvas channel c (R, G, B) of pixel x lies at row + x * px + ch[c]: BGR HWC reads
-// channel 2 - c, RGB CHW plane c.
-__device__ __forceinline__ const uint8_t* lb_source(const yv6_lb_src* srcs, const uint8_t* packed, const int32_t* g, int b, int w0,
-                                                    int64_t& row_pitch, int& px, int64_t (&ch)[3]) {
-  const uint8_t* im;
-  int64_t plane_pitch;
-  int layout;
-  if (srcs) {
-    const yv6_lb_src s = srcs[b];
-    im = s.base, row_pitch = s.row_pitch, plane_pitch = s.plane_pitch, layout = s.layout;
-  } else {
-    im = packed + __ldg(g + 0), row_pitch = (int64_t)w0 * 3, plane_pitch = 0, layout = YV6_LB_BGR_HWC;
-  }
-  const bool chw = layout == YV6_LB_RGB_CHW;
-  px = chw ? 1 : 3;
-#pragma unroll
-  for (int c = 0; c < 3; ++c) ch[c] = chw ? c * plane_pitch : 2 - c;
-  return im;
-}
 
 // geo [B][YV6_LB_GEO] = (src_off, h0, w0, nh, nw, top, left, 0); thread = 16 consecutive pixels of one canvas row.
 // Image b is read through srcs[b] (yv6_letterbox_frames) or, when srcs is null, as packed BGR HWC at packed + src_off
@@ -63,7 +43,7 @@ __global__ void __launch_bounds__(256) letterbox_kernel(const yv6_lb_src* __rest
   const int h0 = __ldg(g + 1), w0 = __ldg(g + 2), nh = __ldg(g + 3), nw = __ldg(g + 4), top = __ldg(g + 5), left = __ldg(g + 6);
   int64_t row_pitch, ch[3];
   int px;
-  const uint8_t* im = lb_source(srcs, packed, g, b, w0, row_pitch, px, ch);
+  const uint8_t* im = frame_source(srcs, b, srcs ? nullptr : packed + __ldg(g + 0), w0, row_pitch, px, ch);
   alignas(16) uint8_t o[3][kLbPix];
   const int ys = y - top;
   if (ys < 0 || ys >= nh) {
@@ -165,7 +145,7 @@ __global__ void __launch_bounds__(256) letterbox_val_kernel(const yv6_lb_src* __
   if (ys >= 0 && ys < nh) {
     int64_t row_pitch, ch[3];
     int px;
-    const uint8_t* im = lb_source(srcs, nullptr, g, b, w0, row_pitch, px, ch);
+    const uint8_t* im = frame_source(srcs, b, nullptr, w0, row_pitch, px, ch);
     const int xa = left - x0, xb = left + nw - x0;      // canvas pixels x0 + [xa, xb) hold the image
     if (mode == YV6_VAL_COPY) {
       const uint8_t* row = im + (int64_t)ys * row_pitch;

@@ -81,18 +81,6 @@ def common_canvas(srcs, H, W, scaleup, stride):
     return canvas
 
 
-def as_frame(im):
-    """uint8 HWC 3-channel host image (numpy array or CPU tensor) -> contiguous uint8 CPU tensor; RuntimeError otherwise."""
-    t = torch.from_numpy(np.ascontiguousarray(im)) if isinstance(im, np.ndarray) else im
-    if not isinstance(t, torch.Tensor) or t.device.type != "cpu":
-        raise RuntimeError(f"letterbox: frames must be host numpy arrays or CPU tensors, got {type(im).__name__}")
-    if t.dtype != torch.uint8:
-        raise RuntimeError(f"letterbox: frames must be uint8, got {t.dtype}")
-    if t.dim() != 3 or t.shape[2] != 3 or t.shape[0] < 1 or t.shape[1] < 1:
-        raise RuntimeError(f"letterbox: frames must be HWC with 3 channels (BGR), got shape {tuple(t.shape)}")
-    return t.contiguous()
-
-
 class LetterboxMeta:
     """Per-image metadata of a letterboxed batch.
     geo: int32 [B, GEO] host table (the device copy is what the kernels read); n: number of real images (slots beyond n are
@@ -126,26 +114,29 @@ def source_pitches(shape, strides, layout):
     return int(h0), int(w0), int(strides[0] if hwc else strides[1]), 0 if hwc else int(strides[0])
 
 
+def check_frame(im, layout, dev):
+    """Validate one frame in `layout`; nothing is copied or enqueued.  A frame is a host numpy array or CPU tensor (staged:
+    returned as a contiguous CPU tensor) or a uint8 tensor on `dev` (read in place).  Returns (tensor, on_device, h0, w0,
+    row_pitch, plane_pitch); RuntimeError when the frame is unusable."""
+    t = torch.from_numpy(np.ascontiguousarray(im)) if isinstance(im, np.ndarray) else im
+    if not isinstance(t, torch.Tensor):
+        raise RuntimeError(f"letterbox: frames must be numpy arrays or tensors, got {type(im).__name__}")
+    on_dev = t.device.type != "cpu"
+    if on_dev and t.device != dev:
+        raise RuntimeError(f"letterbox: a frame on {t.device}, the pipeline runs on {dev}")
+    if t.dtype != torch.uint8:
+        raise RuntimeError(f"letterbox: frames must be uint8, got {t.dtype}")
+    if not on_dev:
+        t = t.contiguous()
+    return (t, on_dev) + source_pitches(tuple(t.shape), t.stride(), layout)
+
+
 def check_frames(frames, B, layout, dev):
-    """Validate 1..B frames for one letterbox launch; nothing is copied or enqueued.  A frame is a host numpy array or CPU
-    tensor (staged: returned as a contiguous CPU tensor) or a uint8 tensor on `dev` (read in place).  Returns one
+    """Validate 1..B frames for one letterbox launch (`check_frame` each); nothing is copied or enqueued.  Returns one
     (tensor, on_device, h0, w0, row_pitch, plane_pitch) per frame; RuntimeError when any frame is unusable."""
     if not 1 <= len(frames) <= B:
         raise RuntimeError(f"letterbox: {len(frames)} frames for a batch of {B}")
-    out = []
-    for im in frames:
-        t = torch.from_numpy(np.ascontiguousarray(im)) if isinstance(im, np.ndarray) else im
-        if not isinstance(t, torch.Tensor):
-            raise RuntimeError(f"letterbox: frames must be numpy arrays or tensors, got {type(im).__name__}")
-        on_dev = t.device.type != "cpu"
-        if on_dev and t.device != dev:
-            raise RuntimeError(f"letterbox: a frame on {t.device}, the pipeline runs on {dev}")
-        if t.dtype != torch.uint8:
-            raise RuntimeError(f"letterbox: frames must be uint8, got {t.dtype}")
-        if not on_dev:
-            t = t.contiguous()
-        out.append((t, on_dev) + source_pitches(tuple(t.shape), t.stride(), layout))
-    return out
+    return [check_frame(im, layout, dev) for im in frames]
 
 
 def pack_sources(srcs, B, H, W, scaleup, layout, src_host, geo_host, rec_host, src_dev_ptr, auto=False, stride=32, canvas=None):
