@@ -690,6 +690,56 @@ int yv6_xform(yv6_handle* h, const yv6_xform_seg* segs_dev, const int32_t* chunk
 int yv6_sgd_ema_step(yv6_handle* h, float* param, const float* grad, float* momentum_buf, float* ema_or_null,
                      const uint8_t* group_per4, int64_t n, const float* hyper_dev, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Inference weight fold (yolov6_b200/refold.py): the train-form state in one flat fp32 buffer (flat.FlatState layout, or
+ * a state_dict staged that way) -> every weight tensor of an inference engine, in place, bit for bit what fold.py's float64
+ * fold and the engine's casts give on the host.  Two phases over records built on the host once per (engine, layout):
+ *   channel phase: one yv6_fold_chan per op: the BatchNorm affine(s) of its branches in float64 -> coef[5 per channel] =
+ *                  (A: main weight scale, B: 1x1 branch scale, D: identity term, P: post-sum scale, folded bias);
+ *   element phase: one yv6_fold_rec per destination region: value(o, r, s, c) in float64, then cast to the region's format.
+ * Every float64 operation is an explicit round-to-nearest intrinsic in fold.py's order (no FMA contraction).
+ * ---------------------------------------------------------------------------------------------- */
+#define YV6_FOLD_CHUNK 4096
+enum { YV6_FOLD_C_DP = 0, YV6_FOLD_C_REP = 1, YV6_FOLD_C_QA = 2, YV6_FOLD_C_BN = 3, YV6_FOLD_C_BIAS = 4 };
+/* element layouts: W: w * A; W_REP: w3 * A + (center ? w1 * B : 0) (+ D on the identity diagonal's center); W_QA:
+ * ((w3 * A + (center ? w1 : 0)) (+ 1 on the diagonal's center) (+ 1/9 on the diagonal if avg)) * P; W_COPY: w; W_CONVT:
+ * w[c][o][r0][s0] of a [Cin][Cout][2][2] ConvTranspose weight; BIAS: the folded bias of channel o; COPY: flat element o. */
+enum { YV6_FOLD_W = 0, YV6_FOLD_W_REP = 1, YV6_FOLD_W_QA = 2, YV6_FOLD_W_COPY = 3, YV6_FOLD_W_CONVT = 4, YV6_FOLD_BIAS = 5,
+       YV6_FOLD_COPY = 6 };
+/* formats: fp32 (float64 -> fp32), bf16 (-> fp32 -> bf16), fp16 (-> fp32 -> fp16, as torch casts float64), split3 (-> fp32 ->
+ * three bf16 planes hi / mid / lo, `plane_stride` elements apart, residuals in fp32) */
+enum { YV6_FOLD_F32 = 0, YV6_FOLD_BF16 = 1, YV6_FOLD_F16 = 2, YV6_FOLD_SPLIT3 = 3 };
+enum { YV6_FOLD_IDENTITY = 1, YV6_FOLD_AVG = 2 };
+typedef struct yv6_fold_chan {
+  int64_t bn[3][4];            /* flat offsets of (weight, bias, running_mean, running_var) of the op's BatchNorms at its first
+                                  channel, -1: absent.  C_DP / C_BN: [0]; C_REP: dense, 1x1, identity; C_QA: dense, post-sum */
+  int64_t b;                   /* flat offset of the conv bias (C_DP, C_BIAS), -1: absent */
+  int64_t coef;                /* first coefficient of channel 0 (5 doubles per channel) */
+  int32_t layout, n;           /* YV6_FOLD_C_*, channels */
+} yv6_fold_chan;
+typedef struct yv6_fold_rec {
+  void* dst;                   /* destination element of domain point 0 */
+  int64_t plane_stride;        /* split3: elements between the planes */
+  int64_t ds[4];               /* destination strides (elements) of the domain axes (o, r, s, c) */
+  int64_t w, w1;               /* flat offsets of the op's weight at its first output channel and of the rep / qa 1x1 weight, -1: absent */
+  int64_t coef;                /* first coefficient of channel 0 */
+  int64_t blk0;                /* first block of the element phase working on this record (records in increasing blk0) */
+  int32_t n[4];                /* domain: output channels, tap rows, tap columns, input channels */
+  int32_t layout, fmt;         /* YV6_FOLD_W*, YV6_FOLD_F* */
+  int32_t k, cin;              /* the weight's kernel size and input channels (per group) */
+  int32_t r0, s0;              /* tap of domain point (r, s) = 0 (column-pair view columns, ConvTranspose quadrant) */
+  int32_t cout;                /* W_CONVT: the weight's output channels */
+  int32_t flags;               /* YV6_FOLD_IDENTITY | YV6_FOLD_AVG */
+  int32_t check;               /* fp16 range check slot, -1: none */
+  int32_t reserved0;
+} yv6_fold_rec;
+/* Records and coef live in DEVICE memory; n_blocks = blk0 of a record past the last.  check_only == 0: both phases, every
+ * record written.  check_only == 1: the channel phase, then the element values of the records with a check slot are rounded
+ * to fp16 (through fp32) and nothing but coef and `checks` is written: checks[2 * slot] |= 1 if one is not finite,
+ * checks[2 * slot + 1] = max of the bits of |value| (the float64 max |value|); the caller zeroes `checks` first. */
+int yv6_fold(yv6_handle* h, const float* flat, const yv6_fold_chan* chans_dev, int32_t n_chans, const yv6_fold_rec* recs_dev,
+             int32_t n_recs, int64_t n_blocks, double* coef, unsigned long long* checks, int32_t check_only, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -113,6 +113,21 @@ class XformSeg(C.Structure):
     ]
 
 
+class FoldChan(C.Structure):
+    """Mirror of `yv6_fold_chan` (include/yv6.h)."""
+    _fields_ = [("bn", (C.c_int64 * 4) * 3), ("b", C.c_int64), ("coef", C.c_int64), ("layout", C.c_int32), ("n", C.c_int32)]
+
+
+class FoldRec(C.Structure):
+    """Mirror of `yv6_fold_rec` (include/yv6.h)."""
+    _fields_ = [
+        ("dst", C.c_void_p), ("plane_stride", C.c_int64), ("ds", C.c_int64 * 4), ("w", C.c_int64), ("w1", C.c_int64),
+        ("coef", C.c_int64), ("blk0", C.c_int64), ("n", C.c_int32 * 4), ("layout", C.c_int32), ("fmt", C.c_int32),
+        ("k", C.c_int32), ("cin", C.c_int32), ("r0", C.c_int32), ("s0", C.c_int32), ("cout", C.c_int32), ("flags", C.c_int32),
+        ("check", C.c_int32), ("reserved0", C.c_int32),
+    ]
+
+
 class PrState(C.Structure):
     """Mirror of `yv6_pr_state` (include/yv6.h)."""
     _fields_ = [
@@ -178,6 +193,11 @@ LB_BGR_HWC, LB_RGB_CHW = 0, 1
 VAL_COPY, VAL_LINEAR, VAL_AREA, VAL_AREA_FAST = 0, 1, 2, 3      # yv6_letterbox_val's per-image modes (geo[7])
 XF_F32, XF_F64, XF_BF16 = 0, 1, 2
 XFORM_CHUNK = 4096
+FOLD_C_DP, FOLD_C_REP, FOLD_C_QA, FOLD_C_BN, FOLD_C_BIAS = 0, 1, 2, 3, 4
+FOLD_W, FOLD_W_REP, FOLD_W_QA, FOLD_W_COPY, FOLD_W_CONVT, FOLD_BIAS, FOLD_COPY = 0, 1, 2, 3, 4, 5, 6
+FOLD_F32, FOLD_BF16, FOLD_F16, FOLD_SPLIT3 = 0, 1, 2, 3
+FOLD_IDENTITY, FOLD_AVG = 1, 2
+FOLD_CHUNK = 4096
 
 
 _lib = None
@@ -258,6 +278,8 @@ _SIGNATURES = {
     "yv6_xform": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p]),
     "yv6_sgd_ema_step": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
                                    C.c_void_p, C.c_void_p]),
+    "yv6_fold": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int64, C.c_void_p, C.c_void_p,
+                           C.c_int32, C.c_void_p]),
     "yv6_pr_workspace_bytes": (C.c_int64, [C.c_int32, C.c_int32]),
     "yv6_pr_match": (C.c_int, [C.c_void_p, C.POINTER(PrState), C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32,
                                C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p]),

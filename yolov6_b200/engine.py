@@ -2,7 +2,8 @@
 
 What the reference does with nested nn.Module.forward calls, cuDNN and ~15 eager ops for the head
 decode (Model.forward yolo.py:33-41, Detect.forward effidehead.py:93-139), this does with:
-  * folded deploy-form weights (fold.py) packed once to KRSC bf16 (or three bf16 planes),
+  * folded deploy-form weights (fold.py's float64 fold, run on the device by yv6_fold: refold.py) packed to KRSC bf16 (or
+    three bf16 planes), refoldable in place from new train-form weights (InferEngine.refold),
   * pre-allocated NHWC activation buffers (concats are channel slices),
   * a prepared list of C-ABI descriptors per input shape, replayed per batch -- optionally as one
     captured CUDA graph (no Python / launch overhead in steady state).
@@ -17,9 +18,8 @@ from dataclasses import dataclass
 
 import torch
 
-from . import _lib, ops
+from . import _lib, ops, refold
 from ._lib import ConvDesc
-from .fold import fold_op, se_weights, to_f16
 
 
 def siblings(g):
@@ -290,48 +290,108 @@ class InferEngine:
 
     # ------------------------------------------------------------------ weight packing
     def _pack(self, sd):
-        sd = {k: v.detach().cpu() for k, v in sd.items()}
-        dev = self.device
-
-        def planes(w, name):  # KRSC weights in the precision's operand layout (folded in fp64, rounded once)
-            if self.f16:
-                return to_f16(w, name).contiguous().to(dev)
-            w = w.float().to(dev)
-            return ops.split3(w).contiguous() if self.nsplit == 3 else w.to(torch.bfloat16).contiguous()
-
+        """Allocate the weight tensors (zeroed) and fold the state_dict sd into them: staged into one flat buffer on the
+        engine's device and folded by yv6_fold (refold.py), then synchronized, as an upload would be."""
         self.sibling = siblings(self.g)
-        for i, op in enumerate(self.g.ops):
-            if op.kind in ("pool", "shuffle", "up") or (op.kind == "pred" and op.head[0] not in ("cls", "reg")):   # fuse_ab / distillation preds: training only
-                continue
-            if op.kind == "se":
-                self.weights[i] = dict(zip(("w1", "b1", "w2", "b2"), (t.float().contiguous().to(dev) for t in se_weights(sd, op))))
-                continue
-            w, b = fold_op(sd, op)
-            ent = {}
-            if op.kind == "stem":
-                cp = stem_channels(self.g, op)
-                w, b = torch.cat([w, w.new_zeros((cp - op.cout,) + w.shape[1:])]), torch.cat([b, b.new_zeros(cp - op.cout)])
-                if self.f16:                   # the stem kernel rounds its fp32 weights to fp16
-                    to_f16(w, op.name)
-                ent["w_dev"] = w.float().permute(1, 2, 3, 0).contiguous().to(dev)       # [3][3][3][Cout]
-                ent["b_dev"] = b.float().contiguous().to(dev)
-            elif op.kind == "dw":
-                # fp32 [k*k][C]: the exact folded weights serve both precision modes and cost k*k*C*4 bytes per launch
-                ent["w_dev"] = w[..., 0].permute(1, 2, 0).reshape(op.k * op.k, op.cin).float().contiguous().to(dev)
-                ent["b_dev"] = b.float().contiguous().to(dev)
-            else:
-                w = w if op.kind == "convT" else window_weights(self.g, op, w)
-                ws = w if isinstance(w, list) else [w]
-                ent["w"] = [planes(wi, op.name) for wi in ws]
-                if pair_view_candidate(op):      # [Cout][3][2][2*Cin] weights of the column-pair view (see pair_view)
-                    ent["w_pair"] = planes(ops.pair_view_weights(ws[0]), op.name)
-                ent["bias"] = ops.pad_bias(b.to(dev), op.cout)
-            ent["alpha"] = float(sd[op.alpha]) if (op.alpha and op.res is not None) else 1.0
+        for i, ent in refold.allocate(self.g, self.precision, self.device).items():
+            op = self.g.ops[i]
+            if op.kind != "se":
+                ent["alpha"] = float(sd[op.alpha]) if (op.alpha and op.res is not None) else 1.0
             self.weights[i] = ent
-        for i, j in self.sibling.items():      # one conv with 2 x Cout output channels: [cls branch | reg branch]
-            (wa, ba), (wb, bb) = fold_op(sd, self.g.ops[i]), fold_op(sd, self.g.ops[j])
-            self.weights[i]["w_fused"] = planes(torch.cat([wa, wb], 0), self.g.ops[i].name)
-            self.weights[i]["bias_fused"] = ops.pad_bias(torch.cat([ba, bb]).to(dev), 2 * self.g.ops[i].cout)
+        flat, slots = refold.stage(sd, self.device)
+        self._fold(flat, slots)
+        if self.device.type == "cuda":
+            torch.cuda.current_stream(self.device).synchronize()
+            self._fold_ev = None
+
+    def _resolve(self, dst):
+        t = self.weights[dst[1]][dst[0]]
+        return t[dst[2]] if dst[0] == "w" else t
+
+    def _fold_plan(self, slots):
+        plans = self.__dict__.setdefault("_fold_plans", {})
+        key = refold.layout_key(self.g, slots)
+        plan = plans.get(key)
+        if plan is None:
+            plan = plans[key] = refold.build_plan(self.g, self.precision, slots)
+        return plan
+
+    def _fold(self, flat, slots, stream=None):
+        """Fold the state in flat (laid out as slots) into the weight tensors.  On the CUDA device the fold is enqueued on
+        `stream` (default: the current stream) after the work already enqueued on the current stream, the batches in flight on
+        the pipelines attached to this engine and the previous fold; fp16 runs the range check first (one host sync)."""
+        plan = self._fold_plan(slots)
+        if self.device.type != "cuda":          # a CPU-device engine (planner tests): the same records, executed on the host
+            refold.replay_host(plan, flat, self._resolve)
+            return
+        if flat.device != self.device or flat.dtype != torch.float32 or not flat.is_contiguous():
+            raise ValueError(f"refold: the source must be a contiguous fp32 tensor on {self.device}")
+        tables = plan.dev.get(id(self))
+        if tables is None:
+            tables = plan.dev[id(self)] = refold.device_tables(plan, self._resolve, self.device)
+        cur = torch.cuda.current_stream(self.device)
+        s = stream if stream is not None else cur
+        if s != cur:
+            s.wait_stream(cur)
+        for x in self._in_flight():
+            if isinstance(x, torch.cuda.Event):
+                s.wait_event(x)
+            else:
+                s.wait_stream(x)
+        if self.__dict__.get("_fold_ev") is not None:
+            s.wait_event(self._fold_ev)
+        if self.f16:
+            refold.device_check(self.lib, self.handle, plan, tables, flat, s)
+        refold.launch(self.lib, self.handle, tables, flat, False, s)
+        self._fold_ev = torch.cuda.Event()
+        self._fold_ev.record(s)
+        if s != cur:                      # the caching allocator must not recycle the source before the fold has read it
+            flat.record_stream(s)
+        self._fold_src = flat
+
+    def _in_flight(self):
+        """Events (or streams) of the batches in flight on the pipelines attached to this engine (pipeline.in_flight)."""
+        out = []
+        for p in list(self.__dict__.get("_users", ())):
+            out += p.in_flight()
+        return out
+
+    def attach(self, pipeline):
+        """Register a pipeline whose captured graphs run this engine: refold orders itself after its batches in flight, and
+        the pipeline calls after_fold before each launch."""
+        import weakref
+        self.__dict__.setdefault("_users", weakref.WeakSet()).add(pipeline)
+
+    def after_fold(self, stream):
+        """Make `stream` wait for the last refold (nothing to do if the engine was never refolded)."""
+        ev = self.__dict__.get("_fold_ev")
+        if ev is not None:
+            stream.wait_event(ev)
+
+    def refold(self, src, slots, stream=None):
+        """Rewrite the weights of this engine in place from the train-form state in the flat fp32 CUDA tensor `src`, laid out
+        as `slots` ({name: (offset, numel, shape)}: FlatState.slots, or refold.stage of a state_dict).  Every plan, launch
+        record and captured CUDA graph of the engine stays valid and runs the new weights.
+
+        Stream order: the fold runs on `stream` (default: the current stream) after the work already enqueued on the current
+        stream -- so after the last FusedSGDEMA step there when src is its `ema` -- and after the batches in flight on the
+        pipelines built on this engine (the done events of their batch slots, or the stream a DetectPipeline without
+        overlap_h2d last launched on); their next launch(), and the next eager forward, wait for it.  The source must not be
+        overwritten until then (the engine keeps a reference).
+
+        Raises refold.AlphaChanged (a ValueError) before anything is written when a BottleRep alpha of src differs from the one
+        the engine was built with (it is baked into the conv descriptors), and in the fp16 mode fold.to_f16's ValueError, also
+        before anything is written, when a folded weight is outside fp16's range."""
+        if self.device.type != "cuda" or src.device != self.device:
+            raise ValueError(f"refold: the source must be a CUDA tensor on {self.device}")
+        alphas = [(i, op.alpha) for i, op in enumerate(self.g.ops) if op.alpha and op.res is not None and i in self.weights]
+        if alphas:
+            idx = torch.tensor([slots[a][0] for _, a in alphas], dtype=torch.int64, device=self.device)
+            for (i, a), v in zip(alphas, src.index_select(0, idx).tolist()):
+                if v != self.weights[i]["alpha"]:
+                    raise refold.AlphaChanged(f"refold: {a} is {v!r}, the engine was built with {self.weights[i]['alpha']!r}; "
+                                              "rebuild the engine (alpha is baked into its conv descriptors)")
+        self._fold(src, slots, stream)
 
     # ------------------------------------------------------------------ per-shape plan
     def _plan(self, N, H, W, in_dtype):
@@ -478,6 +538,8 @@ class InferEngine:
         assert head_set == 0 or not decode, "the alternate head set is for decode=False callers"
         self._select_head_set(plan, head_set)
         main = stream if stream is not None else torch.cuda.current_stream(self.device)
+        if self.__dict__.get("_fold_ev") is not None and not torch.cuda.is_current_stream_capturing():
+            main.wait_event(self._fold_ev)        # eager forward after a refold (captured pipelines wait in launch())
         sp = _lib.stream_ptr(main)
         lib, h = self.lib, self.handle
         plan.stem.x = x.data_ptr()

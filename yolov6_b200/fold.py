@@ -83,9 +83,14 @@ def to_f16(w, name):
     with a tiny running variance); such a weight would become inf, so it raises ValueError naming the layer instead."""
     h = w.to(torch.float16)
     if not torch.isfinite(h).all():
-        raise ValueError(f"{name}: a folded weight ({float(w.abs().max()):.6g}) is outside fp16's finite range (+-{F16_MAX:g}); "
-                         "run this model in the bf16 or fp32 precision mode")
+        raise f16_range_error(name, float(w.abs().max()))
     return h
+
+
+def f16_range_error(name, wmax):
+    """The ValueError of a layer whose folded weights (largest magnitude wmax) do not fit fp16 (to_f16)."""
+    return ValueError(f"{name}: a folded weight ({wmax:.6g}) is outside fp16's finite range (+-{F16_MAX:g}); "
+                      "run this model in the bf16 or fp32 precision mode")
 
 
 def se_weights(sd, op):

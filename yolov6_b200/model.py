@@ -240,14 +240,45 @@ class Model(nn.Module):
         self.precision = precision
         return self
 
+    def _weights_key(self, dev):
+        return (self.precision, str(dev), sum(p._version for p in self.parameters()) +
+                sum(b._version for b in self.buffers()), self.__dict__.get("_weights_epoch", 0))
+
     def engine(self):
         dev = next(self.parameters()).device
-        key = (self.precision, str(dev), sum(p._version for p in self.parameters()) +
-               sum(b._version for b in self.buffers()), self.__dict__.get("_weights_epoch", 0))
+        key = self._weights_key(dev)
         if self._engine is None or self._engine_key != key:
             self._engine = InferEngine(self.graph, self.state_dict(), dev, self.precision)
             self._engine_key = key
         return self._engine
+
+    def load_weights_(self, src):
+        """Load new weights without rebuilding the inference engine.  src: a state_dict, a FusedSGDEMA (its EMA of a training
+        model of the same config; integer buffers from that model, as ema_state_dict) or (flat fp32 tensor, slots) in the
+        FlatState layout.  The state is copied into this model's parameters and buffers (state_dict() describes what runs),
+        then the built engine, if any, is refolded in place (InferEngine.refold: its plans and every pipeline captured on it
+        stay valid, and their next launch runs the new weights) and stays current, so engine() does not rebuild it.
+
+        Raises refold.AlphaChanged (a ValueError) when a BottleRep alpha differs from the engine's: the parameters are loaded,
+        the engine is left untouched and is rebuilt by the next engine() call (pipelines captured on it must be rebuilt)."""
+        from .refold import weight_source
+        return self._load_flat_(*weight_source(src, next(self.parameters()).device))
+
+    def _load_flat_(self, flat, slots, ints):
+        """load_weights_ from a resolved source: flat fp32 state on the model's device, its slots, integer entries."""
+        dev = next(self.parameters()).device
+        with torch.no_grad():
+            for name, t in list(self.named_parameters()) + list(self.named_buffers()):
+                if t.is_floating_point():
+                    o, n, shape = slots[name]
+                    t.copy_(flat[o:o + n].view(shape))
+                elif name in ints:
+                    t.copy_(ints[name])
+        eng = self._engine
+        if eng is not None and eng.precision == self.precision and eng.device == dev:
+            eng.refold(flat, slots)
+            self._engine_key = self._weights_key(dev)
+        return self
 
     def mark_weights_changed(self):
         """Tell the model that its parameters were rewritten through raw device pointers (yv6_sgd_ema_step): the folded

@@ -183,12 +183,21 @@ class _Served:
         self.shape = (batch, height, width, self.slots[0].x_dev.dtype)
         self.eng = engine if engine is not None else model.engine()
         self.eng.pin(*self.shape)          # the graphs point at this shape's buffers
+        self.eng.attach(self)              # a refold of the engine waits for this pipeline's batches in flight
         self.sizes = [(height // int(s), width // int(s)) for s in model.graph.strides]
         A = sum(h * w for h, w in self.sizes)
         # scratch owned by this pipeline: a shared cache could be replaced (freed) while a graph still references it
         self.nms_ws = torch.empty(workspace_bytes(batch, A, model.graph.num_classes, nms_kw["multi_label"]), dtype=torch.uint8,
                                   device=self.dev)
         self.nms = functools.partial(nms_batched_head, sizes=self.sizes, strides=model.graph.strides, workspace=self.nms_ws, **nms_kw)
+
+    def in_flight(self):
+        """What a refold of the engine must follow: the done events of the slots' last steps and, for a pipeline that does not
+        record them (DetectPipeline without overlap_h2d), the stream of its last launch."""
+        out = [sl.ev_done for sl in self.slots if sl.used]
+        if getattr(self, "launch_stream", None) is not None:
+            out.append(self.launch_stream)
+        return out
 
     def _capture(self, warm, bodies):
         """Run `warm` on a side stream (plans, tensor maps, cudaFuncSetAttribute, allocator warm-up), then capture one graph
@@ -232,11 +241,14 @@ class DetectPipeline(_Served):
         self.out_dev, self.count_dev, _ = self.slot.detect(self.nms, cls, reg)
 
     def launch(self):
-        """Enqueue one batch (input already in `x_host` / `x_dev`); asynchronous."""
+        """Enqueue one batch (input already in `x_host` / `x_dev`); asynchronous.  It runs after the last refold of the
+        engine (InferEngine.refold)."""
+        cur = torch.cuda.current_stream(self.dev)
+        self.eng.after_fold(cur)
         if not self.overlap_h2d:
             self.graph.replay()
+            self.launch_stream = cur      # a refold orders itself after this stream's work (in_flight)
             return
-        cur = torch.cuda.current_stream(self.dev)
         self.slot.h2d(self.copy_stream, cur)
         self.graph.replay()
         self.slot.done(cur)
@@ -359,11 +371,13 @@ class DetectStream(_Served):
         cur.wait_event(self.ev_join)
 
     def launch(self):
-        """Enqueue one step on the current stream (input of slot steps & 1 already in x_host / x_dev); asynchronous."""
+        """Enqueue one step on the current stream (input of slot steps & 1 already in x_host / x_dev); asynchronous.  It runs
+        after the last refold of the engine (InferEngine.refold)."""
         slot = self.slots[self.steps & 1]
         cur = torch.cuda.current_stream(self.dev)
         if self.host_input:
             slot.h2d(self.copy_stream, cur)
+        self.eng.after_fold(cur)
         self.graphs[self.steps & 1].replay()
         slot.done(cur)
         self.steps += 1
@@ -456,6 +470,19 @@ class DetectFarm:
         for ev, st in zip(self._ev, self.streams):
             ev.record(st)
             cur.wait_event(ev)
+
+    def load_weights_(self, src):
+        """Load new weights into the model and every lane, in place: Model.load_weights_ for the model (and its engine), then
+        InferEngine.refold of each lane's engine.  No graph is recaptured; each lane's next step runs after the fold of its
+        engine, and each fold after the lane's batches in flight (InferEngine.refold).  A source whose BottleRep alpha differs
+        raises refold.AlphaChanged before any lane is written."""
+        from .refold import weight_source
+        flat, slots, ints = weight_source(src, self.dev)      # staged once for the model and every lane
+        self.model._load_flat_(flat, slots, ints)
+        for lane in self.lanes:
+            if lane.eng is not self.model.__dict__.get("_engine"):
+                lane.eng.refold(flat, slots)
+        return self
 
     def release(self):
         """The lanes wait for everything enqueued on the current stream (e.g. a timing event)."""
