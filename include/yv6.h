@@ -740,6 +740,49 @@ typedef struct yv6_fold_rec {
 int yv6_fold(yv6_handle* h, const float* flat, const yv6_fold_chan* chans_dev, int32_t n_chans, const yv6_fold_rec* recs_dev,
              int32_t n_recs, int64_t n_blocks, double* coef, unsigned long long* checks, int32_t check_only, void* stream);
 
+/* ---- JPEG decode (yv6_jpeg.cu): cv2.imread's pixels of baseline / extended sequential Huffman JPEGs ----
+ * The host parses each header (yolov6_b200/jpeg.py) into one yv6_jpeg_image; one call decodes a batch of them.
+ * yv6_jpeg_huff: one Huffman table: lut[x] = length << 8 | symbol for the codes of at most 9 bits (x: the next 9 bits),
+ *   0 otherwise; maxcode[l] the largest l-bit code (-1: none, [17] a sentinel), vals[code + valoff[l]] its symbol.
+ * yv6_jpeg_comp / yv6_jpeg_image: the caller fills the fields marked (in); yv6_jpeg_workspace_bytes fills the rest. */
+typedef struct yv6_jpeg_huff {
+  uint16_t lut[512];
+  int32_t maxcode[18];
+  int32_t valoff[18];
+  uint8_t vals[256];
+} yv6_jpeg_huff;
+typedef struct yv6_jpeg_comp {
+  int32_t h, v;                /* (in) sampling factors                                                          */
+  int32_t dc, ac;              /* (in) indices of its tables in the call's yv6_jpeg_huff array                    */
+  int32_t bw, bh;              /* plane size in blocks                                                            */
+  int32_t dw, dh;              /* real samples of the plane: ceil(width * h / hmax), ceil(height * v / vmax)       */
+  int64_t plane;               /* workspace offset of the (bw * 8) x (bh * 8) uint8 sample plane                  */
+  uint16_t q[64];              /* (in) quantisation table, natural order                                         */
+} yv6_jpeg_comp;
+typedef struct yv6_jpeg_image {
+  const uint8_t* data;         /* (in) the entropy-coded segment, device memory (after SOS, up to the next non-RST marker) */
+  int64_t len;                 /* (in) its bytes                                                                  */
+  uint8_t* out;                /* (in) height x width x 3 BGR uint8 (width x height x 3 for orientations 5-8)      */
+  int32_t height, width;       /* (in) the frame as coded                                                         */
+  int32_t ncomp;               /* (in) 1 or 3                                                                    */
+  int32_t orientation;         /* (in) EXIF orientation 1..8, applied as cv2.imread does                          */
+  int32_t restart;             /* (in) MCUs per restart interval, 0: none (set to every MCU)                      */
+  int32_t mcux, mcuy, nblk;    /* MCUs per row and column, blocks per MCU                                         */
+  int64_t ws_bytes;            /* workspace offsets: the unstuffed segment (len + 16 bytes),                      */
+  int64_t ws_rst;              /*   the start bit of each restart interval and the end (int64),                   */
+  int64_t ws_coef;             /*   the coefficients, 64 int16 per block in scan order                            */
+  yv6_jpeg_comp comp[3];
+} yv6_jpeg_image;
+enum { YV6_JPEG_OK = 0, YV6_JPEG_SHORT = 1, YV6_JPEG_BAD_CODE = 2, YV6_JPEG_BAD_RUN = 3 };
+/* Host function: lays out the per-call workspace of imgs[0..n) (host records), filling their derived fields; returns its
+ * bytes, or -1 with yv6_last_error set when a record is not one the decoder takes. */
+int64_t yv6_jpeg_workspace_bytes(yv6_jpeg_image* imgs, int32_t n);
+/* Decodes imgs[0..n) (records and tables in DEVICE memory, laid out by yv6_jpeg_workspace_bytes) into their `out` frames.
+ * status[i] (device int32) becomes YV6_JPEG_OK or the first error found in image i's entropy data (its pixels are then
+ * unspecified); nothing is read outside the segments, the tables and the workspace.  The host is never synchronised. */
+int yv6_jpeg_decode(yv6_handle* h, const yv6_jpeg_image* imgs, int32_t n, const yv6_jpeg_huff* huff, void* workspace,
+                    int32_t* status, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -1,5 +1,6 @@
 """Training from frames in GPU memory: a YOLOv6-S TrainStep fed by AugmentFeed from host frames, from CUDA frames uploaded
-once, from JPEGs decoded on the GPU on a side stream (`ready=`), and from a FrameCache, against the same step preloaded.
+once, from JPEGs decoded on the GPU on a side stream (`ready=`) by torchvision's nvJPEG ("decode") and by this project's
+decoder from a JpegStore ("gpujpeg"), and from a FrameCache, against the same step preloaded.
 
     python tools/bench_augment_frames.py [--batch 32] [--size 640] [--steps 10] [--reps 3]
 
@@ -10,7 +11,10 @@ read in the same run:
   - trainstep_ms: median ms per step of each feed and of the preloaded step;
   - submit_cpu_ms: mean host process time per `submit` (and process and wall time per GPU decode call);
   - resize_frames_ms: the first-pass yv6_aug_resize_frames launch of one batch, timed with CUDA events, per feed;
-  - jpeg: the sources' mean JPEG size in MB per frame.
+  - jpeg: the sources' mean JPEG size in MB per frame;
+  - jpeg_decode_ms: this project's decode of one batch's sources from the device store: its device work alone (CUDA
+    events, the stream held until the call has enqueued everything) as ms, images/s, compressed MB/s and output GB/s, and
+    the host time of the call.
 """
 import argparse
 import json
@@ -60,6 +64,7 @@ def main(args):
     from torchvision.io import decode_jpeg, encode_jpeg
 
     from oracle import fabricate as fab
+    from yolov6_b200.jpeg import JpegDecoder, JpegStore
     from yolov6_b200.augment import HYP_YOLOV6S, AugmentFeed, FrameCache, as_source, batch_tables, resize_frames_launch
     from yolov6_b200.loss import ComputeLoss
     from yolov6_b200.model import build_model
@@ -81,14 +86,16 @@ def main(args):
     m.load_state_dict(sd)
     crit = ComputeLoss(num_classes=80, ori_img_size=S, warmup_epoch=0, use_dfl=False, reg_max=0, iou_type="siou")
     step = TrainStep(m.train(), crit, B, S, S, in_dtype=torch.uint8)
-    feeds = {k: AugmentFeed(B, S, S, HYP_YOLOV6S, n, max_src, step=step) for k in ("host", "device", "decode")}
+    feeds = {k: AugmentFeed(B, S, S, HYP_YOLOV6S, n, max_src, step=step) for k in ("host", "device", "decode", "gpujpeg")}
+    store = JpegStore([jpegs[i].numpy().tobytes() for i in range(n)], device=dev)     # every source's JPEG resident on the card
+    gdec = JpegDecoder(dev)
     cache = FrameCache([s.shape[:2] for s in src.values()], feeds["host"].sampler, 4 << 30)
     cache.put(src)
     feeds["cache"] = AugmentFeed(B, S, S, HYP_YOLOV6S, n, max_src, step=step, cache=cache)
     dev_frames = {i: torch.from_numpy(s).to(dev) for i, s in src.items()}
     side = torch.cuda.Stream(dev)
     cpu = {k: [] for k in feeds}
-    decode_cpu = []
+    decode_cpu, gdec_cpu = [], []
 
     def submit(mode, plan):
         feed = feeds[mode]
@@ -99,6 +106,10 @@ def main(args):
             frames = dev_frames
         elif mode == "cache":
             frames = {}
+        elif mode == "gpujpeg":    # yolov6_b200.jpeg from the device store on a side stream
+            c0, w0 = time.process_time(), time.perf_counter()
+            frames, ready = gdec.decode({i: i for i in plan.sources}, stream=side, store=store)
+            gdec_cpu.append(((time.process_time() - c0) * 1e3, (time.perf_counter() - w0) * 1e3, len(plan.sources)))
         else:                      # nvJPEG on a side stream: the step on the current stream keeps running meanwhile
             c0, w0 = time.process_time(), time.perf_counter()
             with torch.cuda.stream(side):
@@ -145,6 +156,39 @@ def main(args):
     for k in cpu:
         cpu[k].clear()
     decode_cpu.clear()
+    gdec_cpu.clear()
+
+    # the GPU decode of one batch's sources alone.  The stream is held behind a sleep kernel while decode() does its host
+    # work (tables, records, staging), so the events bracket the device work only: the H2D copy of the records and the
+    # three kernels.  The host time of the call is reported beside it.
+    srcs = {i: i for i in plan.sources}
+    cbytes = sum(jpegs[i].numel() for i in srcs)
+    obytes = sum(src[i].nbytes for i in srcs)
+    times, call_wall, call_cpu = [], [], []
+    for r in range(args.steps + 2):
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        torch.cuda.synchronize()
+        with torch.cuda.stream(side):
+            torch.cuda._sleep(100_000_000)
+        e0.record(side)
+        c0, w0 = time.process_time(), time.perf_counter()
+        gdec.decode(srcs, stream=side, store=store)
+        w1, c1 = time.perf_counter(), time.process_time()
+        e1.record(side)
+        assert not e0.query(), "the sleep ended before decode() had enqueued its work: the events would include host time"
+        e1.synchronize()
+        if r >= 2:
+            times.append(e0.elapsed_time(e1))
+            call_wall.append((w1 - w0) * 1e3)
+            call_cpu.append((c1 - c0) * 1e3)
+    gdec.check()
+    t = float(np.median(times))
+    print(json.dumps(dict(what="jpeg_decode_ms", images=len(srcs), device_ms=t, device_min_ms=min(times), device_max_ms=max(times),
+                          images_per_s=len(srcs) / (t * 1e-3), compressed_MBps=cbytes / (t * 1e-3) / 1e6,
+                          output_GBps=obytes / (t * 1e-3) / 1e9, compressed_mb=cbytes / 1e6,
+                          call_wall_ms=float(np.median(call_wall)), call_cpu_ms=float(np.mean(call_cpu)),
+                          note="device_ms: CUDA events around the decode's device work alone (record copy + 3 kernels); "
+                               "call_*: host time of the decode() call", card=info)), flush=True)
 
     # step time: preloaded, then each feed, alternating in rounds
     random.seed(1)
@@ -179,6 +223,8 @@ def main(args):
             for k in cpu:
                 cpu[k].clear()
             decode_cpu.clear()
+            gdec_cpu.clear()
+    gdec.check()
     print(json.dumps(dict(what="trainstep_ms", model="yolov6s", batch=B, size=S, steps=args.steps, reps=args.reps,
                           **{k: float(np.median(v)) for k, v in res.items()}, **{f"{k}_min": min(v) for k, v in res.items()},
                           **{f"{k}_max": max(v) for k, v in res.items()}, card=info)), flush=True)
@@ -186,8 +232,10 @@ def main(args):
     print(json.dumps(dict(what="submit_cpu_ms", batch=B, **{k: float(np.mean(v)) for k, v in cpu.items()},
                           calls={k: len(v) for k, v in cpu.items()}, decode_call_cpu=float(dc[:, 0].mean()),
                           decode_call_wall=float(dc[:, 1].mean()), decode_frames_per_call=float(dc[:, 2].mean()),
+                          gpujpeg_call_cpu=float(np.mean([g[0] for g in gdec_cpu])), gpujpeg_call_wall=float(np.mean([g[1] for g in gdec_cpu])),
                           note="process time of all threads, mean over the calls (the clock may tick in 10 ms steps); "
-                               "decode_call_*: torchvision decode_jpeg(device='cuda') of a batch's sources",
+                               "decode_call_*: torchvision decode_jpeg(device='cuda') of a batch's sources; "
+                               "gpujpeg_call_*: yolov6_b200.jpeg's decode of the same sources from the device store",
                           card=info)), flush=True)
 
 

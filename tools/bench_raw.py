@@ -7,6 +7,9 @@ seeded synthetic weights, bench.py's NMS settings), frames/s for several ways of
   jpeg: (--jpeg) raw_input=True -- the same frames encoded once with cv2.imencode; each step decodes its batch on the GPU
         (torchvision.io.decode_jpeg(..., device="cuda"), RGB CHW) and submits the decoder's tensors with layout="rgb_chw",
         so no raw pixel touches the host.  Uniform noise is JPEG's worst case: large files, slow entropy decoding;
+  gpujpeg: (--jpeg) the same JPEG bytes decoded by yolov6_b200.jpeg (cv2.imread's pixels, BGR HWC), staged from the host,
+        and submitted with the decode's `ready` event; its decode of one batch alone is timed as device work (CUDA
+        events) and as host time of the call;
   cv2:  the reference's host path -- data_augment.letterbox (cv2.resize + copyMakeBorder, auto=False) + HWC->CHW + BGR->RGB on
         all host cores into the pinned uint8 batch, then the existing pipeline (rescale not included).
 
@@ -143,6 +146,34 @@ def main():
         jpegs = [[torch.from_numpy(cv2.imencode(".jpg", f)[1].reshape(-1)) for f in fs] for fs in frames]
         jpeg_mb = round(sum(j.numel() for j in jpegs[0]) / B / 1e6, 2)
         feeds["jpeg"] = (raw, lambda i: raw.submit(decode_jpeg(jpegs[i & 1], device=dev), layout="rgb_chw"))
+        from yolov6_b200.jpeg import JpegDecoder
+        gdec = JpegDecoder(dev)
+        jpeg_bytes = [[j.numpy().tobytes() for j in js] for js in jpegs]
+
+        def feed_gpujpeg(i):
+            frames, ready = gdec.decode(dict(enumerate(jpeg_bytes[i & 1])))
+            raw.submit([frames[j] for j in range(B)], ready=ready)
+        feeds["gpujpeg"] = (raw, feed_gpujpeg)
+
+        def gpujpeg_ms(n=5):
+            """This project's decode of one batch from host bytes: (device ms, call ms).  The device work alone (H2D of
+            the staged bytes + the kernels) between CUDA events, the stream held behind a sleep kernel until the call has
+            enqueued it; and the host wall time of the call."""
+            times, calls = [], []
+            for i in range(n + 1):
+                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                torch.cuda.synchronize()
+                torch.cuda._sleep(1_000_000_000)
+                e0.record()
+                w0 = time.perf_counter()
+                gdec.decode(dict(enumerate(jpeg_bytes[i & 1])))
+                calls.append((time.perf_counter() - w0) * 1e3)
+                e1.record()
+                assert not e0.query(), "the sleep ended before decode() had enqueued its work"
+                e1.synchronize()
+                times.append(e0.elapsed_time(e1))
+            gdec.check()
+            return round(float(np.median(times[1:])), 2), round(float(np.median(calls[1:])), 2)
 
         def decode_ms(n=5):
             """The decode of one batch alone: host clock around decode_jpeg + a device synchronise."""
@@ -162,7 +193,8 @@ def main():
                 "cv2_host_frames_per_s": fps["cv2"], "dev_frames_per_s": fps["dev"], "letterbox_frames_kernel": kernel,
                 "host_threads": threads, "steps": args.steps, "run": r, "gpu": gpu_info(0)}
         if args.jpeg:
-            line.update(jpeg_frames_per_s=fps["jpeg"], jpeg_mb_per_frame=jpeg_mb, jpeg_decode_ms_per_batch=decode_ms())
+            line.update(jpeg_frames_per_s=fps["jpeg"], jpeg_mb_per_frame=jpeg_mb, jpeg_decode_ms_per_batch=decode_ms(),
+                        gpujpeg_frames_per_s=fps["gpujpeg"], gpujpeg_decode_ms_per_batch=dict(zip(("device", "call"), gpujpeg_ms())))
         print(json.dumps(line), flush=True)
 
 

@@ -189,6 +189,26 @@ class LbSrc(C.Structure):
     ]
 
 
+class JpegHuff(C.Structure):
+    """Mirror of `yv6_jpeg_huff` (include/yv6.h): one Huffman table in the decoder's form."""
+    _fields_ = [("lut", C.c_uint16 * 512), ("maxcode", C.c_int32 * 18), ("valoff", C.c_int32 * 18), ("vals", C.c_uint8 * 256)]
+
+
+class JpegComp(C.Structure):
+    """Mirror of `yv6_jpeg_comp` (include/yv6.h)."""
+    _fields_ = [("h", C.c_int32), ("v", C.c_int32), ("dc", C.c_int32), ("ac", C.c_int32), ("bw", C.c_int32), ("bh", C.c_int32),
+                ("dw", C.c_int32), ("dh", C.c_int32), ("plane", C.c_int64), ("q", C.c_uint16 * 64)]
+
+
+class JpegImage(C.Structure):
+    """Mirror of `yv6_jpeg_image` (include/yv6.h): one image of a yv6_jpeg_decode call."""
+    _fields_ = [
+        ("data", C.c_void_p), ("len", C.c_int64), ("out", C.c_void_p), ("height", C.c_int32), ("width", C.c_int32),
+        ("ncomp", C.c_int32), ("orientation", C.c_int32), ("restart", C.c_int32), ("mcux", C.c_int32), ("mcuy", C.c_int32),
+        ("nblk", C.c_int32), ("ws_bytes", C.c_int64), ("ws_rst", C.c_int64), ("ws_coef", C.c_int64), ("comp", JpegComp * 3),
+    ]
+
+
 LB_BGR_HWC, LB_RGB_CHW = 0, 1
 VAL_COPY, VAL_LINEAR, VAL_AREA, VAL_AREA_FAST = 0, 1, 2, 3      # yv6_letterbox_val's per-image modes (geo[7])
 XF_F32, XF_F64, XF_BF16 = 0, 1, 2
@@ -300,6 +320,8 @@ _SIGNATURES = {
                                       C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_void_p]),
     "yv6_upsample2x": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
                                  C.c_int64, C.c_int64, C.c_int32, C.c_void_p]),
+    "yv6_jpeg_workspace_bytes": (C.c_int64, [C.c_void_p, C.c_int32]),
+    "yv6_jpeg_decode": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "yv6_nms_workspace_bytes": (C.c_int64, [C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
     "yv6_nms_batched": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_float, C.c_double,
                                   C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,

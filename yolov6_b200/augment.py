@@ -17,8 +17,9 @@ The reference builds every training sample on the host in `TrainValDataset.__get
 `AugmentFeed` ties them to a `TrainStep`: it stages the sources of batch i+1 in pinned memory, copies and resizes them on
 side streams while batch i's graphs run, and writes the augmented images straight into the step's static uint8 input,
 ordered by events rather than host synchronisation.  Frames may also be CUDA tensors (a GPU decoder's output, read in
-place), and `FrameCache` is the reference's --cache-ram in device memory.  Decoding (JPEG / PNG -> pixels) stays with the
-caller.
+place), and `FrameCache` is the reference's --cache-ram in device memory.  JPEGs are decoded on the device, with
+cv2.imread's pixels, by `jpeg.JpegDecoder` (its frames and `ready` event go straight into `submit` or `FrameCache.put`);
+other formats, and the JPEG kinds it refuses, are decoded by the caller.
 
 Off the square: `Sampler(..., target="specific")` is `--specific-shape` (every sample on one H x W, load_image at
 min(W / w0, H / h0)); `target="rect"` with `rect_batches` is `--rect` (each batch on its own aspect-ratio canvas, which

@@ -12,8 +12,9 @@ Both of the reference's padding modes are provided.  auto=False pads every image
 and a fixed-shape server's choice).  auto=True is Inferer's own default: the image is padded only up to the next multiple
 of the stride, so a 1920 x 1080 frame at img_size 640 reaches the network as a 384 x 640 canvas.  Each source shape then
 has its own canvas (`rect_canvas`); a batch takes one canvas, so frames whose canvases differ are refused before anything
-is staged, and a caller serving mixed sources keeps one batch per canvas.  Decoding (JPEG / PNG -> pixels) stays with the
-caller.
+is staged, and a caller serving mixed sources keeps one batch per canvas.  JPEGs are decoded on the device, with
+cv2.imread's pixels, by `jpeg.JpegDecoder`, whose frames and `ready` event go straight into `DetectStream.submit`; other
+formats, and the JPEG kinds it refuses, are decoded by the caller.
 """
 import ctypes as C
 import math
