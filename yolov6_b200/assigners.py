@@ -48,9 +48,11 @@ def _workspace(dev, nbytes):
 
 
 def tal_compact(pd_scores, pd_bboxes, anc_points, gt, mask_gt, topk=13, alpha=1.0, beta=6.0, eps=1e-9, stream=None):
+    B, A, nc = pd_scores.shape
+    if A < topk:      # the reference's torch.topk over the anchors raises here (tal_assigner.py:141); the kernel would pad with -1
+        raise ValueError(f"TAL: top-{topk} candidates of a map with {A} anchors: the map needs at least {topk} anchors")
     _lib.require_cuda(pd_scores, "yolov6_b200 assigners run")
     dev = pd_scores.device
-    B, A, nc = pd_scores.shape
     G = gt.shape[1]
     out = _Compact()
     out.gt, out.B, out.A, out.G, out.nc = gt, B, A, G, nc

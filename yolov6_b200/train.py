@@ -572,8 +572,11 @@ class TrainEngine:
         key = (N, H, W, in_dtype)
         if self._shape == key and (x_static is None or x_static is self.x_static):
             return
-        self._shape = key
         g, dev = self.g, self.dev
+        maxs = max(g.strides)
+        if H % maxs or W % maxs or H <= 0 or W <= 0:      # as InferEngine._plan: every level's map must halve the previous one
+            raise RuntimeError(f"input {H}x{W} must be a multiple of the largest stride {maxs}")
+        self._shape = key
         if self.arena is not None:
             self.arena.off = 0
         self.bufs = [self._new((N, H >> b.level, W >> b.level, b.c_total)) for b in g.bufs]
